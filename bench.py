@@ -51,11 +51,30 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sustained=d["bf16_tflops_sustained"], source="measured")
-    return dict(hbm_gbs=6650.0, tf_burst=1590.0, tf_sustained=1400.0, source="fallback")
+    # NVIDIA H100 SXM data sheet (700 W card): HBM3 3.35 TB/s, dense bf16 989 TFLOP/s; never reached, only an upper bound
+    return dict(hbm_gbs=3350.0, tf_burst=989.0, tf_sustained=989.0, source="H100 SXM data sheet")
+
+
+def dump_outputs(out_dir, tr, torch, sample=1 << 20):
+    """Writes what the last timed step computed, as float32 .npy files under out_dir: the loss and correct count, the
+    logits, and the same fixed, seeded sample (at most `sample` elements each, under 13 MB in all) of the updated fp32 weights,
+    their gradients and the BatchNorm running statistics - so that two builds can be compared output for output."""
+    import numpy as np
+    e = tr.engine
+    torch.cuda.synchronize()
+    arrays = dict(loss=e.scalars[0:1], correct=e.scalars[1:2], logits=e.logits)
+    g = torch.Generator().manual_seed(0)
+    for name, t in (("params", e.params32), ("grads", e.grads32), ("bn_buffers", e.buffers32)):
+        if t.numel() > sample:
+            t = t[torch.randperm(t.numel(), generator=g)[:sample].sort().values.to(t.device)]
+        arrays[name] = t
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clock / throttle sampling DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clock / throttle sampling DURING the timed region."""
 
     def __init__(self, gpu_index):
         super().__init__(daemon=True)
@@ -280,6 +299,8 @@ def run_native(args):
     ms = t0.elapsed_time(t1)
     loss_final = float(e.loss)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, tr, torch)
     if world > 1:
         t = torch.tensor([ms], device="cuda")
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -324,22 +345,10 @@ def run_native(args):
     top = max(fam.items(), key=lambda kv: kv[1]["ms"])
     top_name, tf = top
     ach = tf["bytes"] / (tf["ms"] / 1e3) / 1e9 if tf["ms"] > 0 else 0.0
-    # measured DRAM bytes per launch of that kernel (dram__bytes_read.sum + dram__bytes_write.sum of the committed ncu
-    # launch list, same workload: profiles/r01_ncu_launches.md), valid for the default workload only
-    traffic, traffic_src = None, None
-    tpath = os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")
-    if os.path.exists(tpath) and arch == "efficientnet_b0" and B == 256 and args.dtype == "bf16":
-        try:
-            with open(tpath) as f:
-                tj = json.load(f)
-            ent = tj.get(top_name[len("dfd_"):] + "_kernel")
-            if ent and ent["launches"] == tf["launches"]:
-                traffic, traffic_src = ent["dram_bytes_per_launch"], "profiles/r02_ncu_traffic.json (ncu capture of this build, see its 'build' field)"
-        except Exception:  # noqa: BLE001
-            pass
     if w["bound"] == "tensor":
-        # dense-conv models (SURVEY.md 8d): the dominant family is the tcgen05 GEMM; achieved = its algorithmic FLOPs / its time,
-        # against the SUSTAINED bf16 matmul rate of MEASURED_PEAKS.json (the kernel runs inside a long step)
+        # dense-conv models (SURVEY.md 8d): the dominant family is the tensor-core GEMM; achieved = its algorithmic FLOPs / its
+        # time, against the SUSTAINED bf16 matmul rate of MEASURED_PEAKS.json (the kernel runs inside a long step); without that
+        # file both the sustained and the burst rate are the 989 TFLOP/s dense bf16 figure of the H100 SXM data sheet
         top_name = max((k for k in fam if fam[k]["flops"]), key=lambda k: fam[k]["ms"])
         tf = fam[top_name]
         ach = tf["flops"] / (tf["ms"] / 1e3) / 1e12 if tf["ms"] > 0 else 0.0
@@ -355,7 +364,7 @@ def run_native(args):
                                   for k, v in sorted(fam.items(), key=lambda kv: -kv[1]["ms"])[:8]})
     else:
       roofline = dict(bound="hbm", kernel=top_name, achieved=round(ach, 1), peak=peaks["hbm_gbs"], unit="GB/s",
-                    frac=round(ach / peaks["hbm_gbs"], 4), traffic=traffic, traffic_source=traffic_src,
+                    frac=round(ach / peaks["hbm_gbs"], 4),
                     algorithmic_bytes_per_launch=int(tf["bytes"] / max(tf["launches"], 1)), peak_source=peaks["source"],
                     kernel_share_of_step=round(tf["ms"] / tot_ms, 4), launches=tf["launches"],
                     step_frac_of_ideal_fusion_roofline=round(img_s / world * w["act_mb"] * 1e6 / (peaks["hbm_gbs"] * 1e9), 4),
@@ -370,7 +379,7 @@ def run_native(args):
                 config=dict(workload="%s %s train step, synthetic 3x%dx%d, per-GPU batch %d (%s%s)" % (
                     arch, args.dtype, res, res, B, BASELINE_CFG.get((arch, B, args.dtype), "not a BASELINE.json configuration"),
                     "; DDP weak scaling" if world > 1 else ""), global_batch=B * world,
-                    optimizer=args.opt, l2_policy="working set (activations ~6 GB/step) far exceeds the 126 MB L2",
+                    optimizer=args.opt, l2_policy="working set (activations ~6 GB/step) far exceeds the 50 MB L2",
                     cuda_graph=tr._graph is not None, gemm=args.gemm, loss_final=loss_final),
                 roofline=roofline, cpu_baseline=cpu,
                 e2e=dict(value=round(e2e_img_s, 1), unit="images/sec",
@@ -480,7 +489,7 @@ def cpu_ddp_baseline(arch, world, threads_total, steps=3):
 
 
 def run_library(args):
-    """Stock PyTorch eager on the same B200: the reference's module graph as torch.nn modules (baseline/library_model.py),
+    """Stock PyTorch eager on the same GPU: the reference's module graph as torch.nn modules (baseline/library_model.py),
     autocast to the benchmark dtype, channels_last, SGD-nesterov, torch DDP over NCCL when launched under torchrun.
     No kernel, plan or engine of this repository is on this path."""
     import torch
@@ -621,7 +630,11 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--cpu-steps", type=int, default=4)
     ap.add_argument("--cpu-world", type=int, default=1, help="--impl reference: also time N gloo ranks on the host cores")
+    ap.add_argument("--dump-outputs", metavar="DIR", default="",
+                    help="native arm only: write what the last timed step computed to DIR/<name>.npy (float32, seeded sample)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "native":
+        ap.error("--dump-outputs writes the outputs of the native arm only (got --impl %s)" % args.impl)
     if args.impl == "reference":
         run_reference(args)
     elif args.impl == "library":

@@ -1,4 +1,4 @@
-"""ctypes binding of libdfd_b200.so (the C-ABI of the sm_100a kernels, see include/dfd_b200.h).
+"""ctypes binding of libdfd_b200.so (the C-ABI of the sm_90a kernels, see include/dfd_b200.h).
 
 There is NO fallback: if the shared library is missing or a symbol is absent, importing / calling raises.
 The library is built in-tree by `__graft_entry__.build()` (csrc/Makefile) so that it travels to the GPU box.

@@ -186,7 +186,7 @@ def get_spec(arch, num_classes=2, in_chans=3):
         return _resnet_spec(arch, "basic", (2, 2, 2, 2), in_chans, num_classes, (3, 224, 224))
     if arch == "resnet50":
         return _resnet_spec(arch, "bottleneck", (3, 4, 6, 3), in_chans, num_classes, (3, 224, 224))
-    raise ValueError("arch %r is not on the B200 hot path (see SURVEY.md section 8)" % (arch,))
+    raise ValueError("arch %r is not on the native hot path (see SURVEY.md section 8)" % (arch,))
 
 
 SUPPORTED_ARCHS = ("efficientnet_b0", "efficientnet_b4", "efficientnet_deepfake_v4", "resnet18", "resnet50")

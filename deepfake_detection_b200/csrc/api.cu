@@ -32,7 +32,7 @@ int dfd_memset_async(void* p, int value, long long bytes, void* stream) {
 }  // extern "C"
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Order-deterministic reduction of split partial sums (the second half of the tcgen05 weight gradient and of the fused
+// Order-deterministic reduction of split partial sums (the second half of the wgmma weight gradient and of the fused
 // depthwise backward in workspace mode): for every table entry  dst[i] += sum_{p = 0 .. parts-1} src[p * stride + i],  i < n,
 // the partials added in index order - whatever order the producing CTAs finished in.  One launch serves every entry
 // (blockIdx.y); entries with many parts spread them over 32 part-lanes whose sums meet in a fixed order too.

@@ -62,19 +62,18 @@ struct RowGeom {
     int rows_per_block;
 };
 
-// hw rows per image, n images; target enough CTAs to fill 148 SMs a few times over
+// hw rows per image, n images; target enough CTAs to fill every SM a few times over
 // max_threads: CTA size (256 by default) - target_blocks is scaled so that the resident thread count stays the same.
-// MEASURED (B0 shapes, batch 256, L2 flushed): 512-thread CTAs help the two per-image reductions on the large layers
-// (dfd_se_bwd_reduce 110 -> 93 us at 112x112x32, 124 -> 107 us at 56x56x144; dfd_pool 69 -> 59, 77 -> 68 us: half as many
-// cross-row reductions and tickets per image), change nothing below 28x28 and HURT dfd_bn_act (85 -> 99 us: no reduction
-// to amortise, coarser tail). DFD_ROW_MAXT forces a value for every user (diagnostic).
+// 512-thread CTAs helped the two per-image reductions on the large layers (half as many cross-row reductions and tickets
+// per image), changed nothing below 28x28 and slowed dfd_bn_act (no reduction to amortise, coarser tail) - on the GPU this code was first tuned on (not re-measured on the H100).
+// DFD_ROW_MAXT forces a value for every user (diagnostic).
 static int row_maxt(long long hw, bool reduces_per_image) {
     static int v = -1;
     if (v < 0) { const char* e = getenv("DFD_ROW_MAXT"); v = e ? atoi(e) : 0; if (v != 256 && v != 512 && v != 1024) v = 0; }
     if (v) return v;
     return reduces_per_image && hw >= 784 ? 512 : 256;
 }
-static RowGeom make_geom(int C, long long hw, int n, int target_blocks = 148 * 6, int max_threads = 256) {
+static RowGeom make_geom(int C, long long hw, int n, int target_blocks = DFD_SMS * 6, int max_threads = 256) {
     RowGeom g;
     int V = C / 8;
     int RY = V >= max_threads ? 1 : (max_threads / V);
@@ -199,7 +198,7 @@ __global__ void bn_act_kernel(const T* __restrict__ y, const float* __restrict__
     if (r1 > hw) r1 = hw;
     const size_t img = (size_t)blockIdx.y * hw * C + c0;
     // U rows per trip, all loads issued before any math: a thread with one 16-byte load in flight cannot keep HBM
-    // busy at the occupancy these register counts allow (Little: ~44 KB in flight per SM for 6.5 TB/s)
+    // busy at the occupancy these register counts allow (Little's law: tens of KB must be in flight per SM to sustain its share of the HBM rate)
     constexpr int U = RES ? 2 : 4;
     for (long long r = r0 + threadIdx.y; r < r1; r += (long long)U * blockDim.y) {
         uint4 raw[U], rraw[U];
@@ -682,7 +681,7 @@ int dfd_bn_act(const void* y, const float* scale, const float* shift, const floa
                int n, long long hw, int C, int act, int res_mode, int dt, void* stream) {
     if (C % 8 || C <= 0 || hw <= 0 || n <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_bn_act: C%8, sizes");
     if ((res_mode != 0) != (res != nullptr)) return dfd_set_error(DFD_ERR_ARG, "dfd_bn_act: res/res_mode");
-    RowGeom g = make_geom(C, hw, n, 148 * 6, row_maxt(hw, false));
+    RowGeom g = make_geom(C, hw, n, DFD_SMS * 6, row_maxt(hw, false));
     cudaStream_t st = (cudaStream_t)stream;
 #define LAUNCH(ACT, GATE, RES)                                                                                    \
     bn_act_kernel<T, ACT, GATE, RES><<<g.grid, g.block, 0, st>>>((const T*)y, scale, shift, gate, (const T*)res, \
@@ -754,7 +753,7 @@ int dfd_pool_se(const void* y, const float* scale, const float* shift, float* po
 int dfd_bn_bwd_reduce(const void* g_, const void* y, const void* out, const float* mean, const float* rstd, int n,
                       long long hw, int C, int dt, double* s1, double* s2, const void* fin, void* stream) {
     if (C % 8 || C <= 0 || hw <= 0 || n <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_bn_bwd_reduce: C%8, sizes");
-    RowGeom g = make_geom(C, hw, n, 148 * 6, row_maxt(hw, false));
+    RowGeom g = make_geom(C, hw, n, DFD_SMS * 6, row_maxt(hw, false));
     cudaStream_t st = (cudaStream_t)stream;
     DISPATCH_T(dt, {
         if (out) bn_bwd_reduce_kernel<T, true><<<g.grid, g.block, reduce_smem(g), st>>>((const T*)g_, (const T*)y, (const T*)out, mean, rstd, hw, g.rows_per_block, s1, s2, (const BnBwdFinDesc*)fin);
@@ -782,7 +781,7 @@ int dfd_relu_bn_bwd_reduce(const void* g_, const void* g2, const void* y, const 
                            const float* rstd, int n, long long hw, int C, int dt, double* s1, double* s2, void* stream) {
     if (C % 8 || C <= 0 || hw <= 0 || n <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_relu_bn_bwd_reduce: C%8, sizes");
     if (!out || !gm) return dfd_set_error(DFD_ERR_ARG, "dfd_relu_bn_bwd_reduce: operands");
-    RowGeom g = make_geom(C, hw, n, 148 * 6, row_maxt(hw, false));
+    RowGeom g = make_geom(C, hw, n, DFD_SMS * 6, row_maxt(hw, false));
     cudaStream_t st = (cudaStream_t)stream;
     DISPATCH_T(dt, (bn_bwd_reduce_kernel<T, true><<<g.grid, g.block, reduce_smem(g), st>>>((const T*)g_, (const T*)y, (const T*)out, mean, rstd,
                                                                                            hw, g.rows_per_block, s1, s2, nullptr, (T*)gm, (const T*)g2)));
@@ -861,8 +860,8 @@ int dfd_act_bwd(const void* da, const void* y, const float* scale, const float* 
     static int occ3 = -1;
     if (occ3 < 0) { const char* e = getenv("DFD_ACTBWD_OCC3"); occ3 = e ? atoi(e) : 0; }
     // variant: 0 = 256 threads x 2 CTAs per SM with 6 loads in flight per thread (default), 1 = 256 x 3 with 4 loads in flight
-    // (DFD_ACTBWD_OCC3, diagnostic: MEASURED slower on the large layers, 142 -> 148 us at 112x112x32, 114 -> 131 us at 56x56x96,
-    // and only 10 % faster at 7x7), 2 = more than 2048 channels (one row of C / 8 threads)
+    // (DFD_ACTBWD_OCC3, diagnostic: slower on the large layers and barely faster at 7x7 on the GPU this code was first tuned on (not re-measured on the H100)),
+    // 2 = more than 2048 channels (one row of C / 8 threads)
     const int var = g.block.x * g.block.y > 256 ? 2 : (occ3 ? 1 : 0);
 #define ABARGS (const T*)da, (const T*)y, scale, shift, mean, rstd, gate, dpool, inv_hw, (T*)gu, hw, g.rows_per_block, s1, s2, (const BnBwdFinDesc*)fin
 #define LAUNCH(ACT, HAS) do {                                                                                       \
@@ -891,7 +890,7 @@ int dfd_add_inplace(void* a, const void* b, long long numel, int dt, void* strea
     if (numel % 8) return dfd_set_error(DFD_ERR_ARG, "dfd_add_inplace: numel%8");
     size_t nvec = (size_t)(numel / 8);
     int blocks = (int)((nvec + 255) / 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > DFD_SMS * 16) blocks = DFD_SMS * 16;
     cudaStream_t st = (cudaStream_t)stream;
     DISPATCH_T(dt, (add_inplace_kernel<T><<<blocks, 256, 0, st>>>((T*)a, (const T*)b, nvec)));
     DFD_LAUNCH_CHECK();

@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a kernels of the dfd train/validate hot path.
+// Shared device helpers for the sm_90a kernels of the dfd train/validate hot path.
 // Activations are NHWC in a 16-bit type T (bf16 or fp16); all arithmetic is fp32; per-channel
 // statistics are accumulated in fp64 in HBM (one atomic per channel per CTA).
 #pragma once
@@ -87,7 +87,7 @@ __device__ __forceinline__ void stg16(void* p, const uint4& v) { *reinterpret_ca
 
 // ------------------------------------------------------------------------------------------
 // activations. sigmoid via one MUFU op: sigma(x) = 0.5 * tanh(0.5 x) + 0.5
-// (B200 has 16 MUFU lanes/clk/SM; exp+rcp would make every swish pass MUFU-bound before HBM-bound)
+// (an SM has 16 MUFU lanes per clock; exp+rcp would make every swish pass MUFU-bound before HBM-bound)
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ float fast_tanh(float x) {
     float y;
@@ -137,3 +137,7 @@ __device__ __forceinline__ double stat_total(const double* base, int C, int c) {
 }
 
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
+
+// SM count of the target GPU (H100 SXM). Grid shapes are sized with it; it also fixes the split counts of the
+// order-deterministic weight-gradient reductions, so those results do not depend on the device the library runs on.
+#define DFD_SMS 132

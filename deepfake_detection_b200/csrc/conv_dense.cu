@@ -1,10 +1,10 @@
-// ResNet-side kernels: dense k x k convolution as (im2col -> tcgen05 GEMM), its backward (GEMM -> col2im, GEMM wgrad
+// ResNet-side kernels: dense k x k convolution as (im2col -> tensor-core GEMM), its backward (GEMM -> col2im, GEMM wgrad
 // on the im2col matrix), weight / gradient layout changes between OIHW and the GEMM's [Cout][kh][kw][Cin], 3x3/s2
 // max-pool forward/backward, ReLU-mask and global-average-pool backward.
 //   ResNet.forward            dfd/timm/models/resnet.py:450-468 (conv1 7x7 -> bn -> relu -> maxpool 3x3 s2 p1 :379-382)
 //   BasicBlock / Bottleneck   resnet.py:150-175, :215-246 (3x3 convs :129-136,:195-197; downsample 1x1 s2 :249-260)
 // Round-1 scope note: the 3x3 convolutions go through a MATERIALISED im2col matrix (9x the activation bytes). It is
-// correct and runs on the tcgen05 GEMM, but it is not the final design: the implicit-GEMM kernel with TMA im2col
+// correct and runs on the tensor-core GEMM, but it is not the final design: the implicit-GEMM kernel with TMA im2col
 // descriptors replaces im2col/col2im next (DESIGN.md section 6).
 #include "common.cuh"
 
@@ -81,8 +81,7 @@ struct RepackDesc {
 };
 // weights: OIHW 16-bit -> [O][kh][kw][I] (GEMM B operand), its transpose [(kh,kw,I)][O] and the tap-flipped [I][kh'][kw'][O].
 // One pass per destination layout, each walking ITS OWN element order so that the 2-byte stores of a warp are contiguous
-// (a single pass in dst order scattered the other two layouts with a stride of O elements: 0.52 ms per step for ResNet-50's
-// 11 M weights); the strided source reads of the later passes hit L2.
+// (a single pass in dst order scattered the other two layouts with a stride of O elements); the strided source reads of the later passes hit L2.
 template <typename T>
 __global__ void repack_weights_kernel(const RepackDesc* __restrict__ table) {
     RepackDesc d = table[blockIdx.y];
@@ -245,7 +244,7 @@ __global__ void pool_bwd_kernel(const float* __restrict__ dpooled, T* __restrict
 
 // ---- stem as a GEMM: im2col of the NCHW image in (ci, kh, kw) column order (== OIHW flattening), K padded to a multiple of 8.
 // One CTA per output row: the Cin x k input rows it needs are staged (zero-padded) in shared memory with coalesced reads,
-// then every thread assembles 16-byte column groups from it (a per-thread 2-byte gather from global ran at 0.6 TB/s).
+// then every thread assembles 16-byte column groups from it (a per-thread 2-byte gather from global is request-bound).
 template <typename T>
 __global__ void stem_im2col_kernel(const T* __restrict__ x, T* __restrict__ cols, int N, int Cin, int H, int W, int k, int s,
                                    int pad, int Ho, int Wo, int Kp) {
@@ -302,7 +301,7 @@ __global__ void unpad_grad_kernel(const float* __restrict__ gp, float* __restric
 
 static int nblocks(long long total) {
     long long b = (total + 255) / 256;
-    if (b > 148 * 32) b = 148 * 32;
+    if (b > DFD_SMS * 32) b = DFD_SMS * 32;
     if (b < 1) b = 1;
     return (int)b;
 }
@@ -338,7 +337,7 @@ int dfd_col2im(const void* dcols, const void* add, void* dx, int N, int H, int W
 // table: device array of { const void* src; void* dst; void* dstT; void* dstD; int O, I, k; int pad_; }
 int dfd_repack_weights(const void* table, int count, int dt, void* stream) {
     if (count <= 0) return DFD_OK;
-    dim3 grid(148 * 8, count);       // latency-bound gather: many short grid-stride loops
+    dim3 grid(DFD_SMS * 8, count);       // latency-bound gather: many short grid-stride loops
     CD_T(dt, (repack_weights_kernel<T><<<grid, 256, 0, (cudaStream_t)stream>>>((const RepackDesc*)table)));
     DFD_LAUNCH_CHECK();
     return DFD_OK;

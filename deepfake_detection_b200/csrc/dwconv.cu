@@ -3,7 +3,7 @@
 // dfd/timm/models/layers/create_conv2d.py:11-30 at dfd/timm/models/efficientnet_blocks.py:152-153,283-285
 // with symmetric padding (k-1)//2 (layers/padding.py:12-14).
 //
-// Design (B200): these layers are HBM-bound with k*k-fold reuse of every input element, and the preceding
+// Design: these layers are HBM-bound with k*k-fold reuse of every input element, and the preceding
 // BN + Swish is fused into the load, so:
 //   * a CTA stages an input tile (+halo) for 64 channels in shared memory ONCE, applying BN scale/shift and the
 //     activation exactly once per element (sigmoid = one MUFU tanh), stored as packed 16-bit pairs;
@@ -636,8 +636,9 @@ dwconv_bwd_kernel(const T* __restrict__ gy, const T* __restrict__ yout, const fl
         };
         if (warp < nstrips) prefetch(warp);
         __syncthreads();    // previous image's tile fully consumed
-        // staging batch (16-byte loads in flight per thread and tensor): 4 for k = 5 (two CTAs per SM either way, measured
-        // -8 %), 2 for k = 3 where the deeper batch costs the third resident CTA (measured +3..16 %)
+        // staging batch (16-byte loads in flight per thread and tensor): 4 for k = 5 (two CTAs per SM either way), 2 for k = 3
+        // where the deeper batch costs the third resident CTA; both chosen on the GPU this code was first tuned on, not
+        // re-measured on the H100
         if (!(g.dbg & 2))
             stage_grad_tile<T, AFFINE, (K == 5 ? 4 : 2), CPW>(tile, gy + ooff, AFFINE ? yout + ooff : nullptr, g.Ho, g.Wo, g.C, c0,
                                    S == 1 ? y0 - pp : (y0 >> 1) - 1, S == 1 ? x0 - pp : (x0 >> 1) - 1, g.IH, g.IW, cA, cB, cC);
@@ -763,9 +764,9 @@ dwconv_bwd_kernel(const T* __restrict__ gy, const T* __restrict__ yout, const fl
 }
 
 // channel pairs per sub-strip of the hot kernels for a layer of C channels (see the lane mapping note at the top): 32 unless
-// the last 64-channel block would idle a fifth or more of the lanes; then 16 (C = 32, 96, 144: measured best, also where 8
-// would waste nothing - 56x56x144: backward 0.618 / 0.479 / 0.511 ms, forward 0.254 / 0.254 / 0.281 ms for 32 / 16 / 8), and
-// 8 only where 16 would still idle a fifth (C = 16, 48). DFD_DW_CPW forces a value (diagnostics).
+// the last 64-channel block would idle a fifth or more of the lanes; then 16 (C = 32, 96, 144: best on the GPU this code
+// was first tuned on, not re-measured on the H100; also where 8 would waste nothing), and 8 only where 16 would still idle
+// a fifth (C = 16, 48). DFD_DW_CPW forces a value (diagnostics).
 static int dw_cpw(int C) {
     static int forced = -1;
     if (forced < 0) { const char* e = getenv("DFD_DW_CPW"); forced = e ? atoi(e) : 0; }
@@ -864,8 +865,8 @@ int dfd_dwconv_fwd(const void* x, const float* scale, const float* shift, const 
     DwGeom g;
     const int cpw = dw_cpw(C);
     int smem = fill_geom(g, N, H, W, C, k, stride, false, cpw);
-    // one CTA per (tile, 2*cpw channels, image): walking several images per CTA (as the fused backward does) measured 25 % slower
-    // here - the forward has no per-CTA state worth amortising and loses the overlap between resident CTAs
+    // one CTA per (tile, 2*cpw channels, image): walking several images per CTA (as the fused backward does) was slower
+    // here on the GPU this code was first tuned on (not re-measured on the H100) - the forward has no per-CTA state worth amortising and loses the overlap between resident CTAs
     dim3 grid(g.tiles_x * g.tiles_y, (C + 2 * cpw - 1) / (2 * cpw), N);
     cudaStream_t st = (cudaStream_t)stream;
 #define FW(ACT_, AFF_, CPW_) DW_LAUNCH((dwconv_fwd_kernel<T, K, S, ACT_, AFF_, NT, CPW_>), grid, smem, st, (const T*)x, scale, shift, w, (T*)out, dsum, dsq, (const BnFinDesc*)fin, g)
@@ -912,7 +913,7 @@ int dfd_dwconv_wgrad(const void* x, const float* scale, const float* shift, cons
     DwGeom g;
     int smem = fill_geom(g, N, H, W, C, k, stride, false);
     int tiles = g.tiles_x * g.tiles_y, cbs = (C + CB - 1) / CB;
-    int gz = (148 * 6 + tiles * cbs - 1) / (tiles * cbs);
+    int gz = (DFD_SMS * 6 + tiles * cbs - 1) / (tiles * cbs);
     if (gz > N) gz = N;
     if (gz < 1) gz = 1;
     dim3 grid(tiles, cbs, gz);
@@ -935,7 +936,7 @@ int dfd_dwconv_wgrad(const void* x, const float* scale, const float* shift, cons
 static void dw_bwd_grid(const DwGeom& g, int N, int C, int cpw, int& tiles, int& cbs, int& gz) {
     tiles = g.tiles_x * g.tiles_y;
     cbs = (C + 2 * cpw - 1) / (2 * cpw);
-    gz = (148 * 6 + tiles * cbs - 1) / (tiles * cbs);
+    gz = (DFD_SMS * 6 + tiles * cbs - 1) / (tiles * cbs);
     if (gz > N) gz = N;
     while (gz < N && N % gz) gz++;
 }
@@ -976,7 +977,9 @@ int dfd_dwconv_bwd(const void* gy, const void* yout, const float* cA, const floa
     }
     dim3 grid(tiles, cbs, gz);
     cudaStream_t st = (cudaStream_t)stream;
-    static int pb3 = 0, pb5 = 0;       // strip width per kernel size: 4 for k = 3 (four CTAs per SM, measured -1..-14 %), 8 for k = 5 (4 measured slower); DFD_DW_PB3 / DFD_DW_PB5 override
+    // strip width per kernel size: 4 for k = 3 (four CTAs per SM), 8 for k = 5, chosen on the GPU this code was first tuned
+    // on (not re-measured on the H100); DFD_DW_PB3 / DFD_DW_PB5 override
+    static int pb3 = 0, pb5 = 0;
     if (!pb3) { const char* e3 = getenv("DFD_DW_PB3"); const char* e5 = getenv("DFD_DW_PB5"); pb3 = (e3 && atoi(e3) == 8) ? 8 : 4; pb5 = (e5 && atoi(e5) == 4) ? 4 : 8; }
     const int pb = k == 3 ? pb3 : pb5;
 #define BWARGS (const T*)gy, (const T*)yout, cA, cB, cC, w, (const T*)xin, scale, shift, mean, rstd, (const T*)add, (T*)gx, dW, s1, s2, (const BnBwdFinDesc*)fin, g

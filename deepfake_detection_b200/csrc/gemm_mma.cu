@@ -5,7 +5,7 @@
 //   gemm_wgrad: dW[Nw,Kw] += G[M,Nw]^T * X[M,Kw]   (contraction over the M = N*H*W rows; split over M)
 //
 // This file is the bring-up / cross-check implementation and the weight-gradient path of round 1; the
-// forward/dgrad product path is the tcgen05 + TMA kernel in gemm_tc.cu.
+// forward/dgrad product path is the wgmma + TMA kernel in gemm_tc.cu.
 // Reference ops replaced: nn.Conv2d 1x1 at dfd/timm/models/efficientnet_blocks.py:165,277,299 and
 // efficientnet.py:292, ResNet 1x1 at resnet.py:192,199, and their autograd backward (train.py:634-636).
 #include "common.cuh"
@@ -317,7 +317,7 @@ int dfd_gemm_wgrad_mma(const void* G, const void* X, float* dW, long long M, int
     if (M <= 0 || Nw <= 0 || Kw <= 0 || (Nw % 8) || (Kw % 8)) return dfd_set_error(DFD_ERR_ARG, "dfd_gemm_wgrad_mma: Nw%8, Kw%8");
     int tn = cdiv(Nw, WG_BN), tk = cdiv(Kw, WG_BK);
     long long max_splits = (M + WG_BM * 4 - 1) / (WG_BM * 4);
-    long long splits = (148 * 4 + tn * tk - 1) / (tn * tk);
+    long long splits = (DFD_SMS * 4 + tn * tk - 1) / (tn * tk);
     if (splits > max_splits) splits = max_splits;
     if (splits < 1) splits = 1;
     if (splits > 65535) splits = 65535;

@@ -1,6 +1,6 @@
-// Pointwise (1x1) convolution GEMM on the Blackwell tensor-core path: TMA -> shared memory (128B swizzle) ->
-// tcgen05.mma (cta_group::1, kind::f16, fp32 accumulators in TMEM) -> tcgen05.ld epilogue -> swizzled smem ->
-// TMA store, with the per-channel BatchNorm statistics of the stored tile reduced in the same epilogue.
+// Pointwise (1x1) convolution GEMM on the Hopper tensor-core path: TMA -> shared memory (128B swizzle) ->
+// wgmma.mma_async (kind f16 / bf16, fp32 accumulators in registers) -> swizzled smem -> TMA store, with the per-channel
+// BatchNorm statistics of the stored tile reduced in the same epilogue.
 //
 //   C[M,N] = A[M,K] * B[N,K]^T          A: NHWC activations / output gradients (K-contiguous rows)
 //                                        B: conv weight [Cout,Cin] (forward) or its transpose [Cin,Cout] (dgrad)
@@ -9,14 +9,16 @@
 // efficientnet.py:292, resnet.py:192,199) and its input-gradient (autograd, train.py:634-636).
 //
 // Shape regime (SURVEY.md 8a H1a): M = N*H*W is 12.5k .. 3.2M, K and N are 16 .. 1280 -> every instance is
-// HBM-bound (AI << 219 FLOP/B), so the design goal is to stream A and C at HBM rate, not MMA peak:
-//   * persistent CTAs (one per SM), tiles 128 x BLOCK_N, BLOCK_N = whole N when N <= 256 (A is read once);
+// HBM-bound, so the design goal is to stream A and C at HBM rate, not MMA peak:
+//   * persistent CTAs (one per SM), tiles 128 x BLOCK_N, BLOCK_N = whole N when N <= 128 (A is read once);
 //   * K/N/M tails need no padding copies: TMA zero-fills out-of-bounds loads and clips stores;
-//   * 2 TMEM accumulator stages so the epilogue of tile i overlaps the loads + MMAs of tile i+1;
-//   * warp roles: w0 TMA producer, w1 MMA issuer, w2 TMEM allocator, w4-7 epilogue (TMEM lane quarter = warp%4).
+//   * warp roles: w0 TMA producer (runs up to `stages` k-blocks ahead, so the loads of tile i+1 stream during the
+//     epilogue of tile i); warpgroups 1 and 2 issue the MMAs of rows 0-63 / 64-127 of a tile and drain them.
 #include <cuda.h>
 #include <stdio.h>
 #include <stdlib.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 #include "bn_finalize.cuh"
@@ -25,14 +27,12 @@ namespace {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;          // 64 x 2 B = one 128-byte swizzle row
-constexpr int UMMA_K = 16;
+constexpr int MMA_K = 16;
 constexpr int SLAB = 64;             // epilogue / TMA-store column slab
-constexpr int NUM_THREADS = 384;      // TMA, MMA, TMEM-alloc, spare warp + two epilogue warpgroups
-constexpr int EPI_THREADS = 128;      // per epilogue warpgroup
-constexpr int TMEM_COLS = 256;         // per CTA; two CTAs share an SM's 512 columns
-constexpr int ACC_STRIDE = 128;      // TMEM column offset between the two accumulator stages
+constexpr int NUM_THREADS = 384;     // producer warpgroup (one active thread) + two MMA / epilogue warpgroups
+constexpr int EPI_THREADS = 256;
 constexpr int MAX_BLOCK_N = 128;
-constexpr int SMEM_BUDGET = 200 * 1024;   // one CTA per SM (the epilogue holds a whole 128 x 128 fp32 tile in registers)
+constexpr int SMEM_BUDGET = 224 * 1024;   // one CTA per SM (H100: up to 227 KB of shared memory per block)
 
 __device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -93,61 +93,123 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
 
-// ---- tcgen05 --------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_addr(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---- wgmma ----------------------------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { wgmma_wait<0>(); }
+// keeps the compiler from touching the accumulators while an asynchronous MMA owns them
+template <int R> __device__ __forceinline__ void fence_acc(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_addr(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, bf16/fp16 inputs, fp32 accumulate
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// K-major operand tile in shared memory, 128-byte swizzle: rows of 128 B, 8-row groups 1024 B apart.
-// (cute::UMMA::SmemDescriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48), layout [61,64))
-__device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t saddr) {
+// D[64 x 64] (+)= A[64 x 16] * B[16 x 64], both operands from shared-memory descriptors; TA / TB = 1: that operand
+// is MN-major. accumulate == 0 overwrites D.
+template <typename T, int TA, int TB>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    if constexpr (std::is_same<T, bf16>::value) {
+        asm volatile(
+            "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
+            "%0,%1,%2,%3,%4,%5,%6,%7,"
+            "%8,%9,%10,%11,%12,%13,%14,%15,"
+            "%16,%17,%18,%19,%20,%21,%22,%23,"
+            "%24,%25,%26,%27,%28,%29,%30,%31"
+            "}, %32, %33, p, 1, 1, %35, %36;\n}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
+    }
+    else {
+        asm volatile(
+            "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {"
+            "%0,%1,%2,%3,%4,%5,%6,%7,"
+            "%8,%9,%10,%11,%12,%13,%14,%15,"
+            "%16,%17,%18,%19,%20,%21,%22,%23,"
+            "%24,%25,%26,%27,%28,%29,%30,%31"
+            "}, %32, %33, p, 1, 1, %35, %36;\n}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
+    }
+}
+// D[64 x 128] (+)= A[64 x 16] * B[16 x 128], both operands from shared-memory descriptors; TA / TB = 1: that operand
+// is MN-major. accumulate == 0 overwrites D.
+template <typename T, int TA, int TB>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    if constexpr (std::is_same<T, bf16>::value) {
+        asm volatile(
+            "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+            "%0,%1,%2,%3,%4,%5,%6,%7,"
+            "%8,%9,%10,%11,%12,%13,%14,%15,"
+            "%16,%17,%18,%19,%20,%21,%22,%23,"
+            "%24,%25,%26,%27,%28,%29,%30,%31,"
+            "%32,%33,%34,%35,%36,%37,%38,%39,"
+            "%40,%41,%42,%43,%44,%45,%46,%47,"
+            "%48,%49,%50,%51,%52,%53,%54,%55,"
+            "%56,%57,%58,%59,%60,%61,%62,%63"
+            "}, %64, %65, p, 1, 1, %67, %68;\n}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+              "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+              "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+              "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+              "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
+    }
+    else {
+        asm volatile(
+            "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
+            "%0,%1,%2,%3,%4,%5,%6,%7,"
+            "%8,%9,%10,%11,%12,%13,%14,%15,"
+            "%16,%17,%18,%19,%20,%21,%22,%23,"
+            "%24,%25,%26,%27,%28,%29,%30,%31,"
+            "%32,%33,%34,%35,%36,%37,%38,%39,"
+            "%40,%41,%42,%43,%44,%45,%46,%47,"
+            "%48,%49,%50,%51,%52,%53,%54,%55,"
+            "%56,%57,%58,%59,%60,%61,%62,%63"
+            "}, %64, %65, p, 1, 1, %67, %68;\n}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+              "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+              "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+              "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+              "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
+    }
+}
+
+template <typename T, int BN, int TA, int TB>
+__device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    if constexpr (BN == 64) wgmma_n64<T, TA, TB>(d, adesc, bdesc, accumulate);
+    else wgmma_n128<T, TA, TB>(d, adesc, bdesc, accumulate);
+}
+
+// Shared-memory matrix descriptor (sm_90 GMMA): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), layout [62,64) (1 = 128B
+// swizzle). K-major operand: rows of 128 B, 8-row groups 1024 B apart (SBO), LBO unused. MN-major operand: 64 contiguous
+// MN elements per K row, 8-row groups along K 1024 B apart (SBO), 64-element MN blocks `lbo_bytes` apart (LBO).
+__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t saddr, uint32_t lbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-    d |= (uint64_t)1 << 16;                 // LBO: unused for swizzled K-major
-    d |= (uint64_t)(1024 >> 4) << 32;       // SBO = 1024 B between 8-row core-matrix groups
-    d |= (uint64_t)1 << 46;                 // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                 // SWIZZLE_128B
-    return d;
-}
-// cute::UMMA::InstrDescriptor for kind::f16: c_format F32 (1) [4,6), a/b format [7,10)/[10,13) (F16=0, BF16=1),
-// a/b major K (0) bits 15/16, N>>3 [17,23), M>>4 [24,29)
-__device__ __forceinline__ uint32_t make_idesc(int is_bf16, int n) {
-    uint32_t d = 0;
-    d |= 1u << 4;
-    d |= (uint32_t)(is_bf16 ? 1 : 0) << 7;
-    d |= (uint32_t)(is_bf16 ? 1 : 0) << 10;
-    d |= (uint32_t)(n >> 3) << 17;
-    d |= (uint32_t)(BLOCK_M >> 4) << 24;
+    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
+    d |= (uint64_t)(1024 >> 4) << 32;
+    d |= (uint64_t)1 << 62;
     return d;
 }
 
-__device__ __forceinline__ void epi_barrier(int wg) { asm volatile("bar.sync %0, %1;" ::"r"(wg + 1), "n"(EPI_THREADS) : "memory"); }
+__device__ __forceinline__ void epi_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory"); }
 
 struct BlockDiagDesc {
     const void* src;
@@ -182,58 +244,50 @@ struct TcParams {
     int cv_ntaps;
     int cv_tox[9], cv_toy[9], cv_tk[9];
     int cv_accum;                     // conv mode: the output tile is ADDED to the destination (TMA reduction store)
-    int dbg;              // debug switches (DFD_DBG env): 1 = skip TMA store, 2 = skip stats pass, 4 = skip slabs, 8 = A from L2
-    long long* ts;        // optional trace (DFD_TS env): CTA 0 records clock64 at 8 pipeline points for its first 32 tiles
+    int dbg;              // debug switches (DFD_DBG env): 1 = skip TMA store, 2 = skip stats pass, 8 = A from L2
 };
 
-template <typename T>
+// BN = the MMA's N (64 or 128): the B tile holds block_n <= BN real rows; the MMA also reads the rows above them, whose
+// products land in accumulator columns that are never stored.
+template <typename T, int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const __grid_constant__ CUtensorMap tmap_c, const TcParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // SWIZZLE_128B tiles must sit on 1024-byte boundaries of the shared address space
     uint8_t* smem = smem_raw + ((1024u - (smem_addr(smem_raw) & 1023u)) & 1023u);
-    // carve-up (all tile bases 1024-byte aligned): [A stages][B stages][2 warpgroups x 2 C slabs][barriers]
-    const uint32_t a_bytes = BLOCK_M * BLOCK_K * 2;
-    const uint32_t b_bytes = (uint32_t)p.block_n * BLOCK_K * 2;
-    const uint32_t b_stride = (b_bytes + 1023) & ~1023u;
+    // carve-up (all tile bases 1024-byte aligned): [A stages][B stages][2 C slabs][barriers][statistics scratch]
+    constexpr uint32_t a_bytes = BLOCK_M * BLOCK_K * 2;
+    constexpr uint32_t b_stride = BN * BLOCK_K * 2;
+    const uint32_t b_bytes = (uint32_t)p.block_n * BLOCK_K * 2;      // bytes TMA delivers per B tile
     uint8_t* smem_a = smem;
     uint8_t* smem_b = smem_a + (size_t)p.stages * a_bytes;
     uint8_t* smem_c = smem_b + (size_t)p.stages * b_stride;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem_c + 4 * BLOCK_M * SLAB * 2);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem_c + 2 * BLOCK_M * SLAB * 2);
     uint64_t* full_bar = bars;
     uint64_t* empty_bar = bars + 8;
-    uint64_t* tmem_full = bars + 16;
-    uint64_t* tmem_empty = bars + 18;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 20);
-    float* red_all = reinterpret_cast<float*>(bars + 22);    // [warpgroup][2][2][64]
+    float* red = reinterpret_cast<float*>(bars + 16);    // [sum / sq][4 row quarters][64 columns]
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int lane = threadIdx.x & 31;
+    // warpgroup index made visibly warp-uniform: the compiler can then keep the wgmma sequences of the MMA warpgroups unserialised
+    const int wgi = __shfl_sync(0xffffffffu, (int)threadIdx.x / 128, 0);
     const int num_tiles = p.num_m_tiles * p.num_n_tiles;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         prefetch_tmap(&tmap_a);
         prefetch_tmap(&tmap_b);
         prefetch_tmap(&tmap_c);
-    }
-    if (warp == 1 && lane == 0) {
-        for (int i = 0; i < p.stages; i++) { mbar_init(full_bar + i, 1); mbar_init(empty_bar + i, 1); }
-        for (int i = 0; i < 2; i++) { mbar_init(tmem_full + i, 1); mbar_init(tmem_empty + i, EPI_THREADS); }
+        for (int i = 0; i < p.stages; i++) { mbar_init(full_bar + i, 1); mbar_init(empty_bar + i, 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) tmem_alloc(tmem_ptr, TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
-    if (warp == 0) {
+    if (wgi == 0) {
         // ================= TMA producer =================
-        if (lane == 0) {
+        if (threadIdx.x == 0) {
             int stage = 0;
             uint32_t phase = 0;
-            int lt = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, lt++) {
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
                 const int m_idx = tile / p.num_n_tiles, n_idx = tile - m_idx * p.num_n_tiles;
                 int cx0 = 0, cy0 = 0, cn0 = 0;
                 if (p.conv) {
@@ -242,7 +296,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                 }
                 for (int kb = 0; kb < p.num_k_blocks; kb++) {
                     mbar_wait(empty_bar + stage, phase ^ 1);
-                    if (p.ts && kb == 0 && blockIdx.x == 0 && lt < 32) p.ts[lt * 8 + 0] = clock64();
                     int bk = kb * BLOCK_K;
                     if (p.conv) {
                         const int tap = kb / p.cv_cpb, cb = kb - tap * p.cv_cpb;
@@ -265,126 +318,81 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        if (lane == 0) {
-            const uint32_t idesc = make_idesc(p.is_bf16, p.block_n);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            int lt = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, lt++) {
-                mbar_wait(tmem_empty + acc, acc_phase ^ 1);
-                tc_fence_after();
-                const bool rec = p.ts && blockIdx.x == 0 && lt < 32;
-                if (rec) p.ts[lt * 8 + 1] = clock64();
-                const uint32_t d_tmem = tmem_base + acc * ACC_STRIDE;
-                for (int kb = 0; kb < p.num_k_blocks; kb++) {
-                    mbar_wait(full_bar + stage, phase);
-                    tc_fence_after();
-                    if (rec && kb == 0) p.ts[lt * 8 + 2] = clock64();
-                    const uint32_t a_addr = smem_addr(smem_a + (size_t)stage * a_bytes);
-                    const uint32_t b_addr = smem_addr(smem_b + (size_t)stage * b_stride);
-                    int krem = p.K - kb * BLOCK_K;
-                    int nk = krem >= BLOCK_K ? BLOCK_K / UMMA_K : (krem + UMMA_K - 1) / UMMA_K;
-                    for (int k = 0; k < nk; k++) {
-                        uint64_t adesc = make_kmajor_sw128_desc(a_addr + k * UMMA_K * 2);
-                        uint64_t bdesc = make_kmajor_sw128_desc(b_addr + k * UMMA_K * 2);
-                        umma_f16(d_tmem, adesc, bdesc, idesc, (kb | k) != 0 ? 1u : 0u);
-                    }
-                    umma_commit(empty_bar + stage);          // frees the smem stage when the MMAs have read it
-                    if (++stage == p.stages) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(tmem_full + acc);                // accumulator complete -> epilogue
-                if (rec) p.ts[lt * 8 + 3] = clock64();
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else if (warp >= 4) {
-        // ================= epilogue: two warpgroups, one per accumulator stage =================
-        // The CTA's i-th tile accumulates in TMEM stage i & 1 and is drained by warpgroup i & 1, so two tiles are in the
-        // epilogue at once (measured: one warpgroup needs ~2500 cycles per 128 x 96 tile - TMEM load, pack, staging,
-        // TMA store - which alone caps output-heavy GEMMs at a third of the HBM rate).
-        const int wg = (warp - 4) >> 2;                                // 0 / 1
-        const int et = (threadIdx.x - 128) & 127;                      // 0..127 == TMEM lane == tile row
-        const int q = warp & 3;                                        // TMEM lane quarter this warp may access
+    } else {
+        // ================= MMA + epilogue: warpgroup wg owns rows 64 * wg .. 64 * wg + 63 of every tile =================
+        const int et = threadIdx.x - (NUM_THREADS - EPI_THREADS);      // 0..255
+        const int wg = wgi - 1;
+        const int r0 = wg * 64 + ((et >> 5) & 3) * 16 + (lane >> 2);    // this thread's accumulator rows: r0 and r0 + 8
+        const int cq = (lane & 3) * 2;                                  // and columns 8 j + cq, 8 j + cq + 1
         const bool leader = et == 0;
-        uint8_t* my_c = smem_c + (size_t)wg * (2 * BLOCK_M * SLAB * 2);
-        float* red = red_all + wg * 256;
-        uint32_t acc_phase = 0;
+        int stage = 0;
+        uint32_t phase = 0;
         uint32_t slab_count = 0;
         const int nslabs = (p.block_n + SLAB - 1) / SLAB;
         const bool keep = p.num_n_tiles == 1;          // column identity is fixed -> keep sums in registers
         float ks[2] = {0.f, 0.f}, kq[2] = {0.f, 0.f};
-        const uint32_t t_base = tmem_base + wg * ACC_STRIDE + ((uint32_t)(q * 32) << 16);
-        int lt = wg;                                    // index of the tile within this CTA's sequence
-        for (int tile = blockIdx.x + wg * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x, lt += 2) {
+        float acc[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             const int m_idx = tile / p.num_n_tiles, n_idx = tile - m_idx * p.num_n_tiles;
-            const bool rec = p.ts && leader && blockIdx.x == 0 && lt < 32;
-            // convolution mode: this thread's row is output pixel (n0 + tn, y0 + ty, x0 + tx) of the patch; rows beyond the patch
+            // convolution mode: row r of the tile is output pixel (n0 + tn, y0 + ty, x0 + tx) of the patch; rows beyond the patch
             // or the image hold garbage accumulators and are zeroed (they would otherwise enter the BatchNorm statistics)
             int cx0 = 0, cy0 = 0, cn0 = 0;
-            bool row_ok = true;
+            bool ok0 = true, ok1 = true;
             if (p.conv) {
                 const int txi = m_idx % p.cv_tiles_x, r = m_idx / p.cv_tiles_x;
                 cx0 = txi * p.cv_TW; cy0 = (r % p.cv_tiles_y) * p.cv_TH; cn0 = (r / p.cv_tiles_y) * p.cv_TN;
-                const int px = et % p.cv_TW, q2 = et / p.cv_TW;
-                const int py = q2 % p.cv_TH, pn = q2 / p.cv_TH;
-                row_ok = et < p.cv_rows && cx0 + px < p.cv_W && cy0 + py < p.cv_H && cn0 + pn < p.cv_N;
+                auto row_ok = [&](int row) {
+                    const int px = row % p.cv_TW, q2 = row / p.cv_TW;
+                    const int py = q2 % p.cv_TH, pn = q2 / p.cv_TH;
+                    return row < p.cv_rows && cx0 + px < p.cv_W && cy0 + py < p.cv_H && cn0 + pn < p.cv_N;
+                };
+                ok0 = row_ok(r0); ok1 = row_ok(r0 + 8);
             }
-            if (rec) p.ts[lt * 8 + 4] = clock64();
-            mbar_wait(tmem_full + wg, acc_phase);
-            tc_fence_after();
-            if (rec) p.ts[lt * 8 + 5] = clock64();
-            uint32_t v[SLAB / 16][16];
+            // one k-block's MMAs stay in flight while the next block's are issued; a stage goes back to the producer once the
+            // MMAs that read it have completed (the wait for all but the newest group)
+            int prev_stage = -1;
+            for (int kb = 0; kb < p.num_k_blocks; kb++) {
+                mbar_wait(full_bar + stage, phase);
+                const uint32_t a_addr = smem_addr(smem_a + (size_t)stage * a_bytes) + wg * 64 * 128;
+                const uint32_t b_addr = smem_addr(smem_b + (size_t)stage * b_stride);
+                const int krem = p.K - kb * BLOCK_K;
+                const int nk = krem >= BLOCK_K ? BLOCK_K / MMA_K : (krem + MMA_K - 1) / MMA_K;
+                fence_acc(acc);
+                wgmma_fence();
+                for (int k = 0; k < nk; k++)
+                    wgmma_tile<T, BN, 0, 0>(acc, make_sw128_desc(a_addr + k * MMA_K * 2, 16),
+                                            make_sw128_desc(b_addr + k * MMA_K * 2, 16), (kb | k) != 0 ? 1u : 0u);
+                wgmma_commit();
+                wgmma_wait<1>();
+                fence_acc(acc);
+                if (prev_stage >= 0 && (et & 127) == 0) mbar_arrive(empty_bar + prev_stage);   // this warpgroup is done with it
+                prev_stage = stage;
+                if (++stage == p.stages) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait_all();
+            fence_acc(acc);
+            if ((et & 127) == 0) mbar_arrive(empty_bar + prev_stage);
 #pragma unroll
-            for (int q4 = 0; q4 < SLAB / 16; q4++)
-                if (q4 * 16 < p.block_n) tmem_ld16(t_base + q4 * 16, v[q4]);
-#pragma unroll
-            for (int s = 0; s < MAX_BLOCK_N / SLAB; s++) {
-                if (s >= nslabs || (p.dbg & 4)) break;
-                uint8_t* cbuf = my_c + (size_t)(slab_count & 1) * (BLOCK_M * SLAB * 2);
+            for (int s = 0; s < BN / SLAB; s++) {
+                if (s >= nslabs) break;
+                uint8_t* cbuf = smem_c + (size_t)(slab_count & 1) * (BLOCK_M * SLAB * 2);
                 const int ncols = min(SLAB, p.block_n - s * SLAB);
                 if (leader) tma_store_wait_read<1>();       // the store that last used this buffer has drained
-                tmem_ld_wait();
-                epi_barrier(wg);
+                epi_barrier();
 #pragma unroll
-                for (int q4 = 0; q4 < SLAB / 16; q4++) {
-                    if (q4 * 16 < ncols) {
-                        uint32_t (&w)[16] = v[q4];
-                        if (!row_ok) {
-#pragma unroll
-                            for (int z = 0; z < 16; z++) w[z] = 0u;
-                        }
-                        uint4 lo, hi;
-                        lo.x = pack2<T>(__uint_as_float(w[0]), __uint_as_float(w[1]));
-                        lo.y = pack2<T>(__uint_as_float(w[2]), __uint_as_float(w[3]));
-                        lo.z = pack2<T>(__uint_as_float(w[4]), __uint_as_float(w[5]));
-                        lo.w = pack2<T>(__uint_as_float(w[6]), __uint_as_float(w[7]));
-                        hi.x = pack2<T>(__uint_as_float(w[8]), __uint_as_float(w[9]));
-                        hi.y = pack2<T>(__uint_as_float(w[10]), __uint_as_float(w[11]));
-                        hi.z = pack2<T>(__uint_as_float(w[12]), __uint_as_float(w[13]));
-                        hi.w = pack2<T>(__uint_as_float(w[14]), __uint_as_float(w[15]));
-                        const int j = q4 * 2;            // logical 16-byte chunk index within the 128-byte row
-                        uint8_t* row = cbuf + et * 128;
-                        *reinterpret_cast<uint4*>(row + ((j ^ (et & 7)) << 4)) = lo;
-                        *reinterpret_cast<uint4*>(row + (((j + 1) ^ (et & 7)) << 4)) = hi;
+                for (int j = 0; j < SLAB / 8; j++) {
+                    if (j * 8 < ncols) {
+                        const int i = (s * (SLAB / 8) + j) * 4;
+                        // logical 16-byte chunk j of a 128-byte row sits at chunk j ^ (row & 7) (r0 and r0 + 8 share row & 7)
+                        const uint32_t off = ((j ^ (r0 & 7)) << 4) + cq * 2;
+                        *reinterpret_cast<uint32_t*>(cbuf + r0 * 128 + off) = ok0 ? pack2<T>(acc[i], acc[i + 1]) : 0u;
+                        *reinterpret_cast<uint32_t*>(cbuf + (r0 + 8) * 128 + off) = ok1 ? pack2<T>(acc[i + 2], acc[i + 3]) : 0u;
                     }
                 }
-                if (s + 1 < nslabs) {
-                    // the next slab's TMEM loads fly while this one is fenced, stored and reduced
-#pragma unroll
-                    for (int q4 = 0; q4 < SLAB / 16; q4++)
-                        if ((s + 1) * SLAB + q4 * 16 < p.block_n) tmem_ld16(t_base + (s + 1) * SLAB + q4 * 16, v[q4]);
-                } else {
-                    // all TMEM reads of this accumulator are done: hand it back to the MMA warp
-                    tc_fence_before();
-                    mbar_arrive(tmem_empty + wg);
-                    if (rec) p.ts[lt * 8 + 6] = clock64();
-                }
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                epi_barrier(wg);
+                epi_barrier();
                 if (leader && !(p.dbg & 1)) {
                     if (p.conv && p.cv_accum) tma_reduce_add_4d(&tmap_c, cbuf, n_idx * p.block_n + s * SLAB, cx0, cy0, cn0);
                     else if (p.conv) tma_store_4d(&tmap_c, cbuf, n_idx * p.block_n + s * SLAB, cx0, cy0, cn0);
@@ -393,14 +401,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                 }
                 if (p.dsum && !(p.dbg & 2)) {
                     // column statistics of the stored (rounded) slab; rows past M are exact zeros
-                    const int c = et & 63, half = et >> 6;
+                    const int c = et & 63, qd = et >> 6;
                     float sum = 0.f, sq = 0.f;
                     if (c < ncols) {
                         const uint8_t* colp = cbuf + (c & 7) * 2;
                         const int jc = c >> 3;
                         float s1 = 0.f, q1 = 0.f;            // two chains: the adds are latency-, not throughput-bound
 #pragma unroll 8
-                        for (int r = half * 64; r < half * 64 + 64; r += 2) {
+                        for (int r = qd * 32; r < qd * 32 + 32; r += 2) {
                             float x0 = to_f<T>(*reinterpret_cast<const T*>(colp + r * 128 + ((jc ^ (r & 7)) << 4)));
                             float x1 = to_f<T>(*reinterpret_cast<const T*>(colp + (r + 1) * 128 + ((jc ^ ((r + 1) & 7)) << 4)));
                             sum += x0; s1 += x1;
@@ -408,11 +416,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                         }
                         sum += s1; sq += q1;
                     }
-                    red[(0 * 2 + half) * 64 + c] = sum;
-                    red[(1 * 2 + half) * 64 + c] = sq;
-                    epi_barrier(wg);
+                    red[qd * 64 + c] = sum;
+                    red[256 + qd * 64 + c] = sq;
+                    epi_barrier();
                     if (et < 64) {
-                        float ts = red[et] + red[64 + et], tq = red[128 + et] + red[192 + et];
+                        float ts = (red[et] + red[64 + et]) + (red[128 + et] + red[192 + et]);
+                        float tq = (red[256 + et] + red[320 + et]) + (red[384 + et] + red[448 + et]);
                         if (keep) { ks[s] += ts; kq[s] += tq; }
                         else {
                             int gc = n_idx * p.block_n + s * SLAB + et;
@@ -425,9 +434,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                 }
                 slab_count++;
             }
-            if (p.dbg & 4) { tmem_ld_wait(); tc_fence_before(); mbar_arrive(tmem_empty + wg); }
-            if (rec) p.ts[lt * 8 + 7] = clock64();
-            acc_phase ^= 1;
         }
         if (p.dsum && keep && et < 64) {
 #pragma unroll
@@ -442,32 +448,22 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         if (leader) tma_store_wait_read<0>();
     }
 
-    tc_fence_before();
     __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, TMEM_COLS);
     bn_finalize_tail(p.fin, threadIdx.x, NUM_THREADS);
 }
 
 // =============================================================================================
-// 1x1 conv weight gradient on tcgen05: dW[Nw,Kw] (fp32, accumulated) += G[M,Nw]^T * X[M,Kw].
+// 1x1 conv weight gradient on wgmma: dW[Nw,Kw] (fp32, accumulated) += G[M,Nw]^T * X[M,Kw].
 // The contraction runs over the NHWC rows, so BOTH operands are MN-major for the MMA: a TMA box of {64 channels, 64 rows}
-// with 128-byte swizzle is already the canonical MN-major SW128 atom sequence (64 contiguous MN elements per K row, 8-row
+// with 128-byte swizzle is already the canonical MN-major SW128 layout (64 contiguous MN elements per K row, 8-row
 // groups 1024 B apart = SBO; 64-channel column blocks one box apart = LBO), so the tiles go from NHWC memory to the tensor
 // core without any transpose. One CTA = one (128 x block_n) tile of dW and one contiguous range of 64-row blocks (split-K);
-// the fp32 accumulator lives in TMEM for the whole range and is flushed once with red.global.add.
+// warpgroup w accumulates rows 64 w .. 64 w + 63 of the tile in registers for the whole range and flushes them once.
+// Thread 0 also issues the TMA loads, `stages` row blocks ahead of the MMAs.
 // =============================================================================================
 constexpr int WG_KP = 64;                      // rows (pixels) per pipeline stage
 constexpr int WG_BOX_BYTES = WG_KP * 128;      // one {64 ch, 64 rows} box
-
-__device__ __forceinline__ uint64_t make_mnmajor_sw128_desc(uint32_t saddr, uint32_t lbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;     // LBO: next 64-element block along M / N
-    d |= (uint64_t)(1024 >> 4) << 32;                     // SBO: next 8-row group along K
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;                               // SWIZZLE_128B
-    return d;
-}
+constexpr int WG_THREADS = 256;
 
 struct WgParams {
     long long M;
@@ -492,23 +488,22 @@ struct WgParams {
     int cv_k, cv_pad, cv_cpb, cv_S;
 };
 
-template <typename T>
-__global__ void __launch_bounds__(256, 2)
+// BN = the MMA's N (64 or 128) = 64 x the number of X boxes per stage
+template <typename T, int BN>
+__global__ void __launch_bounds__(WG_THREADS, 2)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_constant__ CUtensorMap tmap_x,
                 float* __restrict__ dW, const WgParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_addr(smem_raw) & 1023u)) & 1023u);
-    const int nbox_b = p.block_n > 64 ? 2 : 1;
-    const uint32_t a_bytes = 2 * WG_BOX_BYTES, b_bytes = (uint32_t)nbox_b * WG_BOX_BYTES;
+    constexpr int nbox_b = BN / 64;
+    constexpr uint32_t a_bytes = 2 * WG_BOX_BYTES, b_bytes = nbox_b * WG_BOX_BYTES;
     uint8_t* smem_a = smem;
     uint8_t* smem_b = smem_a + (size_t)p.stages * a_bytes;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + (size_t)p.stages * b_bytes);
     uint64_t* full_bar = bars;
     uint64_t* empty_bar = bars + 8;
-    uint64_t* tmem_full = bars + 16;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 17);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int lane = threadIdx.x & 31;
     const int m0 = blockIdx.x * 128, n0 = blockIdx.y * p.block_n;
     const long long kb0 = (long long)blockIdx.z * p.kb_per_split;
     long long kb1 = kb0 + p.kb_per_split;
@@ -517,130 +512,100 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_constan
     const bool a_box1 = m0 + 64 < p.Nw;                       // second 64-channel block of the tile exists
     const bool b_box1 = nbox_b == 2 && n0 + 64 < p.Kw;
 
-    if (warp == 0 && lane == 0) { prefetch_tmap(&tmap_g); prefetch_tmap(&tmap_x); }
     if (p.conv && p.cv_rows < WG_KP) {
         uint4* z = reinterpret_cast<uint4*>(smem_a);
         const int n16 = (int)((size_t)p.stages * (a_bytes + b_bytes) / 16);
         for (int i = threadIdx.x; i < n16; i += blockDim.x) z[i] = make_uint4(0u, 0u, 0u, 0u);
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
-    if (warp == 1 && lane == 0) {
-        for (int i = 0; i < p.stages; i++) { mbar_init(full_bar + i, 1); mbar_init(empty_bar + i, 1); }
-        mbar_init(tmem_full, 1);
+    if (threadIdx.x == 0) {
+        prefetch_tmap(&tmap_g);
+        prefetch_tmap(&tmap_x);
+        for (int i = 0; i < p.stages; i++) { mbar_init(full_bar + i, 1); mbar_init(empty_bar + i, 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) tmem_alloc(tmem_ptr, 128);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
-    if (warp == 0) {
-        if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
-            const uint32_t box_bytes = p.conv ? (uint32_t)p.cv_rows * 128u : (uint32_t)WG_BOX_BYTES;
-            const uint32_t tx = ((a_box1 ? 2u : 1u) + (b_box1 ? 2u : 1u)) * box_bytes;
-            // convolution mode: (tap, channel block) of this tile's one or two 64-column blocks
-            int bt_c[2] = {0, 0}, bt_dx[2] = {0, 0}, bt_dy[2] = {0, 0};
-            if (p.conv) {
-#pragma unroll
-                for (int i = 0; i < 2; i++) {
-                    const int jb = n0 / 64 + i, tap = jb / p.cv_cpb;
-                    bt_c[i] = (jb - tap * p.cv_cpb) * 64;
-                    bt_dy[i] = tap / p.cv_k - p.cv_pad;
-                    bt_dx[i] = tap % p.cv_k - p.cv_pad;
-                }
+    // loads of row block kb into `stage` (thread 0 only)
+    auto issue = [&](long long kb, int stage) {
+        const uint32_t box_bytes = p.conv ? (uint32_t)p.cv_rows * 128u : (uint32_t)WG_BOX_BYTES;
+        mbar_arrive_expect_tx(full_bar + stage, ((a_box1 ? 2u : 1u) + (b_box1 ? 2u : 1u)) * box_bytes);
+        uint8_t* a = smem_a + (size_t)stage * a_bytes;
+        uint8_t* b = smem_b + (size_t)stage * b_bytes;
+        if (p.conv) {
+            const int pt = (int)kb, txi = pt % p.cv_tiles_x, r = pt / p.cv_tiles_x;
+            const int cx0 = txi * p.cv_TW, cy0 = (r % p.cv_tiles_y) * p.cv_TH, cn0 = (r / p.cv_tiles_y) * p.cv_TN;
+            tma_load_4d(a, &tmap_g, full_bar + stage, m0, cx0, cy0, cn0);
+            if (a_box1) tma_load_4d(a + WG_BOX_BYTES, &tmap_g, full_bar + stage, m0 + 64, cx0, cy0, cn0);
+            // (tap, channel block) of this tile's one or two 64-column blocks
+            for (int i = 0; i < (b_box1 ? 2 : 1); i++) {
+                const int jb = n0 / 64 + i, tap = jb / p.cv_cpb;
+                tma_load_4d(b + i * WG_BOX_BYTES, &tmap_x, full_bar + stage, (jb - tap * p.cv_cpb) * 64,
+                            cx0 * p.cv_S + tap % p.cv_k - p.cv_pad, cy0 * p.cv_S + tap / p.cv_k - p.cv_pad, cn0);
             }
-            for (long long kb = kb0; kb < kb1; kb++) {
-                mbar_wait(empty_bar + stage, phase ^ 1);
-                mbar_arrive_expect_tx(full_bar + stage, tx);
-                uint8_t* a = smem_a + (size_t)stage * a_bytes;
-                uint8_t* b = smem_b + (size_t)stage * b_bytes;
-                if (p.conv) {
-                    const int pt = (int)kb, txi = pt % p.cv_tiles_x, r = pt / p.cv_tiles_x;
-                    const int cx0 = txi * p.cv_TW, cy0 = (r % p.cv_tiles_y) * p.cv_TH, cn0 = (r / p.cv_tiles_y) * p.cv_TN;
-                    tma_load_4d(a, &tmap_g, full_bar + stage, m0, cx0, cy0, cn0);
-                    if (a_box1) tma_load_4d(a + WG_BOX_BYTES, &tmap_g, full_bar + stage, m0 + 64, cx0, cy0, cn0);
-                    tma_load_4d(b, &tmap_x, full_bar + stage, bt_c[0], cx0 * p.cv_S + bt_dx[0], cy0 * p.cv_S + bt_dy[0], cn0);
-                    if (b_box1) tma_load_4d(b + WG_BOX_BYTES, &tmap_x, full_bar + stage, bt_c[1], cx0 * p.cv_S + bt_dx[1], cy0 * p.cv_S + bt_dy[1], cn0);
-                    if (++stage == p.stages) { stage = 0; phase ^= 1; }
-                    continue;
-                }
-                const int row = (int)(kb * WG_KP);
-                tma_load_2d(a, &tmap_g, full_bar + stage, m0, row);
-                if (a_box1) tma_load_2d(a + WG_BOX_BYTES, &tmap_g, full_bar + stage, m0 + 64, row);
-                tma_load_2d(b, &tmap_x, full_bar + stage, n0, row);
-                if (b_box1) tma_load_2d(b + WG_BOX_BYTES, &tmap_x, full_bar + stage, n0 + 64, row);
-                if (++stage == p.stages) { stage = 0; phase ^= 1; }
-            }
+            return;
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // instruction descriptor: fp32 accumulate, 16-bit inputs, A and B MN-major (bits 15 / 16), N, M = 128
-            uint32_t idesc = make_idesc(p.is_bf16, p.block_n) | (1u << 15) | (1u << 16);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (long long kb = kb0; kb < kb1; kb++) {
-                mbar_wait(full_bar + stage, phase);
-                tc_fence_after();
-                const uint32_t a_addr = smem_addr(smem_a + (size_t)stage * a_bytes);
-                const uint32_t b_addr = smem_addr(smem_b + (size_t)stage * b_bytes);
+        const int row = (int)(kb * WG_KP);
+        tma_load_2d(a, &tmap_g, full_bar + stage, m0, row);
+        if (a_box1) tma_load_2d(a + WG_BOX_BYTES, &tmap_g, full_bar + stage, m0 + 64, row);
+        tma_load_2d(b, &tmap_x, full_bar + stage, n0, row);
+        if (b_box1) tma_load_2d(b + WG_BOX_BYTES, &tmap_x, full_bar + stage, n0 + 64, row);
+    };
+
+    const long long nkb = kb1 - kb0;
+    if (threadIdx.x == 0)
+        for (int s = 0; s < p.stages && s < nkb; s++) issue(kb0 + s, s);
+
+    const int wg = threadIdx.x >> 7;
+    float acc[BN / 2];
 #pragma unroll
-                for (int k = 0; k < WG_KP / UMMA_K; k++) {
-                    // 16 rows of K = two 8-row groups = 2048 bytes further into every box
-                    const uint64_t adesc = make_mnmajor_sw128_desc(a_addr + k * (UMMA_K * 128), WG_BOX_BYTES);
-                    const uint64_t bdesc = make_mnmajor_sw128_desc(b_addr + k * (UMMA_K * 128), WG_BOX_BYTES);
-                    umma_f16(tmem_base, adesc, bdesc, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-                }
-                umma_commit(empty_bar + stage);
-                if (++stage == p.stages) { stage = 0; phase ^= 1; }
-            }
-            umma_commit(tmem_full);
+    for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (long long i = 0; i < nkb; i++) {
+        mbar_wait(full_bar + stage, phase);
+        const uint32_t a_addr = smem_addr(smem_a + (size_t)stage * a_bytes + wg * WG_BOX_BYTES);
+        const uint32_t b_addr = smem_addr(smem_b + (size_t)stage * b_bytes);
+        fence_acc(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < WG_KP / MMA_K; k++)      // 16 rows of K = two 8-row groups = 2048 bytes further into every box
+            wgmma_tile<T, BN, 1, 1>(acc, make_sw128_desc(a_addr + k * (MMA_K * 128), WG_BOX_BYTES),
+                                    make_sw128_desc(b_addr + k * (MMA_K * 128), WG_BOX_BYTES), (i > 0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait_all();
+        fence_acc(acc);
+        if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar + stage);
+        if (threadIdx.x == 0 && i + p.stages < nkb) {
+            mbar_wait(empty_bar + stage, phase);            // both warpgroups have read the stage: refill it
+            issue(kb0 + i + p.stages, stage);
         }
-    } else if (warp >= 4) {
-        const int q = warp & 3;
-        mbar_wait(tmem_full, 0);
-        tc_fence_after();
-        const int row = m0 + q * 32 + lane;                  // dW row (output channel) of this TMEM lane
-        const uint32_t t_base = tmem_base + ((uint32_t)(q * 32) << 16);
-        if (p.part) {
-            // ---- deterministic path: plain stores of this split's partial tile (summed later in split order) ----
-            float* mine = p.part + (size_t)blockIdx.z * p.Nw * p.Kw;
-            for (int c = 0; c < p.block_n; c += 16) {
-                uint32_t v[16];
-                tmem_ld16(t_base + c, v);
-                tmem_ld_wait();
-                if (row < p.Nw) {
-                    float* dst = mine + (size_t)row * p.Kw + n0 + c;
+        __syncwarp();
+        if (++stage == p.stages) { stage = 0; phase ^= 1; }
+    }
+
+    // Accumulator (row r, columns 8 j + 2 q, +1) and (row r + 8, same columns), q = lane & 3. Neighbouring lanes swap one pair
+    // so that each holds four consecutive columns of one row: 16-byte stores / reductions (the small-M layers are bound by
+    // the NUMBER of L2 reduction ops, not by their bytes). Kw % 8 == 0 keeps every group of 4 columns aligned and all-or-nothing.
+    const int q = lane & 3;
+    const bool odd = q & 1;
+    const int row = m0 + wg * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2) + (odd ? 8 : 0);
+    const int cb = 2 * (q & 2);
+    float* base = p.part ? p.part + (size_t)blockIdx.z * p.Nw * p.Kw : dW;
 #pragma unroll
-                    for (int j = 0; j < 16; j += 4)
-                        if (n0 + c + j < p.Kw)
-                            *reinterpret_cast<float4*>(dst + j) = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]),
-                                                                              __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-                }
-            }
-        } else
-        for (int c = 0; c < p.block_n; c += 16) {
-            uint32_t v[16];
-            tmem_ld16(t_base + c, v);
-            tmem_ld_wait();
-            if (row < p.Nw) {
-                // 16-byte vector reductions (Kw % 8 == 0 keeps every group of 4 columns aligned and all-or-nothing): the
-                // small-M layers are bound by the NUMBER of L2 reduction ops, not by their bytes
-                float* dst = dW + (size_t)row * p.Kw + n0 + c;
-#pragma unroll
-                for (int j = 0; j < 16; j += 4)
-                    if (n0 + c + j < p.Kw)
-                        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + j), "f"(__uint_as_float(v[j])),
-                                     "f"(__uint_as_float(v[j + 1])), "f"(__uint_as_float(v[j + 2])), "f"(__uint_as_float(v[j + 3]))
-                                     : "memory");
-            }
+    for (int j = 0; j < BN / 8; j++) {
+        const float s0 = odd ? acc[4 * j] : acc[4 * j + 2], s1 = odd ? acc[4 * j + 1] : acc[4 * j + 3];
+        const float o0 = __shfl_xor_sync(0xffffffffu, s0, 1), o1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+        const float4 v = odd ? make_float4(o0, o1, acc[4 * j + 2], acc[4 * j + 3]) : make_float4(acc[4 * j], acc[4 * j + 1], o0, o1);
+        const int col = n0 + 8 * j + cb;
+        if (8 * j < p.block_n && row < p.Nw && col < p.Kw) {
+            float* dst = base + (size_t)row * p.Kw + col;
+            if (p.part) *reinterpret_cast<float4*>(dst) = v;     // deterministic path: summed later in split order
+            else
+                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
+                             : "memory");
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, 128);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -702,6 +667,51 @@ static int make_map_nhwc(CUtensorMap* m, const void* base, int N, int H, int W, 
     return DFD_OK;
 }
 
+template <typename T, int BN>
+static void launch_tc_kernel(int grid, size_t smem, cudaStream_t st, const CUtensorMap& ma, const CUtensorMap& mb,
+                             const CUtensorMap& mc, const TcParams& p) {
+    static bool attr = false;
+    if (!attr) { cudaFuncSetAttribute(gemm_tc_kernel<T, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BUDGET); attr = true; }
+    gemm_tc_kernel<T, BN><<<grid, NUM_THREADS, smem, st>>>(ma, mb, mc, p);
+}
+
+template <typename T, int BN>
+static void launch_wgrad_kernel(dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& mg, const CUtensorMap& mx, float* dW,
+                                const WgParams& p) {
+    static bool attr = false;
+    if (!attr) { cudaFuncSetAttribute(wgrad_tc_kernel<T, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024); attr = true; }
+    wgrad_tc_kernel<T, BN><<<grid, WG_THREADS, smem, st>>>(mg, mx, dW, p);
+}
+
+// pipeline depth, shared memory and grid of gemm_tc_kernel for the tile shape in p, then the launch
+static int run_tc(TcParams& p, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mc, void* stream, const char* what) {
+    const int bn = p.block_n <= 64 ? 64 : 128;
+    p.dbg = 0;
+    { const char* e = getenv("DFD_DBG"); if (e) p.dbg = atoi(e); }
+    const int stage_bytes = BLOCK_M * BLOCK_K * 2 + bn * BLOCK_K * 2;
+    const int fixed = 2 * BLOCK_M * SLAB * 2 + 16 * 8 + 2 * 4 * 64 * 4 + 1024 /* alignment slack */;
+    int stages = (SMEM_BUDGET - fixed) / stage_bytes;
+    if (stages > 6) stages = 6;
+    if (stages < 2) return dfd_set_error(DFD_ERR_UNSUPPORTED, what);
+    p.stages = stages;
+    const size_t smem = (size_t)stages * stage_bytes + fixed;
+    int device = 0, sms = DFD_SMS;
+    cudaGetDevice(&device);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    int grid = p.num_m_tiles * p.num_n_tiles;
+    if (grid > sms) grid = sms;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (p.is_bf16) {
+        if (bn == 64) launch_tc_kernel<bf16, 64>(grid, smem, st, ma, mb, mc, p);
+        else launch_tc_kernel<bf16, 128>(grid, smem, st, ma, mb, mc, p);
+    } else {
+        if (bn == 64) launch_tc_kernel<__half, 64>(grid, smem, st, ma, mb, mc, p);
+        else launch_tc_kernel<__half, 128>(grid, smem, st, ma, mb, mc, p);
+    }
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
 // Implicit-GEMM convolution on the kernel above (conv mode): y[N,H,W,Cout] = conv_{k x k, stride 1, pad (k-1)/2}(x[N,H,W,Cin]),
 // wpk = packed weight [Cout][kh][kw][Cin] (K-major rows of k*k*Cin). Cin % 64 == 0 keeps every 64-channel K block inside one tap.
 struct ConvTaps { int n, ox[9], oy[9], kidx[9]; };
@@ -739,40 +749,12 @@ static int launch_conv_tc(const void* x, const void* wpk, void* y, int N, int Hi
     p.num_n_tiles = cdiv(Cout, p.block_n);
     p.num_k_blocks = (taps ? taps->n : k * k) * p.cv_cpb;
     p.dsum = dsum; p.dsq = dsq;
-    { const char* e = getenv("DFD_DBG"); p.dbg = e ? atoi(e) : 0; }
-    p.ts = nullptr;
-    const int a_bytes = BLOCK_M * BLOCK_K * 2;
-    const int b_stride = ((p.block_n * BLOCK_K * 2) + 1023) & ~1023;
-    const int fixed = 4 * BLOCK_M * SLAB * 2 + 22 * 8 + 2 * 4 * 64 * 4 + 1024;
-    int stages = (SMEM_BUDGET - fixed) / (a_bytes + b_stride);
-    if (stages > 6) stages = 6;
-    if (stages < 2) return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_conv_tc: smem");
-    p.stages = stages;
-    size_t smem = (size_t)stages * (a_bytes + b_stride) + fixed;
     CUtensorMap ma, mb, mc;
     int rc;
     if ((rc = make_map_nhwc(&ma, x, N, Hin, Win, Cin, TW, TH, TN, p.is_bf16, S))) return rc;
     if ((rc = make_map(&mb, wpk, Cout, K, p.block_n, p.is_bf16))) return rc;
     if ((rc = make_map_nhwc(&mc, y, N, H, W, Cout, TW, TH, TN, p.is_bf16, 1, out_view))) return rc;
-    int device = 0, sms = 148;
-    cudaGetDevice(&device);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-    int grid = p.num_m_tiles * p.num_n_tiles;
-    if (grid > sms) grid = sms;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (p.is_bf16) {
-        auto kf = gemm_tc_kernel<bf16>;
-        static bool attr = false;
-        if (!attr) { cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BUDGET); attr = true; }
-        kf<<<grid, NUM_THREADS, smem, st>>>(ma, mb, mc, p);
-    } else {
-        auto kf = gemm_tc_kernel<__half>;
-        static bool attr = false;
-        if (!attr) { cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BUDGET); attr = true; }
-        kf<<<grid, NUM_THREADS, smem, st>>>(ma, mb, mc, p);
-    }
-    DFD_LAUNCH_CHECK();
-    return DFD_OK;
+    return run_tc(p, ma, mb, mc, stream, "dfd_conv_tc: smem");
 }
 
 // C[M,N] = A[M,K] * B[N,K]^T; statistics of output column c go to channel c % stat_n
@@ -789,59 +771,12 @@ static int launch_gemm_tc(const void* A, const void* B, void* C, long long M, in
     p.num_n_tiles = cdiv(N, p.block_n);
     p.num_k_blocks = cdiv(K, BLOCK_K);
     p.dsum = dsum; p.dsq = dsq;
-    { const char* e = getenv("DFD_DBG"); p.dbg = e ? atoi(e) : 0; }
-    p.ts = nullptr;
-    static long long* ts_buf = nullptr;
-    const bool trace = getenv("DFD_TS") != nullptr;
-    if (trace) { if (!ts_buf) cudaMalloc(&ts_buf, 32 * 8 * sizeof(long long)); cudaMemset(ts_buf, 0, 32 * 8 * sizeof(long long)); p.ts = ts_buf; }
-    const int a_bytes = BLOCK_M * BLOCK_K * 2;
-    const int b_stride = ((p.block_n * BLOCK_K * 2) + 1023) & ~1023;
-    const int fixed = 4 * BLOCK_M * SLAB * 2 + 22 * 8 + 2 * 4 * 64 * 4 + 1024 /* alignment slack */;
-    int stages = (SMEM_BUDGET - fixed) / (a_bytes + b_stride);
-    if (stages > 6) stages = 6;
-    if (stages < 2) return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_gemm_tn: smem");
-    p.stages = stages;
-    size_t smem = (size_t)stages * (a_bytes + b_stride) + fixed;
-
     CUtensorMap ma, mb, mc;
     int rc;
     if ((rc = make_map(&ma, A, M, K, BLOCK_M, p.is_bf16))) return rc;
     if ((rc = make_map(&mb, B, N, K, p.block_n, p.is_bf16))) return rc;
     if ((rc = make_map(&mc, C, M, N, BLOCK_M, p.is_bf16))) return rc;
-
-    int device = 0, sms = 148;
-    cudaGetDevice(&device);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-    int grid = p.num_m_tiles * p.num_n_tiles;
-    if (grid > sms) grid = sms;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (p.is_bf16) {
-        auto kf = gemm_tc_kernel<bf16>;
-        static bool attr = false;
-        if (!attr) { cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BUDGET); attr = true; }
-        kf<<<grid, NUM_THREADS, smem, st>>>(ma, mb, mc, p);
-    } else {
-        auto kf = gemm_tc_kernel<__half>;
-        static bool attr = false;
-        if (!attr) { cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BUDGET); attr = true; }
-        kf<<<grid, NUM_THREADS, smem, st>>>(ma, mb, mc, p);
-    }
-    DFD_LAUNCH_CHECK();
-    if (trace) {
-        // diagnostics only: synchronous dump of CTA 0's pipeline timestamps (cycles relative to its first event)
-        long long h[32 * 8];
-        cudaDeviceSynchronize();
-        cudaMemcpy(h, ts_buf, sizeof(h), cudaMemcpyDeviceToHost);
-        long long t0 = h[0];
-        fprintf(stderr, "gemm_tc trace M=%d N=%d K=%d block_n=%d stages=%d: tile | prod_go mma_acc_free mma_data mma_commit | epi_wait epi_go epi_ld epi_end\n",
-                M, N, K, p.block_n, p.stages);
-        for (int t = 0; t < 32 && h[t * 8 + 1]; t++) {
-            fprintf(stderr, "  %2d |", t);
-            for (int j = 0; j < 8; j++) fprintf(stderr, " %7lld%s", h[t * 8 + j] - t0, j == 3 ? " |" : "");
-            fprintf(stderr, "\n");
-        }
-    }
-    return DFD_OK;
+    return run_tc(p, ma, mb, mc, stream, "dfd_gemm_tn: smem");
 }
 
 #define DISPATCH_16(dt, ...)                                          \
@@ -866,7 +801,7 @@ __global__ void blockdiag_kernel(const BlockDiagDesc* __restrict__ table) {
 
 extern "C" {
 
-// C[M,N] = A[M,K] * B[N,K]^T on tcgen05; optional fp64 column statistics of the stored C ([8][N] slots).
+// C[M,N] = A[M,K] * B[N,K]^T on wgmma; optional fp64 column statistics of the stored C ([8][N] slots).
 // All pointers must be 16-byte aligned, K % 8 == 0 and N % 8 == 0 (TMA global strides are multiples of 16 B).
 int dfd_gemm_tn(const void* A, const void* B, void* C, long long M, int N, int K, int dt, double* dsum, double* dsq,
                 const void* fin, void* stream) {
@@ -888,7 +823,7 @@ int dfd_gemm_tn_rowpack(const void* A, const void* Bd, void* C, long long M, int
     return launch_gemm_tc(A, Bd, C, M / pack, N * pack, K * pack, dt, dsum, dsq, N, fin, stream);
 }
 
-// Dense k x k convolution (stride 1, padding (k-1)/2) as an IMPLICIT GEMM on tcgen05: no im2col matrix exists in memory - the
+// Dense k x k convolution (stride 1, padding (k-1)/2) as an IMPLICIT GEMM on wgmma: no im2col matrix exists in memory - the
 // TMA producer fetches, per tap and 64-channel block, the input box shifted by the tap through a 4-D tensor map over the NHWC
 // tensor (out-of-bounds rows arrive as zeros = the padding) straight into the swizzled MMA operand buffer.
 //   forward : x = input,  wpk = [Cout][kh][kw][Cin]                      (resnet.py:129-136,195-197: nn.Conv2d 3x3)
@@ -964,7 +899,7 @@ int dfd_blockdiag_weights(const void* table, int count, int dt, void* stream) {
     return DFD_OK;
 }
 
-// dW[Nw,Kw] (fp32, accumulated) += G[M,Nw]^T * X[M,Kw] on tcgen05 (MN-major operands straight from NHWC, split over M)
+// dW[Nw,Kw] (fp32, accumulated) += G[M,Nw]^T * X[M,Kw] on wgmma (MN-major operands straight from NHWC, split over M)
 // split count of the workspace (order-deterministic) mode: as many row ranges as fill the GPU once, but no more than keep
 // the partial-sum traffic (one write + one read of splits x Nw x Kw floats) under half of the operand traffic
 static long long wgrad_ws_splits(long long M, int Nw, int Kw, int sms, long long kblocks = 0) {
@@ -984,7 +919,7 @@ static long long wgrad_ws_splits(long long M, int Nw, int Kw, int sms, long long
 // number of partial matrices [Nw, Kw] dfd_gemm_wgrad writes into its workspace for this shape (workspace bytes = that x Nw x Kw x 4)
 int dfd_gemm_wgrad_splits(long long M, int Nw, int Kw) {
     if (M <= 0 || Nw <= 0 || Kw <= 0) return 0;
-    return (int)wgrad_ws_splits(M, Nw, Kw, 148);
+    return (int)wgrad_ws_splits(M, Nw, Kw, DFD_SMS);
 }
 
 // patch (TW x TH x TN <= 64 output pixels) of one pipeline stage of the implicit-GEMM weight gradient: the shape that covers
@@ -1021,7 +956,7 @@ int dfd_conv_wgrad_splits(int N, int H, int W, int Cin, int Cout, int k, int str
     if (N <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0 || stride <= 0) return 0;
     const int Ho = conv_out_extent(H, k, stride), Wo = conv_out_extent(W, k, stride);
     WgPatch pt = wg_patch(N, Ho, Wo);
-    return (int)wgrad_ws_splits((long long)N * Ho * Wo, Cout, k * k * Cin, 148, pt.patches);
+    return (int)wgrad_ws_splits((long long)N * Ho * Wo, Cout, k * k * Cin, DFD_SMS, pt.patches);
 }
 
 int dfd_conv_wgrad_tc(const void* dy, const void* x, float* dW, int N, int H, int W, int Cin, int Cout, int k, int stride, int dt,
@@ -1052,7 +987,7 @@ static int launch_wgrad_tc(const void* G, const void* X, float* dW, long long M,
         p.kblocks = pt.patches;
     }
     const int tm = cdiv(Nw, 128), tn = cdiv(Kw, p.block_n);
-    int device = 0, sms = 148;
+    int device = 0, sms = DFD_SMS;
     cudaGetDevice(&device);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     long long splits = (2LL * sms + tm * tn - 1) / (tm * tn);
@@ -1062,7 +997,7 @@ static int launch_wgrad_tc(const void* G, const void* X, float* dW, long long M,
     if (splits > 65535) splits = 65535;
     p.part = nullptr;
     if (ws) {
-        splits = wgrad_ws_splits(M, Nw, Kw, 148, p.conv ? p.kblocks : 0);
+        splits = wgrad_ws_splits(M, Nw, Kw, DFD_SMS, p.conv ? p.kblocks : 0);
         if (splits * (long long)Nw * Kw * 4 > ws_bytes)
             return dfd_set_error(DFD_ERR_ARG, "dfd_gemm_wgrad: workspace too small (dfd_gemm_wgrad_splits x Nw x Kw floats)");
         p.part = (float*)ws;
@@ -1071,8 +1006,8 @@ static int launch_wgrad_tc(const void* G, const void* X, float* dW, long long M,
     splits = (p.kblocks + p.kb_per_split - 1) / p.kb_per_split;
     const int nbox_b = p.block_n > 64 ? 2 : 1;
     const int stage_bytes = (2 + nbox_b) * WG_BOX_BYTES;
-    const int fixed = 18 * 8 + 64 + 1024;
-    // ~100 KB per CTA: two CTAs (128 TMEM columns each) share an SM, so 2 x SMs splits run as one wave
+    const int fixed = 16 * 8 + 1024;
+    // ~100 KB per CTA: two CTAs share an SM, so 2 x SMs splits run as one wave
     int stages = (100 * 1024 - fixed) / stage_bytes;
     if (stages > 6) stages = 6;
     if (stages < 2) stages = 2;
@@ -1090,15 +1025,11 @@ static int launch_wgrad_tc(const void* G, const void* X, float* dW, long long M,
     dim3 grid(tm, tn, (unsigned)splits);
     cudaStream_t st = (cudaStream_t)stream;
     if (p.is_bf16) {
-        auto kf = wgrad_tc_kernel<bf16>;
-        static bool attr = false;
-        if (!attr) { cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); attr = true; }
-        kf<<<grid, 256, smem, st>>>(mg, mx, dW, p);
+        if (nbox_b == 1) launch_wgrad_kernel<bf16, 64>(grid, smem, st, mg, mx, dW, p);
+        else launch_wgrad_kernel<bf16, 128>(grid, smem, st, mg, mx, dW, p);
     } else {
-        auto kf = wgrad_tc_kernel<__half>;
-        static bool attr = false;
-        if (!attr) { cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); attr = true; }
-        kf<<<grid, 256, smem, st>>>(mg, mx, dW, p);
+        if (nbox_b == 1) launch_wgrad_kernel<__half, 64>(grid, smem, st, mg, mx, dW, p);
+        else launch_wgrad_kernel<__half, 128>(grid, smem, st, mg, mx, dW, p);
     }
     DFD_LAUNCH_CHECK();
     return DFD_OK;

@@ -45,7 +45,7 @@ __device__ __forceinline__ float softplus_precise(float x) {
 // ---------------------------------------------------------------------------------------------
 // SE excite: gate[n,:] = sigmoid(We * swish(Wr * pooled[n,:] + br) + be).  A CTA handles IMG images: every weight element
 // is fetched once per CTA and used for IMG images (with one image per CTA the 256 CTAs of a batch re-read both weight
-// matrices - 113 MB of L2 traffic for the 1152-channel layers, which is what bounded this kernel at ~20 us).  The arithmetic
+// matrices - 113 MB of L2 traffic for the 1152-channel layers, which bounds the kernel).  The arithmetic
 // order per image does not depend on IMG.
 // ---------------------------------------------------------------------------------------------
 template <int IMG>
@@ -318,7 +318,7 @@ __global__ void head_dgrad_kernel(const float* __restrict__ dlogits, const float
     dpooled[idx] = s;
 }
 // dW[k,f] += sum_n dlogits[n,k] pooled[n,f]; db[k] += sum_n dlogits[n,k]; the batch is split over blockIdx.y
-// (a single thread walking all N images serialises N dependent L2 round trips: measured 100 us at N = 256)
+// (a single thread walking all N images serialises N dependent L2 round trips)
 __global__ void head_wgrad_kernel(const float* __restrict__ dlogits, const float* __restrict__ pooled,
                                   float* __restrict__ dW, float* __restrict__ db, int N, int F, int K) {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -526,23 +526,22 @@ __global__ void transpose_weights_kernel(const TransposeDesc* __restrict__ table
     }
 }
 
-// The per-image FC chains are latency-bound (ncu: 8 % issue utilisation, long-scoreboard stalls, 0.2 waves): the only
+// The per-image FC chains are latency-bound (low issue utilisation, long-scoreboard stalls, a fraction of a wave): the only
 // lever is a shorter dependent chain per warp, i.e. more warps per image for the wide layers.
 static int se_threads(int C) { return C >= 768 ? 1024 : (C >= 384 ? 512 : 256); }
 
 static int flat_blocks(size_t n) {
     size_t b = (n + 255) / 256;
-    if (b > 148 * 8) b = 148 * 8;
+    if (b > DFD_SMS * 8) b = DFD_SMS * 8;
     if (b < 1) b = 1;
     return (int)b;
 }
 
-// images per CTA of the SE FC kernels. Several images per CTA fetch every weight element once for all of them, but
-// MEASURED (B0, batch 256): 4 images per CTA are 12 % slower than 1 (0.80 vs 0.69 ms over the 16 backward launches) - the
-// kernels are bound by the dependent FC chain of a CTA, which gets longer, not by the L2 traffic of the weights. So: one
-// image per CTA until the batch is so large that the grid exceeds a few waves - EXCEPT for the widest layers, where the
-// weight traffic does bound the kernel (1152 x 48: 2 x 221 KB per CTA; per layer, weights L2-resident: forward 43 / 31 / 37 us
-// and backward + wgrad 98 / 77 / 82 us for 1 / 2 / 4 images per CTA; 672 x 28 and below: 1 is best).
+// images per CTA of the SE FC kernels. Several images per CTA fetch every weight element once for all of them, but 4 images
+// per CTA were slower than 1 on the GPU this code was first tuned on (not re-measured on the H100) - the kernels are bound by the dependent FC chain of a
+// CTA, which gets longer, not by the L2 traffic of the weights. So: one image per CTA until the batch is so large that the
+// grid exceeds a few waves - EXCEPT for the widest layers, where the weight traffic does bound the kernel (1152 x 48:
+// 2 x 221 KB per CTA; 2 images per CTA were best there, 1 for 672 x 28 and below).
 static int se_img(int N, int C, int Cse, size_t floats_per_image, size_t fixed_floats) {
     int img = N >= 2048 ? 4 : (N >= 1024 ? 2 : 1);
     if (img < 2 && N >= 128 && (long long)C * Cse >= 32768) img = 2;

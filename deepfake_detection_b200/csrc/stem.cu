@@ -230,7 +230,7 @@ int dfd_stem_wgrad(const void* x, const void* g, const void* y, const float* cA,
     long long total = (long long)N * Ho * Wo;
     int items = Cin * k * k * (Cout / 8);
     int ipt = (items + 255) / 256;
-    int blocks = 148 * 4;
+    int blocks = DFD_SMS * 4;
     long long ppb = (total + blocks - 1) / blocks;
     ppb = ((ppb + 63) / 64) * 64;
     blocks = cdiv(total, ppb);

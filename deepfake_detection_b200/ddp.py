@@ -83,7 +83,8 @@ class GradReducer:
         # bucket_mb: the arena is cut greedily in backward order. Parameters concentrate in the LAST layers (EfficientNet-B0:
         # 11.6 of 16 MB sit in the head and stages 5-6), so 4 MB buckets start reducing early and leave ~2.6 MB (stages 1-4
         # and the stem) for the one collective that cannot overlap with anything - the final one. 1 MB buckets (12
-        # collectives) measured WORSE at 2 GPUs (17.03 vs 16.64 ms: NCCL CTAs compete with the memory-bound kernels)
+        # collectives) were slower at 2 GPUs, NCCL CTAs competing with the memory-bound kernels (measured on the GPU this
+        # code was first tuned on, not re-measured on the H100)
         self.engine = engine                      # default plan (Trainer) or the arena (NativeDDP)
         self.arena = engine.arena
         self.group = group

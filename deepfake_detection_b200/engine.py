@@ -1,4 +1,4 @@
-"""Native train / validate engine: lays the network out in HBM and drives the sm_100a kernels.
+"""Native train / validate engine: lays the network out in HBM and drives the sm_90a kernels.
 
 This is the host side of the hot path (dfd/runners/train.py:610-649): given an architecture spec it
   * owns the flat fp32 parameter / gradient arenas (reference tensor names, OIHW shapes) plus their 16-bit
@@ -42,7 +42,7 @@ class Engine:
         if self._plan_only:
             device = "cpu"
         elif not torch.cuda.is_available():
-            raise _lib.NativeError("deepfake_detection_b200.Engine needs a CUDA device (B200, sm_100a); "
+            raise _lib.NativeError("deepfake_detection_b200.Engine needs a CUDA device (H100, sm_90a); "
                                    "there is no CPU path")
         self.L = _lib.lib()
         self.spec = spec = get_spec(arch, num_classes=num_classes, in_chans=in_chans)
@@ -71,7 +71,7 @@ class Engine:
         self.bn_momentum = float(bn_momentum)
         self.bn_eps = float(bn_eps)
         self.gemm_impl = gemm_impl
-        # 1x1 weight gradient: tcgen05 with MN-major operands, or the mma.sync cross-check path
+        # 1x1 weight gradient: wgmma with MN-major operands, or the mma.sync cross-check path
         self._wgrad_name = "dfd_gemm_wgrad" if gemm_impl == "tc" and not os.environ.get("DFD_WGRAD_MMA") else "dfd_gemm_wgrad_mma"
         self.stem_impl = stem_impl
         self.training = True
@@ -223,7 +223,7 @@ class Engine:
     # plan construction
     # ------------------------------------------------------------------------------------------
     # ---- order-deterministic weight gradients ------------------------------------------------------------------
-    # The tcgen05 weight gradient and the fused depthwise backward run in WORKSPACE mode: every CTA stores its split partial
+    # The tensor-core weight gradient and the fused depthwise backward run in WORKSPACE mode: every CTA stores its split partial
     # sum in a fixed slot of one workspace (plain stores, no atomics) and `dfd_ordered_reduce` - one table-driven launch per
     # block of the network, right behind that block's backward ops - adds the partials into the gradient arena in slot
     # order. Gradients (and with them every later step) therefore do not depend on the arrival order of CTAs; the reduce
@@ -304,8 +304,8 @@ class Engine:
         self._keep.append(t)
         return t
 
-    # rows of A fused per TMA row for small-K pointwise convs, measured on B200 at batch 256 (tools/gemm_time2.py): the best
-    # factor makes pack*K a multiple of the 64-element k-block where that keeps pack*N modest
+    # rows of A fused per TMA row for small-K pointwise convs (tools/gemm_time2.py times the choices): the factor makes
+    # pack*K a multiple of the 64-element k-block where that keeps pack*N modest
     _ROW_PACK = {8: 8, 16: 4, 24: 8, 32: 4, 40: 2, 48: 4, 56: 2}
 
     @classmethod
@@ -367,7 +367,7 @@ class Engine:
         o._derived_dirty = False
 
     def _stem_gemm_setup(self, wname, Cout, k, M):
-        """stem convolution as im2col + tcgen05 GEMM (K = Cin*k*k padded to a multiple of 8)"""
+        """stem convolution as im2col + tensor-core GEMM (K = Cin*k*k padded to a multiple of 8)"""
         taps = self.spec.in_chans * k * k
         Kp = (taps + 7) // 8 * 8
         o = self.arena
@@ -459,13 +459,11 @@ class Engine:
         mom, eps = self.bn_momentum, self.bn_eps
 
         # BatchNorm finalisation by the last CTA of the statistics-producing kernel (descriptors, csrc/bn_finalize.cuh) instead of
-        # 98 one-block launches: implemented and tested, but MEASURED SLOWER inside the captured graph (17.29 vs 16.69 ms per
-        # B0 step): every CTA pays a __threadfence + a same-address ticket atomic before it may retire (the depthwise kernels
-        # run ~14k short CTAs), and the one finalising CTA walks C channels with a fraction of the threads of the standalone
-        # launch. Off unless DFD_FUSED_FINALIZE=1.
-        # DFD_FUSED_FINALIZE=gemm: only the BatchNorms whose statistics come from the persistent tcgen05 GEMM (148 CTAs: the
-        # ticket is free there) are finalised by their producer - MEASURED slower too (15.38 vs 15.30 ms: one CTA finalising C
-        # channels is a longer dependent chain than the standalone launch); =1: every producer, forward and backward.
+        # 98 one-block launches: implemented and tested, but off by default: every CTA pays a __threadfence + a same-address
+        # ticket atomic before it may retire (the depthwise kernels run ~14k short CTAs), and the one finalising CTA walks C
+        # channels with a fraction of the threads of the standalone launch. Off unless DFD_FUSED_FINALIZE=1.
+        # DFD_FUSED_FINALIZE=gemm: only the BatchNorms whose statistics come from the persistent tensor-core GEMM (one CTA per
+        # SM: the ticket is free there) are finalised by their producer; =1: every producer, forward and backward.
         ff_mode = os.environ.get("DFD_FUSED_FINALIZE", "")
         fused_fin = ff_mode not in ("", "0", "gemm") and not self.sync_bn
         fused_gemm = (fused_fin or ff_mode == "gemm") and not self.sync_bn
@@ -587,8 +585,9 @@ class Engine:
                 rec.update(pooled=pooled, gate=gate)
                 if os.environ.get("DFD_SE_FUSED"):
                     # squeeze + excite in ONE launch (the CTA that completes an image's pooled vector runs its FC chain):
-                    # measured SLOWER than the two launches (+0.2 ms per step: a 256-thread CTA walks the latency-bound chain
-                    # four times longer than the 1024-thread FC kernel and the tail is not hidden); kept selectable
+                    # slower than the two launches on the GPU this code was first tuned on (not re-measured on the H100):
+                    # a 256-thread CTA walks the latency-bound chain four times longer than the 1024-thread FC kernel and
+                    # the tail is not hidden; kept selectable
                     fwd.append(("dfd_pool_se", (_ptr(y2), bn_mid.scale, bn_mid.shift, _ptr(pooled), P32(p + ".se.conv_reduce.weight"),
                                                 P32(p + ".se.conv_reduce.bias"), P32(p + ".se.conv_expand.weight"),
                                                 P32(p + ".se.conv_expand.bias"), _ptr(gate), N, ho * wo, b.cmid, b.cse, ACT_SWISH, dt,

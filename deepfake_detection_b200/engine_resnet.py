@@ -3,12 +3,12 @@
 Reference graph: dfd/timm/models/resnet.py:450-468 (stem 7x7 s2 -> BN -> ReLU -> maxpool 3x3 s2 -> 4 stages -> GAP
 -> fc), BasicBlock :150-175, Bottleneck :215-246 (stride on the 3x3, :195-197), downsample 1x1 conv + BN :249-260.
 
-Dense 3x3 convolutions with stride 1 (13 of the 16 in resnet50, all but 3 in resnet18) run as IMPLICIT GEMMs on tcgen05
+Dense 3x3 convolutions with stride 1 (13 of the 16 in resnet50, all but 3 in resnet18) run as IMPLICIT GEMMs on wgmma
 (`dfd_conv_tc`, csrc/gemm_tc.cu conv mode: the TMA producer fetches the input box shifted by the tap through a 4-D tensor
 map, no im2col matrix in memory) in the forward pass and for the input gradient (same kernel on dY with the tap-flipped
 [Cin][kh'][kw'][Cout] weights). The strided 3x3 convolutions keep the round-1 formulation (csrc/conv_dense.cu):
-materialised im2col -> tcgen05 GEMM (forward), GEMM -> col2im (input gradient). The weight gradient of every 3x3 is the
-MN-major tcgen05 wgrad GEMM, implicit too (`dfd_conv_wgrad_tc`: one pipeline stage = one patch of <= 64 output pixels of dY
+materialised im2col -> tensor-core GEMM (forward), GEMM -> col2im (input gradient). The weight gradient of every 3x3 is the
+MN-major wgmma wgrad GEMM, implicit too (`dfd_conv_wgrad_tc`: one pipeline stage = one patch of <= 64 output pixels of dY
 and the input box shifted by the tap). Stride-2 convolutions (the three strided 3x3 and the strided 1x1 downsample inputs) use
 the same kernels with TMA element strides {1, 2, 2, 1} in the forward pass and the weight gradient; the input gradient of a
 strided 3x3 is four parity-class implicit GEMMs (`dfd_conv_dgrad_s2_tc`) storing through strided views of dx. Only the strided
@@ -88,7 +88,7 @@ def build_resnet(e):
     e._alloc_bn(bn_specs)
     bns = e.bns
 
-    fused_fin = os.environ.get("DFD_FUSED_FINALIZE", "") not in ("", "0", "gemm")   # measured slower than the standalone launches, see engine.py
+    fused_fin = os.environ.get("DFD_FUSED_FINALIZE", "") not in ("", "0", "gemm")   # off by default, see engine.py
 
     def gemm(A, B, C, M, Nn, K, bn=None):
         fs, fq = (bn.fsum, bn.fsq) if bn is not None else (None, None)

@@ -1,4 +1,4 @@
-/* dfd_b200.h — C ABI of libdfd_b200.so: the sm_100a device kernels behind the data-parallel train / validate
+/* dfd_b200.h — C ABI of libdfd_b200.so: the sm_90a (H100) device kernels behind the data-parallel train / validate
  * step of TARTRL/Deepfake_Detection (dfd/runners/train.py:610-649, :713-746).
  *
  * The reference has NO native/FFI layer (SURVEY.md section 2.1): every entry point below replaces a stock
@@ -44,7 +44,7 @@ int dfd_memset_async(void* p, int value, long long bytes, void* stream);
 
 /* ---- pointwise (1x1) convolution: nn.Conv2d via create_conv2d, efficientnet_blocks.py:165,277,299,
  *      efficientnet.py:292, resnet.py:192,199 -------------------------------------------------------- */
-/* C[M,N] = A[M,K] * B[N,K]^T on tcgen05 (TMA in/out, TMEM accumulators). Forward: A = input [N*H*W, Cin],
+/* C[M,N] = A[M,K] * B[N,K]^T on wgmma (TMA in/out, accumulators in registers). Forward: A = input [N*H*W, Cin],
  * B = weight [Cout, Cin]. Input gradient: A = dY [N*H*W, Cout], B = weight^T [Cin, Cout].
  * dsum/dsq (optional): per-column sum / sum of squares of the stored C for the following BatchNorm. */
 int dfd_gemm_tn(const void* A, const void* B, void* C, long long M, int N, int K, int dt, double* dsum, double* dsq,
@@ -65,8 +65,8 @@ int dfd_gemm_tn_mma(const void* A, const void* B, void* C, const void* add, long
                     double* dsum, double* dsq, void* stream);
 /* weight gradient dW[Nw,Kw] (fp32, accumulated) += G[M,Nw]^T * X[M,Kw]  (autograd of the conv, train.py:634) */
 int dfd_gemm_wgrad_mma(const void* G, const void* X, float* dW, long long M, int Nw, int Kw, int dt, void* stream);
-/* the same contract on tcgen05: both operands MN-major straight from NHWC memory (TMA 128-byte swizzle boxes), fp32
- * accumulator in TMEM over a contiguous range of rows per CTA, one red.global.add flush */
+/* the same contract on wgmma: both operands MN-major straight from NHWC memory (TMA 128-byte swizzle boxes), fp32
+ * accumulators in registers over a contiguous range of rows per CTA, one red.global.add flush */
 int dfd_gemm_wgrad(const void* G, const void* X, float* dW, long long M, int Nw, int Kw, int dt, void* ws, long long ws_bytes,
                    void* stream);
 /* ws (optional): ORDER-DETERMINISTIC mode - split z stores its fp32 partial matrix at ws[z][Nw][Kw] with plain stores, dW is
@@ -132,7 +132,7 @@ int dfd_col2im(const void* dcols, const void* add, void* dx, int N, int H, int W
 /* table: device array of { const void* src_OIHW16; void* dst_OHWI16; void* dstT_HWI_O16; void* dstD_IH'W'O16 (flipped taps);
  *                          int O; int I; int k; int pad; }  - dstT / dstD may be null */
 int dfd_repack_weights(const void* table, int count, int dt, void* stream);
-/* Dense k x k convolution, stride 1, padding (k-1)/2, as an IMPLICIT GEMM on tcgen05 (no im2col matrix in memory): the TMA
+/* Dense k x k convolution, stride 1, padding (k-1)/2, as an IMPLICIT GEMM on wgmma (no im2col matrix in memory): the TMA
  * producer loads, per tap and 64-channel block, the NHWC input box shifted by the tap through a 4-D tensor map; out-of-image
  * rows arrive as zeros (= the padding). Replaces nn.Conv2d 3x3 stride 1 of BasicBlock / Bottleneck (resnet.py:129-136,195-197):
  *   forward: x = input [N,H,W,Cin],  wpk = dst_OHWI16,             y [N,H,W,Cout]; dsum/dsq = BatchNorm statistics of y
@@ -142,7 +142,7 @@ int dfd_repack_weights(const void* table, int count, int dt, void* stream);
  * stride 2 is the strided 1x1 downsample convolution (resnet.py:249-260) without its gather. */
 int dfd_conv_tc(const void* x, const void* wpk, void* y, int N, int H, int W, int Cin, int Cout, int k, int stride, int dt,
                 double* dsum, double* dsq, const void* fin, void* stream);
-/* Weight gradient of the same convolution, also an implicit GEMM (MN-major tcgen05 operands straight from the NHWC tensors,
+/* Weight gradient of the same convolution, also an implicit GEMM (MN-major wgmma operands straight from the NHWC tensors,
  * one pipeline stage = one patch of <= 64 output pixels, its input box shifted by the tap): dW_OHWI fp32 [Cout][kh][kw][Cin]
  * += sum_pixels dY[pixel, co] * x[pixel + tap, ci]. `ws` / `ws_bytes` as for dfd_gemm_wgrad: when given, the split partials
  * (dfd_conv_wgrad_splits x Cout x k*k*Cin floats) are written there for dfd_ordered_reduce and dW is left alone. */

@@ -608,7 +608,7 @@ def check_transpose(dtype=torch.bfloat16):
 
 
 def check_conv_dense(N, H, W, Cin, Cout, k, s, dtype=torch.bfloat16, seed=0):
-    """k x k dense conv = im2col + tcgen05 GEMM; dgrad = GEMM + col2im; wgrad = mma GEMM on im2col + unpack, vs F.conv2d."""
+    """k x k dense conv = im2col + tensor-core GEMM; dgrad = GEMM + col2im; wgrad = mma GEMM on im2col + unpack, vs F.conv2d."""
     import struct
     g = torch.Generator(device="cuda").manual_seed(seed)
     pad = (k - 1) // 2

@@ -135,7 +135,7 @@ def test_fp16_dynamic_loss_scaling():
 
 def test_train_step_is_run_to_run_deterministic():
     """Two independent engines, same weights and batch: bit-identical logits, loss AND gradients.  Weight gradients are
-    flushed through fixed-slot partials added in a fixed order (tcgen05 wgrad, fused depthwise backward, SE / classifier
+    flushed through fixed-slot partials added in a fixed order (tensor-core wgrad, fused depthwise backward, SE / classifier
     parameter gradients, the loss), never through fp32 atomics.  The one order-dependent accumulation left is the fp64 BN
     statistic (8 interleaved slots): its order effect is 2^-53 relative, i.e. a different fp32 mean / rstd with probability
     ~2^-29 per channel - about 5e-5 per step for this network (documented in DESIGN.md section 4)."""

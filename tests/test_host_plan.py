@@ -89,7 +89,7 @@ def test_row_pack_rule():
 
 def test_plan_uses_the_fused_and_packed_kernels():
     """EfficientNet-B0 plan: every expansion block's depthwise backward is ONE fused launch, small-K pointwise convs go
-    through the row-packed GEMM with block-diagonal weights registered for refresh, weight gradients use tcgen05."""
+    through the row-packed GEMM with block-diagonal weights registered for refresh, weight gradients use the tensor-core kernel."""
     from deepfake_detection_b200.engine import Engine
     eng = Engine("efficientnet_b0", 4, 224, 224, device="plan-only")
     names_f = [op[1] for op in eng.fwd_ops]

@@ -52,7 +52,7 @@ def test_wgrad(M, Nw, Kw):
 @pytest.mark.parametrize("M,Nw,Kw", [(5000, 96, 16), (12345, 144, 24), (3000, 1152, 192), (777, 320, 1280), (64, 24, 144),
                                      (50176, 672, 112), (130, 40, 240), (4096, 128, 128), (70, 8, 8)])
 def test_wgrad_tcgen05(M, Nw, Kw):
-    """MN-major tcgen05 weight gradient (operands straight from NHWC rows) against fp64"""
+    """MN-major wgmma weight gradient (operands straight from NHWC rows) against fp64"""
     assert _gc().check_wgrad(M, Nw, Kw, impl="dfd_gemm_wgrad")["rel"] < 1e-4
 
 

@@ -8,10 +8,10 @@ Tolerances (north_star: 1e-3 rel fp32 / 1e-2 for the 16-bit paths), written once
                                                                             exceeds that, <= 1.5 x yardstick + 5e-3
 The yardstick is the ORACLE ITSELF run in fp32 arithmetic with nothing but its ~100 stored activation tensors rounded to the
 16-bit type (`act_dtype`): its distance from its own fp32 result is what any implementation that keeps activations in that
-type pays before a single kernel differs - the reference under AMP included.  Measured (profiles/r02_parity_full.md):
+type pays before a single kernel differs - the reference under AMP included.  The yardstick (CPU, fp32):
 EfficientNet-B0 256 x 224^2 bf16 1.7e-2 / fp16 2.1e-3; EfficientNet-B4 32 x 380^2 fp16 1.3e-2 (its logits are ~0 at
-loss = ln 2, so a relative error of the logits is ill-conditioned); what the optimizer consumes (loss, updated weights) sits
-at 1e-4 .. 1e-3 in every case and is held to the 1e-2 of north_star without any yardstick.
+loss = ln 2, so a relative error of the logits is ill-conditioned); what the optimizer consumes (loss, updated weights) is
+held to the 1e-2 of north_star without any yardstick.
 """
 import os
 
@@ -110,7 +110,7 @@ def test_efficientnet_b0_config2_256x224(dtype):
 
 def test_efficientnet_b4_config5_380_fp16():
     """BASELINE configs[4]: EfficientNet-B4 fp16 3x380x380 (batch 32 of the 128: the fp32 oracle passes are what bound it;
-    the full batch 128 run is recorded in profiles/r02_parity_full.md)"""
+    the step at batch 32 runs the same kernels as at 128)"""
     r = _native("efficientnet_b4", 32, 380, "fp16")
     bound, yard = _logits_bound("efficientnet_b4", 32, 380, "fp16")
     assert r["loss_rel"] < 1e-2 and r["weights_rel_worst"] < 1e-2 and r["buffers_rel_worst"] < 1e-2, r
@@ -131,7 +131,7 @@ def test_resnet50_config4_224_untamed_synthetic(dtype):
     """The same configuration on the synthetic formula weights AS THEY ARE (gamma ~ 1 on every BN, nothing damped). With all
     16 residual branches at full strength the ReLU network amplifies 16-bit rounding chaotically: the ORACLE ITSELF, fp32
     arithmetic with only its stored activations rounded, moves conv1.weight's update by 0.79 (bf16) / 0.43 (fp16) relative to
-    its own fp32 result (measured, profiles/r02_parity_full.md) - no 16-bit implementation can meet 1e-2 here, the reference
+    its own fp32 result (the oracle on the CPU) - no 16-bit implementation can meet 1e-2 here, the reference
     under AMP included. The statement that CAN be tested: the native path is no further from fp32 than 1.5x that storage
     yardstick (+ 1e-2) on every tensor, on the logits and on the loss."""
     tdt = torch.bfloat16 if dtype == "bf16" else torch.float16

@@ -1,4 +1,4 @@
-"""3x3 stride-1 convolution on the resnet50 layer shapes (batch 256): materialised im2col + tcgen05 GEMM vs the implicit GEMM
+"""3x3 stride-1 convolution on the resnet50 layer shapes (batch 256): materialised im2col + tensor-core GEMM vs the implicit GEMM
 (dfd_conv_tc), forward (+statistics) and input gradient (GEMM + col2im vs implicit on dY)."""
 import os, struct, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,4 +1,4 @@
-"""Diagnostics: plain vs row-packed tcgen05 GEMM on the small-K shapes of EfficientNet-B0 (batch 256)."""
+"""Diagnostics: plain vs row-packed tensor-core GEMM on the small-K shapes of EfficientNet-B0 (batch 256)."""
 import os, sys, struct, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from deepfake_detection_b200 import _lib

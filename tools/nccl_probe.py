@@ -1,4 +1,4 @@
-"""all-reduce (AVG, fp32) time by payload on this box: the numbers behind the DDP overhead in profiles/r02_summary.md.
+"""all-reduce (AVG, fp32) time by payload on this machine.
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 tools/nccl_probe.py"""
 import os, torch, torch.distributed as dist
 lr = int(os.environ["LOCAL_RANK"]); torch.cuda.set_device(lr)

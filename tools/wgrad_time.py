@@ -1,4 +1,4 @@
-"""mma.sync vs tcgen05 1x1 weight gradient on the EfficientNet-B0 layer shapes (batch 256)."""
+"""mma.sync vs wgmma 1x1 weight gradient on the EfficientNet-B0 layer shapes (batch 256)."""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from deepfake_detection_b200 import _lib
