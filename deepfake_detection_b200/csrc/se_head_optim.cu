@@ -1,5 +1,5 @@
-// Small per-image kernels (squeeze-excite FCs, classifier + sigmoid-BCE loss) and the flat-arena
-// optimizer / weight-preparation kernels.
+// Small per-image kernels (squeeze-excite FCs, classifier + softmax-CE loss: sigmoid-BCE for 2 classes, a tiled GEMM and
+// a per-image log-sum-exp pass for any other class count) and the flat-arena optimizer / weight-preparation kernels.
 //
 // Reference semantics restated here:
 //   SqueezeExcite.forward         dfd/timm/models/efficientnet_blocks.py:104-110  (FC+bias, Swish, FC+bias, sigmoid)
@@ -252,9 +252,10 @@ __global__ void se_fc_wgrad_kernel(const float* __restrict__ d_e, const float* _
 }
 
 // ---------------------------------------------------------------------------------------------
-// classifier: logits[n,k] = W[k,:] . pooled[n,:] + b[k]   (one CTA per image, one warp per class round-robin)
+// 2-class classifier: logits[n,k] = W[k,:] . pooled[n,:] + b[k]   (one CTA per image, one warp per class round-robin)
 // fused 2-class loss (sigmoid-BCE on d = z1 - z0 == softmax-CE), top-1, and dL/dlogits.
-// target: int64 hard labels (tgt_i) or float soft targets [N,2] (tgt_f).
+// target: int64 hard labels (tgt_i) or float soft targets [N,2] (tgt_f).  Every other class count: head_gemm_kernel +
+// head_ce_kernel below.
 // ---------------------------------------------------------------------------------------------
 __global__ void head_fwd_kernel(const float* __restrict__ pooled, const float* __restrict__ W,
                                 const float* __restrict__ b, float* __restrict__ logits, int F, int K,
@@ -347,6 +348,229 @@ __global__ void head_wgrad_kernel(const float* __restrict__ dlogits, const float
     }
     dW[idx] += s;
     if (f == 0) db[k] += sb;
+}
+
+// ---------------------------------------------------------------------------------------------
+// K-class head (every K != 2): three fp32 SIMT GEMMs plus a per-image softmax-CE pass.
+//
+// head_gemm_kernel: C[m, c] = (bias[c] +) sum_r A(m, r) B(c, r)   (ACCUM: C[m, c] += sum_r ...)
+//   A(m, r) = A[m * a_m + r * a_r], B(c, r) = B[c * b_c + r * b_r]; A_RC / B_RC: the operand is contiguous along r (else
+//   along m / c), which picks the coalesced load order.  A BK-deep shared-memory tile per step, a register micro-tile of
+//   (BM/16) x (BN/16) outputs per thread (rows ty + 16 i, columns tx + 16 j), the next tile prefetched into registers
+//   while the current one is multiplied.
+//   rowsum (optional): rowsum[m] += sum_r A(m, r), by the CTAs of the first column tile.
+// Every output (and every rowsum) is reduced by ONE thread over r = 0 .. R-1 in ascending order: no split over r, no
+// scratch, no atomics, so the results are bit-reproducible and the problem size is bounded only by int indexing.
+// ---------------------------------------------------------------------------------------------
+constexpr int HG_BK = 16, HG_THREADS = 256;
+
+template <int BM, bool RC, int L>
+__device__ __forceinline__ void head_gemm_load(float (&reg)[L], const float* __restrict__ X, int s_m, int s_r, int m0,
+                                               int M, int r0, int R) {
+#pragma unroll
+    for (int i = 0; i < L; i++) {
+        const int e = threadIdx.x + i * HG_THREADS;
+        const int m = RC ? e / HG_BK : e % BM, r = RC ? e % HG_BK : e / BM;
+        const int gm = m0 + m, gr = r0 + r;
+        reg[i] = (gm < M && gr < R) ? __ldg(X + (size_t)gm * s_m + (size_t)gr * s_r) : 0.f;
+    }
+}
+
+template <int BM, bool RC, int L>
+__device__ __forceinline__ void head_gemm_store(float (*S)[BM + 1], const float (&reg)[L]) {
+#pragma unroll
+    for (int i = 0; i < L; i++) {
+        const int e = threadIdx.x + i * HG_THREADS;
+        const int m = RC ? e / HG_BK : e % BM, r = RC ? e % HG_BK : e / BM;
+        S[r][m] = reg[i];
+    }
+}
+
+template <int BM, int BN, bool A_RC, bool B_RC, bool ACCUM>
+__global__ void __launch_bounds__(HG_THREADS) head_gemm_kernel(const float* __restrict__ A, int a_m, int a_r,
+                                                               const float* __restrict__ B, int b_c, int b_r,
+                                                               float* __restrict__ C, int ldc,
+                                                               const float* __restrict__ bias, float* __restrict__ rowsum,
+                                                               int M, int Nc, int R) {
+    constexpr int TM = BM / 16, TN = BN / 16, LA = BM * HG_BK / HG_THREADS, LB = BN * HG_BK / HG_THREADS;
+    static_assert(BM % 16 == 0 && BN % 16 == 0 && LA * HG_THREADS == BM * HG_BK && LB * HG_THREADS == BN * HG_BK, "tile");
+    __shared__ float As[HG_BK][BM + 1], Bs[HG_BK][BN + 1];
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const int m0 = blockIdx.y * BM, c0 = blockIdx.x * BN;
+    const bool do_rowsum = rowsum != nullptr && blockIdx.x == 0 && tid < BM;
+    float acc[TM][TN];
+#pragma unroll
+    for (int i = 0; i < TM; i++)
+#pragma unroll
+        for (int j = 0; j < TN; j++) acc[i][j] = 0.f;
+    float ra[LA], rb[LB], rs = 0.f;
+    head_gemm_load<BM, A_RC>(ra, A, a_m, a_r, m0, M, 0, R);
+    head_gemm_load<BN, B_RC>(rb, B, b_c, b_r, c0, Nc, 0, R);
+    for (int r0 = 0; r0 < R; r0 += HG_BK) {
+        head_gemm_store<BM, A_RC>(As, ra);
+        head_gemm_store<BN, B_RC>(Bs, rb);
+        __syncthreads();
+        if (r0 + HG_BK < R) {
+            head_gemm_load<BM, A_RC>(ra, A, a_m, a_r, m0, M, r0 + HG_BK, R);
+            head_gemm_load<BN, B_RC>(rb, B, b_c, b_r, c0, Nc, r0 + HG_BK, R);
+        }
+#pragma unroll
+        for (int kk = 0; kk < HG_BK; kk++) {
+            float a[TM], b[TN];
+#pragma unroll
+            for (int i = 0; i < TM; i++) a[i] = As[kk][ty + 16 * i];
+#pragma unroll
+            for (int j = 0; j < TN; j++) b[j] = Bs[kk][tx + 16 * j];
+#pragma unroll
+            for (int i = 0; i < TM; i++)
+#pragma unroll
+                for (int j = 0; j < TN; j++) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+        }
+        if (do_rowsum) {
+#pragma unroll
+            for (int kk = 0; kk < HG_BK; kk++) rs += As[kk][tid];     // the zero padding past R adds nothing
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int i = 0; i < TM; i++) {
+        const int m = m0 + ty + 16 * i;
+        if (m >= M) continue;
+#pragma unroll
+        for (int j = 0; j < TN; j++) {
+            const int c = c0 + tx + 16 * j;
+            if (c >= Nc) continue;
+            float* o = C + (size_t)m * ldc + c;
+            if (ACCUM) *o += acc[i][j];
+            else *o = bias ? acc[i][j] + bias[c] : acc[i][j];
+        }
+    }
+    if (do_rowsum && m0 + tid < M) rowsum[m0 + tid] += rs;
+}
+
+// the head kernels index [N,K], [K,F] and [N,F] with int
+inline bool head_sizes_fit_int(int N, int F, int K) {
+    const long long lim = 0x7fffffffLL;
+    return (long long)N * K <= lim && (long long)K * F <= lim && (long long)N * F <= lim;
+}
+
+// 64x64 tiles once they alone fill the GPU, else 32x32 tiles (4x the CTAs) so that a small output still spreads over the SMs
+template <bool A_RC, bool B_RC, bool ACCUM>
+void head_gemm(const float* A, int a_m, int a_r, const float* B, int b_c, int b_r, float* C, int ldc, const float* bias,
+               float* rowsum, int M, int Nc, int R, cudaStream_t st) {
+    if ((long long)cdiv(M, 64) * cdiv(Nc, 64) >= DFD_SMS)
+        head_gemm_kernel<64, 64, A_RC, B_RC, ACCUM><<<dim3(cdiv(Nc, 64), cdiv(M, 64)), HG_THREADS, 0, st>>>(
+            A, a_m, a_r, B, b_c, b_r, C, ldc, bias, rowsum, M, Nc, R);
+    else
+        head_gemm_kernel<32, 32, A_RC, B_RC, ACCUM><<<dim3(cdiv(Nc, 32), cdiv(M, 32)), HG_THREADS, 0, st>>>(
+            A, a_m, a_r, B, b_c, b_r, C, ldc, bias, rowsum, M, Nc, R);
+}
+
+// Deterministic CTA reductions (fixed shuffle tree, then the warp partials in warp order); every thread gets the result.
+constexpr int HCE_THREADS = 128;
+
+__device__ __forceinline__ float hce_block_sum(float v, float* s_f) {
+    v = warp_sum(v);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) s_f[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float t = 0.f;
+#pragma unroll
+    for (int w = 0; w < HCE_THREADS / 32; w++) t += s_f[w];
+    return t;
+}
+
+// (value, index) maximum; on equal values the smaller index wins (torch.topk / argmax return the first maximum)
+__device__ __forceinline__ void hce_argmax_merge(float& v, int& i, float v2, int i2) {
+    if (v2 > v || (v2 == v && i2 < i)) { v = v2; i = i2; }
+}
+
+__device__ __forceinline__ void hce_block_argmax(float& v, int& i, float* s_f, int* s_i) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float v2 = __shfl_xor_sync(0xffffffffu, v, o);
+        const int i2 = __shfl_xor_sync(0xffffffffu, i, o);
+        hce_argmax_merge(v, i, v2, i2);
+    }
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) { s_f[threadIdx.x >> 5] = v; s_i[threadIdx.x >> 5] = i; }
+    __syncthreads();
+    v = s_f[0]; i = s_i[0];
+#pragma unroll
+    for (int w = 1; w < HCE_THREADS / 32; w++) hce_argmax_merge(v, i, s_f[w], s_i[w]);
+}
+
+// Softmax cross-entropy of one image per CTA on logits [N, K] (any K), max-subtracted log-sum-exp:
+//   hard label y, smoothing s:  loss = lse - (1-s) z_y - (s/K) sum_k z_k        (LabelSmoothingCrossEntropy; s = 0: CE)
+//   soft targets t:             loss = sum_k t_k (lse - z_k)                   (SoftTargetCrossEntropy)
+//   dlogits = (softmax(z) sum_k t_k - t) * loss_scale [* *loss_scale_dev] / N, t the effective (smoothed) target
+//   top-1 hit: first index of the max logit == the label (soft: the first index of the max target)
+// A hard label outside [0, K) is never used as an index: the image's loss is NaN, its dlogits row zero, no hit.
+// Per-image loss / hit go to fixed slots; the last CTA adds them in image order (no atomics).
+__global__ void __launch_bounds__(HCE_THREADS) head_ce_kernel(const float* __restrict__ logits, int K,
+                                                              const long long* __restrict__ tgt_i,
+                                                              const float* __restrict__ tgt_f, float smoothing,
+                                                              float inv_n, float loss_scale,
+                                                              const float* __restrict__ loss_scale_dev,
+                                                              float* __restrict__ loss_acc, float* __restrict__ correct_acc,
+                                                              float* __restrict__ dlogits) {
+    __shared__ float s_f[HCE_THREADS / 32];
+    __shared__ int s_i[HCE_THREADS / 32];
+    const int n = blockIdx.x, tid = threadIdx.x;
+    const float* z = logits + (size_t)n * K;
+    const float* t = tgt_f ? tgt_f + (size_t)n * K : nullptr;
+    const long long y = t ? 0 : tgt_i[n];
+    const bool valid = t != nullptr || (y >= 0 && y < K);
+    // pass 1: max logit (+ its first index); soft targets: max target (+ its first index) and sum t
+    float zm = -INFINITY, tm = -INFINITY, st = 0.f;
+    int zi = K, ti = K;
+    for (int k = tid; k < K; k += HCE_THREADS) {
+        const float v = z[k];
+        if (v > zm) { zm = v; zi = k; }
+        if (t) {
+            const float tv = t[k];
+            if (tv > tm) { tm = tv; ti = k; }
+            st += tv;
+        }
+    }
+    hce_block_argmax(zm, zi, s_f, s_i);
+    if (t) {
+        hce_block_argmax(tm, ti, s_f, s_i);
+        st = hce_block_sum(st, s_f);
+    }
+    // pass 2: log-sum-exp
+    float se = 0.f;
+    for (int k = tid; k < K; k += HCE_THREADS) se += expf(z[k] - zm);
+    const float lse = zm + logf(hce_block_sum(se, s_f));
+    // pass 3: loss = sum_k t_k (lse - z_k) with the effective target t (hard: (1-s) one-hot + s/K; the one-hot term is
+    // added once below, which is lse - (1-s) z_y - (s/K) sum_k z_k without the cancellation of the expanded form), dlogits
+    const float s = smoothing, off = s / (float)K, on = 1.f - s;
+    const float ls = loss_scale_dev ? loss_scale * *loss_scale_dev : loss_scale;       // fp16 dynamic loss scaling
+    const float scale = ls * inv_n, tsum = t ? st : 1.f;
+    float* d = dlogits ? dlogits + (size_t)n * K : nullptr;
+    float sl = 0.f;
+    for (int k = tid; k < K; k += HCE_THREADS) {
+        const float v = z[k];
+        sl = fmaf(t ? t[k] : off, lse - v, sl);
+        if (d) d[k] = valid ? (expf(v - lse) * tsum - (t ? t[k] : (k == (int)y ? on + off : off))) * scale : 0.f;
+    }
+    sl = hce_block_sum(sl, s_f);
+    if (tid == 0) {
+        float loss;
+        if (!valid) loss = __int_as_float(0x7fc00000);    // NaN
+        else if (t) loss = sl;
+        else loss = fmaf(on, lse - z[(int)y], sl);
+        const int lab = t ? ti : (int)y;
+        g_small_ws[n] = loss * inv_n;
+        g_small_ws[gridDim.x + n] = valid && zi == lab ? 1.f : 0.f;
+    }
+    if (!ticket_last(g_small_tk, gridDim.x)) return;
+    if (tid == 0) {
+        float l = 0.f, c = 0.f;
+        for (int i = 0; i < (int)gridDim.x; i++) { l += __ldcg(g_small_ws + i); c += __ldcg(g_small_ws + gridDim.x + i); }
+        *loss_acc += l;
+        *correct_acc += c;
+    }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -618,23 +842,50 @@ int dfd_se_fc_wgrad(const float* d_e, const float* r, const float* d_rpre, const
 int dfd_head_fwd(const float* pooled, const float* W, const float* b, float* logits, int N, int F, int K,
                  const long long* tgt_i, const float* tgt_f, float smoothing, float loss_scale,
                  const float* loss_scale_dev, float* loss_acc, float* correct_acc, float* dlogits, void* stream) {
-    if (N <= 0 || F <= 0 || K <= 0 || K > 32) return dfd_set_error(DFD_ERR_ARG, "dfd_head_fwd: sizes");
-    if (loss_acc && K != 2) return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_head_fwd: fused sigmoid-BCE needs num_classes == 2");
+    if (N <= 0 || F <= 0 || K <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_head_fwd: sizes");
+    if (!head_sizes_fit_int(N, F, K)) return dfd_set_error(DFD_ERR_ARG, "dfd_head_fwd: N*K, K*F or N*F exceeds int");
     if (loss_acc && !tgt_i && !tgt_f) return dfd_set_error(DFD_ERR_ARG, "dfd_head_fwd: loss without target");
     if (loss_acc && 2 * (long long)N > SMALL_WS_FLOATS) return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_head_fwd: batch exceeds the reduction scratch");
-    head_fwd_kernel<<<N, 64, 0, (cudaStream_t)stream>>>(pooled, W, b, logits, F, K, tgt_i, tgt_f, smoothing,
-                                                         1.f / (float)N, loss_scale, loss_scale_dev, loss_acc, correct_acc, dlogits);
+    cudaStream_t st = (cudaStream_t)stream;
+    const float inv_n = 1.f / (float)N;
+    if (K == 2) {
+        head_fwd_kernel<<<N, 64, 0, st>>>(pooled, W, b, logits, F, K, tgt_i, tgt_f, smoothing, inv_n, loss_scale,
+                                          loss_scale_dev, loss_acc, correct_acc, dlogits);
+        DFD_LAUNCH_CHECK();
+        return DFD_OK;
+    }
+    // logits[N,K] = pooled[N,F] . W[K,F]^T + b
+    head_gemm<true, true, false>(pooled, F, 1, W, F, 1, logits, K, b, nullptr, N, K, F, st);
     DFD_LAUNCH_CHECK();
+    if (loss_acc) {
+        head_ce_kernel<<<N, HCE_THREADS, 0, st>>>(logits, K, tgt_i, tgt_f, smoothing, inv_n, loss_scale, loss_scale_dev,
+                                                  loss_acc, correct_acc, dlogits);
+        DFD_LAUNCH_CHECK();
+    }
     return DFD_OK;
 }
 
 int dfd_head_bwd(const float* dlogits, const float* pooled, const float* W, float* dW, float* db, float* dpooled,
                  int N, int F, int K, void* stream) {
     if (N <= 0 || F <= 0 || K <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_head_bwd: sizes");
+    if (!head_sizes_fit_int(N, F, K)) return dfd_set_error(DFD_ERR_ARG, "dfd_head_bwd: N*K, K*F or N*F exceeds int");
     cudaStream_t st = (cudaStream_t)stream;
-    head_dgrad_kernel<<<cdiv((long long)N * F, 256), 256, 0, st>>>(dlogits, W, dpooled, N, F, K);
+    if (K == 2) {
+        // head_wgrad_kernel's split partials take nsplit * bx * 256 floats of the scratch and one ticket per column group
+        const int bx = cdiv((long long)K * F, 128), nsplit = N >= 64 ? 16 : (N >= 8 ? 4 : 1);
+        if ((long long)nsplit * bx * 256 > SMALL_WS_FLOATS || bx > SMALL_TICKETS)
+            return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_head_bwd: feature count exceeds the reduction scratch");
+        head_dgrad_kernel<<<cdiv((long long)N * F, 256), 256, 0, st>>>(dlogits, W, dpooled, N, F, K);
+        DFD_LAUNCH_CHECK();
+        head_wgrad_kernel<<<dim3(bx, nsplit), 128, 0, st>>>(dlogits, pooled, dW, db, N, F, K);
+        DFD_LAUNCH_CHECK();
+        return DFD_OK;
+    }
+    // dpooled[N,F] = dlogits[N,K] . W[K,F]
+    head_gemm<true, false, false>(dlogits, K, 1, W, 1, F, dpooled, F, nullptr, nullptr, N, F, K, st);
     DFD_LAUNCH_CHECK();
-    head_wgrad_kernel<<<dim3(cdiv((long long)K * F, 128), N >= 64 ? 16 : (N >= 8 ? 4 : 1)), 128, 0, st>>>(dlogits, pooled, dW, db, N, F, K);
+    // dW[K,F] += dlogits^T . pooled, db[K] += sum_n dlogits[n,:]   (both summed over the images in order)
+    head_gemm<false, false, true>(dlogits, 1, K, pooled, 1, F, dW, F, nullptr, db, K, F, N, st);
     DFD_LAUNCH_CHECK();
     return DFD_OK;
 }

@@ -867,7 +867,7 @@ class Engine:
         return self.logits
 
     def head(self, with_loss, smoothing=0.0, loss_scale=1.0, soft=False, stream=None, loss_scale_dev=None):
-        """classifier (+ fused sigmoid-BCE loss, top-1 count and dL/dlogits when with_loss)."""
+        """classifier (+ fused softmax-CE loss, top-1 count and dL/dlogits when with_loss; any num_classes)."""
         st = stream if stream is not None else torch.cuda.current_stream().cuda_stream
         spec = self.spec
         pw = _ptr(self.params32, self.p_off[self.cls_name + ".weight"][0])

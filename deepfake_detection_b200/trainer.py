@@ -133,7 +133,7 @@ class Trainer:
         self._graph.replay()
 
     def train_step(self, x, target):
-        """x: [N,C,H,W] on any device; target: int64 [N] or float [N,2]. Returns (loss, correct) DEVICE scalars."""
+        """x: [N,C,H,W] on any device; target: int64 [N] or float [N, num_classes]. Returns (loss, correct) DEVICE scalars."""
         e = self.engine
         e.set_input(x)
         e.set_target(target)

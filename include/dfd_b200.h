@@ -223,7 +223,12 @@ int dfd_se_bwd_chain(const void* da, const void* y, const float* scale, const fl
 
 /* ---- classifier + loss + accuracy: nn.Linear (efficientnet.py:348, resnet.py:467), LabelSmoothing /
  *      SoftTarget / nn.CrossEntropyLoss (loss/cross_entropy.py:20-36, train.py:509-520), accuracy
- *      (utils.py:170-186).  2-class softmax-CE is computed as sigmoid-BCE on z1 - z0 (exactly equal). ----- */
+ *      (utils.py:170-186).  Any K >= 1.  K == 2: one CTA per image, softmax-CE computed as sigmoid-BCE on z1 - z0
+ *      (exactly equal); the backward splits the batch into fixed scratch slots added in order.  Every other K: fp32
+ *      tiled SIMT GEMMs for logits / dpooled / dW (each output reduced by one thread in a fixed order, no split, no
+ *      scratch) and a per-image max-subtracted log-sum-exp pass for loss, top-1 and dlogits; there a hard label outside
+ *      [0, K) gives that image a NaN loss and a zero dlogits row.  Loss and correct count are added in image order:
+ *      both heads are run-to-run bit-identical. ----- */
 int dfd_head_fwd(const float* pooled, const float* W, const float* b, float* logits, int N, int F, int K,
                  const long long* target_i64, const float* target_soft, float smoothing, float loss_scale,
                  const float* loss_scale_dev, float* loss_acc, float* correct_acc, float* dlogits, void* stream);
