@@ -41,12 +41,14 @@ SIGNATURES = {
     "dfd_bn_finalize": "ppd" "ppppp" "ffii" "ppppp",
     "dfd_bn_act": "pppppp" "ili" "iii" "p",
     "dfd_pool": "pppp" "ili" "ii" "pi" "p",
+    "dfd_global_pool": "ppppp" "ili" "iii" "i" "p",
     "dfd_bn_bwd_reduce": "ppppp" "ili" "i" "ppp" "p",
     "dfd_relu_bn_bwd_reduce": "ppppppp" "ili" "i" "pp" "p",
     "dfd_bn_bwd_finalize": "ppd" "pppppppp" "i" "p",
     "dfd_bn_bwd_apply": "ppppppp" "ili" "i" "p",
     "dfd_se_bwd_reduce": "ppppp" "ili" "i" "p",
     "dfd_act_bwd": "ppppppppp" "ili" "ii" "ppp" "p",
+    "dfd_act_bwd_gpool": "pppppppp" "ili" "iii" "ppp" "p",
     "dfd_add_inplace": "pp" "li" "p",
     "dfd_se_fc_fwd": "pppppp" "iii" "p",
     "dfd_se_fc_bwd": "pppppp" "pppppppp" "iii" "p",
@@ -77,6 +79,7 @@ SIGNATURES = {
     "dfd_maxpool_bwd": "ppp" "iiii" "i" "p",
     "dfd_relu_bwd": "ppp" "li" "p",
     "dfd_pool_bwd": "pp" "ili" "i" "p",
+    "dfd_gpool_bwd": "ppp" "ili" "ii" "p",
     "dfd_stem_im2col": "pp" "iiiiiiii" "i" "p",
     "dfd_pad_weight": "pp" "iii" "i" "p",
     "dfd_unpad_grad": "pp" "iii" "p",
@@ -84,6 +87,7 @@ SIGNATURES = {
 
 DT_BF16, DT_FP16 = 0, 1
 ACT_NONE, ACT_SWISH, ACT_RELU = 0, 1, 2
+POOL_TYPES = {"avg": 0, "max": 1, "avgmax": 2, "catavgmax": 3}     # DFD_POOL_* (adaptive_avgmax_pool.py:35-48)
 
 
 class NativeError(RuntimeError):

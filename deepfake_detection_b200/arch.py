@@ -75,6 +75,12 @@ class EfficientNetSpec:
     num_classes: int
     input_size: Tuple[int, int, int]
     family: str = "efficientnet"
+    global_pool: str = "avg"
+
+    @property
+    def pooled_features(self):
+        """width of the pooled vector the classifier reads: num_features * feat_mult (adaptive_avgmax_pool.py:17-21)"""
+        return self.num_features * pool_feat_mult(self.global_pool)
 
 
 _EFFNET_ARCH_DEF = [
@@ -150,6 +156,11 @@ class ResNetSpec:
     num_classes: int
     input_size: Tuple[int, int, int]
     family: str = "resnet"
+    global_pool: str = "avg"
+
+    @property
+    def pooled_features(self):
+        return self.num_features * pool_feat_mult(self.global_pool)
 
 
 def _resnet_spec(arch, kind, layers, in_chans, num_classes, input_size):
@@ -172,7 +183,24 @@ def _resnet_spec(arch, kind, layers, in_chans, num_classes, input_size):
 # registry of the variants on the hot path
 # ----------------------------------------------------------------------------------------------
 
-def get_spec(arch, num_classes=2, in_chans=3):
+GLOBAL_POOL_TYPES = ("avg", "max", "avgmax", "catavgmax")
+
+
+def pool_feat_mult(pool_type):
+    return 2 if pool_type == "catavgmax" else 1
+
+
+def get_spec(arch, num_classes=2, in_chans=3, global_pool="avg"):
+    """`global_pool`: the SelectAdaptivePool2d type behind the last feature map (efficientnet.py:297-300,
+    resnet.py:407-409); 'catavgmax' doubles the classifier input."""
+    if global_pool not in GLOBAL_POOL_TYPES:
+        raise ValueError("Invalid pool type: %s" % (global_pool,))      # adaptive_avgmax_pool.py:82-84
+    spec = _base_spec(arch, num_classes, in_chans)
+    spec.global_pool = global_pool
+    return spec
+
+
+def _base_spec(arch, num_classes, in_chans):
     if arch == "efficientnet_b0":
         return _efficientnet_spec(arch, 1.0, 1.0, 32, 1280, in_chans, num_classes, (3, 224, 224))
     if arch == "efficientnet_b4":
@@ -234,7 +262,7 @@ def state_entries(spec):
                 out += _bn_entries(p + ".bn2", b.cout)
         out.append(("conv_head.weight", (spec.num_features, spec.head_in, 1, 1), "conv_w"))
         out += _bn_entries("bn2", spec.num_features)
-        out.append(("classifier.weight", (spec.num_classes, spec.num_features), "fc_w"))
+        out.append(("classifier.weight", (spec.num_classes, spec.pooled_features), "fc_w"))
         out.append(("classifier.bias", (spec.num_classes,), "fc_b"))
     else:
         out.append(("conv1.weight", (64, spec.in_chans, 7, 7), "conv_w"))
@@ -256,7 +284,7 @@ def state_entries(spec):
             if b.downsample:
                 out.append((p + ".downsample.0.weight", (b.cout, b.cin, 1, 1), "conv_w"))
                 out += _bn_entries(p + ".downsample.1", b.cout)
-        out.append(("fc.weight", (spec.num_classes, spec.num_features), "fc_w"))
+        out.append(("fc.weight", (spec.num_classes, spec.pooled_features), "fc_w"))
         out.append(("fc.bias", (spec.num_classes,), "fc_b"))
     return out
 

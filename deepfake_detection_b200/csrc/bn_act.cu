@@ -12,6 +12,10 @@
 //   Swish fwd/bwd        dfd/timm/models/layers/activations.py:19-33
 //   SE gate, residual    dfd/timm/models/efficientnet_blocks.py:104-110, 343-346
 //   global average pool  dfd/timm/models/efficientnet.py:340-343
+//   max / avgmax / catavgmax global pool and argmax   dfd/timm/models/layers/adaptive_avgmax_pool.py:24-48
+#include <climits>
+#include <cmath>
+
 #include "common.cuh"
 #include "se_chain.cuh"
 #include "bn_finalize.cuh"
@@ -314,6 +318,145 @@ __global__ void pool_kernel(const T* __restrict__ y, const float* __restrict__ s
 }
 
 // ---------------------------------------------------------------------------------------------
+// selectable global pool (avg / max / avgmax / catavgmax) + argmax, one pass
+// ---------------------------------------------------------------------------------------------
+// does (m_new, i_new) replace (m_cur, i_cur)?  torch's adaptive_max_pool2d scans row-major and replaces on `v > max || isnan(v)`:
+// over any set of (value, index) pairs that gives the last NaN if there is one, else the max with the lowest index. This
+// comparison yields exactly that for ANY two disjoint sets, so strided per-thread rows, rows of the CTA and row chunks all
+// combine to the sequential result. i_cur == INT_MAX marks an empty set (loses every tie, so an all -inf column -> index 0).
+__device__ __forceinline__ bool gp_takes(float m_new, int i_new, float m_cur, int i_cur) {
+    if (m_new != m_new) return m_cur == m_cur || i_new > i_cur;
+    if (m_cur != m_cur) return false;
+    return m_new > m_cur || (m_new == m_cur && i_new < i_cur);
+}
+
+// max / argmax partials of the chunked pool, laid out like the sums in g_rowred_ws ([chunk][image][C]) and as large, so that
+// dfd_global_pool can always use dfd_pool's chunk geometry (and hence its summation order)
+__device__ float g_rowred_max[ROWRED_WS_FLOATS];
+__device__ int g_rowred_arg[ROWRED_WS_FLOATS];
+
+template <int PT>
+__device__ __forceinline__ void gpool_emit(float* pooled, int* argmax, int n, int C, int c, float sum, float inv, float m, int i) {
+    const float a = sum * inv;          // dfd_pool's mean, same operands
+    if (PT == DFD_POOL_AVG) pooled[(size_t)n * C + c] = a;
+    else if (PT == DFD_POOL_MAX) pooled[(size_t)n * C + c] = m;
+    else if (PT == DFD_POOL_AVGMAX) pooled[(size_t)n * C + c] = 0.5f * (a + m);
+    else { pooled[(size_t)n * 2 * C + c] = a; pooled[(size_t)n * 2 * C + C + c] = m; }
+    if (argmax) argmax[(size_t)n * C + c] = i;
+}
+
+// one activation value: the sum term exactly as pool_kernel's `acc += act_fwd(u)` compiles (for Swish the product contracts
+// into fma(u, sigmoid(u), acc)), so that the mean keeps dfd_pool's bits; the max sees the rounded act(u)
+template <int ACT>
+__device__ __forceinline__ float gpool_term(float u, float& acc) {
+    if (ACT == DFD_ACT_SWISH) {
+        const float s = sigmoid_fast(u);
+        acc = fmaf(u, s, acc);
+        return u * s;
+    }
+    const float v = act_fwd<ACT>(u);
+    acc += v;
+    return v;
+}
+
+// pool_kernel's geometry and sum order, plus a running (max, argmax) per thread channel; smem [3][RY][C]
+template <typename T, int ACT, int PT>
+__global__ void gpool_kernel(const T* __restrict__ y, const float* __restrict__ scale, const float* __restrict__ shift,
+                             float* __restrict__ pooled, int* __restrict__ argmax, long long hw, long long rows_per_block) {
+    extern __shared__ float sm[];
+    const int V = blockDim.x, RY = blockDim.y, C = V * 8;
+    const int c0 = threadIdx.x * 8;
+    float sc[8], sh[8], acc[8], mx[8];
+    int ix[8];
+    ldg_f8(scale ? scale + c0 : nullptr, sc, 1.f);
+    ldg_f8(shift ? shift + c0 : nullptr, sh, 0.f);
+#pragma unroll
+    for (int i = 0; i < 8; i++) { acc[i] = 0.f; mx[i] = -INFINITY; ix[i] = INT_MAX; }
+    const T* base = y + (size_t)blockIdx.y * hw * C + c0;
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    long long r1 = r0 + rows_per_block;
+    if (r1 > hw) r1 = hw;
+    constexpr int U = 4;
+    long long r = r0 + threadIdx.y;
+    for (; r + (long long)(U - 1) * blockDim.y < r1; r += (long long)U * blockDim.y) {
+        uint4 raw[U];
+#pragma unroll
+        for (int u = 0; u < U; u++) raw[u] = ldg16(base + (size_t)(r + (long long)u * blockDim.y) * C);
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+            float f[8];
+            unpack8<T>(raw[u], f);
+            const int rr = (int)(r + (long long)u * blockDim.y);
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                const float v = gpool_term<ACT>(fmaf(f[i], sc[i], sh[i]), acc[i]);
+                if (gp_takes(v, rr, mx[i], ix[i])) { mx[i] = v; ix[i] = rr; }
+            }
+        }
+    }
+    for (; r < r1; r += blockDim.y) {
+        float f[8];
+        unpack8<T>(ldg16(base + (size_t)r * C), f);
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+            const float v = gpool_term<ACT>(fmaf(f[i], sc[i], sh[i]), acc[i]);
+            if (gp_takes(v, (int)r, mx[i], ix[i])) { mx[i] = v; ix[i] = (int)r; }
+        }
+    }
+    // rows of the CTA: sums in reduce_rows_and_emit's order, (max, argmax) by gp_takes
+    float* rs = sm;
+    float* rm = sm + (size_t)RY * C;
+    int* ri = reinterpret_cast<int*>(sm + (size_t)2 * RY * C);
+    {
+        const size_t o = (size_t)threadIdx.y * C + c0;
+#pragma unroll
+        for (int i = 0; i < 8; i++) { rs[o + i] = acc[i]; rm[o + i] = mx[i]; ri[o + i] = ix[i]; }
+    }
+    __syncthreads();
+    const float inv = 1.f / (float)hw;
+    const int tid = threadIdx.y * V + threadIdx.x, nt = V * RY;
+    const int n = blockIdx.y;
+    const size_t slot = ((size_t)blockIdx.x * gridDim.y + n) * C;
+    for (int c = tid; c < C; c += nt) {
+        float s = 0.f, m = -INFINITY;
+        int im = INT_MAX;
+        for (int k = 0; k < RY; k++) {
+            s += rs[(size_t)k * C + c];
+            const float mk = rm[(size_t)k * C + c];
+            const int ik = ri[(size_t)k * C + c];
+            if (gp_takes(mk, ik, m, im)) { m = mk; im = ik; }
+        }
+        if (gridDim.x == 1) gpool_emit<PT>(pooled, argmax, n, C, c, s, inv, m, im);
+        else { g_rowred_ws[slot + c] = s; g_rowred_max[slot + c] = m; g_rowred_arg[slot + c] = im; }
+    }
+    if (gridDim.x == 1) return;
+    // several row chunks per image: fixed-slot partials, combined in chunk order by the last chunk to arrive (as pool_kernel)
+    __shared__ int s_last;
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) {
+        const int t = atomicAdd(g_rowred_tk + n, 1);
+        s_last = (t == (int)gridDim.x - 1);
+        if (s_last) g_rowred_tk[n] = 0;
+    }
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    for (int c = tid; c < C; c += nt) {
+        float s = 0.f, m = -INFINITY;
+        int im = INT_MAX;
+        for (int k = 0; k < (int)gridDim.x; k++) {
+            const size_t o = ((size_t)k * gridDim.y + n) * C + c;
+            s += __ldcg(g_rowred_ws + o);
+            const float mk = __ldcg(g_rowred_max + o);
+            const int ik = __ldcg(g_rowred_arg + o);
+            if (gp_takes(mk, ik, m, im)) { m = mk; im = ik; }
+        }
+        gpool_emit<PT>(pooled, argmax, n, C, c, s, inv, m, im);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
 // BN backward, phase 1: s1[c] += sum g, s2[c] += sum g * xhat, xhat = (y - mean) * rstd
 // RELU_MASK: g is first masked by (out > 0) (ResNet: gradient through the post-add ReLU)
 // ---------------------------------------------------------------------------------------------
@@ -536,23 +679,39 @@ __global__ void se_bwd_reduce_kernel(const T* __restrict__ da, const T* __restri
 #ifndef ACTBWD_U_RELU
 #define ACTBWD_U_RELU 3
 #endif
-template <typename T, int ACT, bool HAS_DA, int MAXT, int OCC>
+// GP (global-pool gradient, no da, no gate): dpool is dpooled [n, P] of dfd_global_pool of type pool_type, the operand slots
+// hold g_max (4), g_avg * inv_hw (5) and the argmax (6), and gin = g_avg / hw + (row == argmax) * g_max
+template <typename T, int ACT, bool HAS_DA, int MAXT, int OCC, bool GP = false>
 __global__ void __launch_bounds__(MAXT, OCC) act_bwd_kernel(const T* __restrict__ da, const T* __restrict__ y, const float* __restrict__ scale,
                                const float* __restrict__ shift, const float* __restrict__ mean,
                                const float* __restrict__ rstd, const float* __restrict__ gate,
                                const float* __restrict__ dpool, float inv_hw, T* __restrict__ gu, long long hw,
                                int rows_per_block, double* __restrict__ s1, double* __restrict__ s2,
-                               const BnBwdFinDesc* __restrict__ fin) {
+                               const BnBwdFinDesc* __restrict__ fin, const int* __restrict__ argmax = nullptr,
+                               int pool_type = DFD_POOL_AVG) {
     extern __shared__ __align__(16) float sm[];
     const int V = blockDim.x, C = V * 8;
     const int c0 = threadIdx.x * 8;
     const int tid = threadIdx.y * blockDim.x + threadIdx.x, nt = blockDim.x * blockDim.y;
     float4* ps = reinterpret_cast<float4*>(sm + (size_t)blockDim.y * C);      // behind the [RY][C] reduction scratch
-    for (int e = tid; e < 12 * V; e += nt) {
+    for (int e = tid; e < (GP ? 14 : 12) * V; e += nt) {
         const int k = e / (2 * V), rem = e - k * 2 * V, h = rem / V, v = rem - h * V;
         const int c = v * 8 + h * 4;
         float4 val;
-        if (k == 0) val = ldg_f4(scale + c);
+        if (GP && k >= 4) {
+            const size_t nC = (size_t)blockIdx.y * C;
+            if (k == 6) {
+                const int* a = argmax + nC + c;
+                val = make_float4(__int_as_float(a[0]), __int_as_float(a[1]), __int_as_float(a[2]), __int_as_float(a[3]));
+            } else if (pool_type == DFD_POOL_CATAVGMAX) {
+                val = ldg_f4(dpool + 2 * nC + (k == 4 ? C : 0) + c);
+            } else {
+                const float4 d = ldg_f4(dpool + nC + c);
+                const float f = pool_type == DFD_POOL_AVGMAX ? 0.5f : (k == 4 ? 1.f : 0.f);
+                val = make_float4(d.x * f, d.y * f, d.z * f, d.w * f);
+            }
+            if (k == 5) val = make_float4(val.x * inv_hw, val.y * inv_hw, val.z * inv_hw, val.w * inv_hw);
+        } else if (k == 0) val = ldg_f4(scale + c);
         else if (k == 1) val = ldg_f4(shift + c);
         else if (k == 2) {
             const float4 m = ldg_f4(mean + c), r = ldg_f4(rstd + c);
@@ -605,11 +764,18 @@ __global__ void __launch_bounds__(MAXT, OCC) act_bwd_kernel(const T* __restrict_
                 const float sc[4] = {sc4.x, sc4.y, sc4.z, sc4.w}, sh[4] = {sh4.x, sh4.y, sh4.z, sh4.w};
                 const float nm[4] = {nm4.x, nm4.y, nm4.z, nm4.w}, rs[4] = {rs4.x, rs4.y, rs4.z, rs4.w};
                 const float gt[4] = {gt4.x, gt4.y, gt4.z, gt4.w}, dp[4] = {dp4.x, dp4.y, dp4.z, dp4.w};
+                int am[4] = {0, 0, 0, 0};
+                if (GP) {
+                    const float4 am4 = ps[(6 * 2 + h) * V + threadIdx.x];
+                    am[0] = __float_as_int(am4.x); am[1] = __float_as_int(am4.y);
+                    am[2] = __float_as_int(am4.z); am[3] = __float_as_int(am4.w);
+                }
 #pragma unroll
                 for (int j = 0; j < 4; j++) {
                     const int i = h * 4 + j;
                     float uu = fmaf(f[i], sc[j], sh[j]);
                     float gin = HAS_DA ? fmaf(d[i], gt[j], dp[j]) : dp[j];
+                    if (GP && rr == (long long)am[j]) gin = dp[j] + gt[j];          // gt holds g_max here
                     float o = gin * act_bwd<ACT>(uu);
                     // the stored (rounded) value is what the consumers see: reduce the rounded value
                     o = round_t<T>(o);
@@ -705,11 +871,9 @@ int dfd_bn_act(const void* y, const float* scale, const float* shift, const floa
     return DFD_OK;
 }
 
-static int launch_pool(const void* y, const float* scale, const float* shift, float* pooled, int n, long long hw, int C,
-                       int act, int dt, int max_chunks, const SeFwdArgs& se, void* stream) {
-    if (C % 8 || C <= 0 || hw <= 0 || n <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_pool: C%8, sizes");
-    // one CTA per image while the batch fills the GPU; otherwise up to max_chunks row chunks per image (fixed-slot partials
-    // in the library scratch, summed in chunk order by the last chunk of the image to arrive)
+// geometry of the per-image pools: one CTA per image while the batch fills the GPU; otherwise up to max_chunks row chunks per
+// image (fixed-slot partials in the library scratch, combined in chunk order by the last chunk of the image to arrive)
+static RowGeom pool_geom(int C, long long hw, int n, int max_chunks) {
     const bool chunked = max_chunks > 1 && n < 296 && n <= ROWRED_TICKETS;
     RowGeom g = make_geom(C, hw, n, chunked ? 592 : 1, row_maxt(hw, true));
     if (!chunked) { g.grid = dim3(1, n, 1); g.rows_per_block = (int)hw; }
@@ -720,6 +884,13 @@ static int launch_pool(const void* y, const float* scale, const float* shift, fl
         g.grid.x = (unsigned)((hw + rpb - 1) / rpb);
     }
     if ((long long)g.grid.x * n * C > ROWRED_WS_FLOATS) { g.grid = dim3(1, n, 1); g.rows_per_block = (int)hw; }
+    return g;
+}
+
+static int launch_pool(const void* y, const float* scale, const float* shift, float* pooled, int n, long long hw, int C,
+                       int act, int dt, int max_chunks, const SeFwdArgs& se, void* stream) {
+    if (C % 8 || C <= 0 || hw <= 0 || n <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_pool: C%8, sizes");
+    const RowGeom g = pool_geom(C, hw, n, max_chunks);
     cudaStream_t st = (cudaStream_t)stream;
     const long long rpb = g.rows_per_block;
     const size_t smem = reduce_smem(g) + (size_t)(C + se.Cse) * sizeof(float);
@@ -738,6 +909,36 @@ int dfd_pool(const void* y, const float* scale, const float* shift, float* poole
     (void)partial;       // kept in the signature: the chunk partials now live in the library's own scratch
     SeFwdArgs se = {nullptr, nullptr, nullptr, nullptr, nullptr, 0};
     return launch_pool(y, scale, shift, pooled, n, hw, C, act, dt, max_chunks, se, stream);
+}
+
+int dfd_global_pool(const void* y, const float* scale, const float* shift, float* pooled, int* argmax, int n, long long hw,
+                    int C, int act, int pool_type, int dt, int max_chunks, void* stream) {
+    if (C % 8 || C <= 0 || hw <= 0 || n <= 0 || hw > INT_MAX) return dfd_set_error(DFD_ERR_ARG, "dfd_global_pool: C%8, sizes");
+    if (pool_type < DFD_POOL_AVG || pool_type > DFD_POOL_CATAVGMAX) return dfd_set_error(DFD_ERR_ARG, "dfd_global_pool: pool_type");
+    if (act != DFD_ACT_NONE && act != DFD_ACT_SWISH && act != DFD_ACT_RELU) return dfd_set_error(DFD_ERR_ARG, "dfd_global_pool: act");
+    // dfd_pool's geometry, so the mean is summed in dfd_pool's order (the max scratch is as large as the sums')
+    const RowGeom g = pool_geom(C, hw, n, max_chunks);
+    cudaStream_t st = (cudaStream_t)stream;
+    const long long rpb = g.rows_per_block;
+    const size_t smem = 3 * reduce_smem(g);       // sums, maxima, argmax per row of the CTA
+    if (smem > 48 * 1024) return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_global_pool: channel count exceeds shared memory");
+#define GP_LAUNCH(ACT, PT) gpool_kernel<T, ACT, PT><<<g.grid, g.block, smem, st>>>((const T*)y, scale, shift, pooled, argmax, hw, rpb)
+#define GP_ACT(PT)                                            \
+    if (act == DFD_ACT_SWISH) GP_LAUNCH(DFD_ACT_SWISH, PT);    \
+    else if (act == DFD_ACT_RELU) GP_LAUNCH(DFD_ACT_RELU, PT); \
+    else GP_LAUNCH(DFD_ACT_NONE, PT)
+    DISPATCH_T(dt, {
+        switch (pool_type) {
+            case DFD_POOL_AVG: GP_ACT(DFD_POOL_AVG); break;
+            case DFD_POOL_MAX: GP_ACT(DFD_POOL_MAX); break;
+            case DFD_POOL_AVGMAX: GP_ACT(DFD_POOL_AVGMAX); break;
+            default: GP_ACT(DFD_POOL_CATAVGMAX); break;
+        }
+    });
+#undef GP_ACT
+#undef GP_LAUNCH
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
 }
 
 // global pooling + the whole squeeze-excite gate in ONE launch: pooled[n,c] = mean_hw act(scale*y + shift), then
@@ -882,6 +1083,38 @@ int dfd_act_bwd(const void* da, const void* y, const float* scale, const float* 
         else { if (da) LAUNCH(0, true); else LAUNCH(0, false); }
     });
 #undef LAUNCH
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+int dfd_act_bwd_gpool(const void* y, const float* scale, const float* shift, const float* mean, const float* rstd,
+                      const float* dpooled, const int* argmax, void* gu, int n, long long hw, int C, int act, int pool_type,
+                      int dt, double* s1, double* s2, const void* fin, void* stream) {
+    if (C % 8 || C <= 0 || hw <= 0 || n <= 0 || hw > INT_MAX) return dfd_set_error(DFD_ERR_ARG, "dfd_act_bwd_gpool: C%8, sizes");
+    if (!dpooled || !argmax) return dfd_set_error(DFD_ERR_ARG, "dfd_act_bwd_gpool: operands");
+    if (pool_type != DFD_POOL_MAX && pool_type != DFD_POOL_AVGMAX && pool_type != DFD_POOL_CATAVGMAX)
+        return dfd_set_error(DFD_ERR_ARG, "dfd_act_bwd_gpool: pool_type (avg: dfd_act_bwd)");
+    if (act != DFD_ACT_SWISH) return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_act_bwd_gpool: activation (Swish only)");
+    RowGeom g = make_geom(C, hw, n);
+    cudaStream_t st = (cudaStream_t)stream;
+    const float inv_hw = 1.f / (float)hw;
+    const size_t smem_ab = reduce_smem(g) + (size_t)14 * g.block.x * sizeof(float4);     // + g_max, g_avg / hw, argmax
+    if (smem_ab > 200 * 1024) return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_act_bwd_gpool: channel count exceeds shared memory");
+    static bool smem_attr[2][2] = {};
+    const int var = g.block.x * g.block.y > 256 ? 1 : 0;      // 1: more than 2048 channels (one row of C / 8 threads)
+#define GARGS nullptr, (const T*)y, scale, shift, mean, rstd, nullptr, dpooled, inv_hw, (T*)gu, hw, g.rows_per_block, s1, s2, \
+              (const BnBwdFinDesc*)fin, argmax, pool_type
+    DISPATCH_T(dt, {
+        if (smem_ab > 48 * 1024 && !smem_attr[dt == DFD_DT_FP16][var]) {
+            cudaError_t e_ = var ? cudaFuncSetAttribute(act_bwd_kernel<T, 1, false, 512, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)
+                                 : cudaFuncSetAttribute(act_bwd_kernel<T, 1, false, 256, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+            if (e_ != cudaSuccess) return dfd_set_cuda_error(e_, __FILE__, __LINE__);
+            smem_attr[dt == DFD_DT_FP16][var] = true;
+        }
+        if (var) act_bwd_kernel<T, 1, false, 512, 1, true><<<g.grid, g.block, smem_ab, st>>>(GARGS);
+        else act_bwd_kernel<T, 1, false, 256, 2, true><<<g.grid, g.block, smem_ab, st>>>(GARGS);
+    });
+#undef GARGS
     DFD_LAUNCH_CHECK();
     return DFD_OK;
 }

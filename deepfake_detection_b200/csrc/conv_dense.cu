@@ -1,6 +1,6 @@
 // ResNet-side kernels: dense k x k convolution as (im2col -> tensor-core GEMM), its backward (GEMM -> col2im, GEMM wgrad
 // on the im2col matrix), weight / gradient layout changes between OIHW and the GEMM's [Cout][kh][kw][Cin], 3x3/s2
-// max-pool forward/backward, ReLU-mask and global-average-pool backward.
+// max-pool forward/backward, ReLU-mask and global-pool (avg, and max / avgmax / catavgmax by argmax) backward.
 //   ResNet.forward            dfd/timm/models/resnet.py:450-468 (conv1 7x7 -> bn -> relu -> maxpool 3x3 s2 p1 :379-382)
 //   BasicBlock / Bottleneck   resnet.py:150-175, :215-246 (3x3 convs :129-136,:195-197; downsample 1x1 s2 :249-260)
 // Round-1 scope note: the 3x3 convolutions go through a MATERIALISED im2col matrix (9x the activation bytes). It is
@@ -240,7 +240,38 @@ __global__ void pool_bwd_kernel(const float* __restrict__ dpooled, T* __restrict
         stg16(dout + (size_t)t * C + v * 8, pack8<T>(f));
     }
 }
-
+// dout[n, hw, c] = g_avg[n, c] / HW + (hw == argmax[n, c]) * g_max[n, c]   (backward of the max / avgmax / catavgmax global
+// pool; g_avg / g_max are read from dpooled [N, P] by pool type, as dfd_act_bwd_gpool does)
+template <typename T>
+__global__ void gpool_bwd_kernel(const float* __restrict__ dpooled, const int* __restrict__ argmax, T* __restrict__ dout, int N,
+                                 long long hw, int C, int pool_type) {
+    const int V = C / 8;
+    const long long total = (long long)N * hw * V;
+    const float inv = 1.f / (float)hw;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        int v = (int)(i % V);
+        long long t = i / V;
+        int n = (int)(t / hw);
+        const long long p = t - (long long)n * hw;
+        float f[8];
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+            const int c = v * 8 + j;
+            float ga, gm;
+            if (pool_type == DFD_POOL_CATAVGMAX) {
+                ga = dpooled[(size_t)n * 2 * C + c];
+                gm = dpooled[(size_t)n * 2 * C + C + c];
+            } else {
+                const float d = dpooled[(size_t)n * C + c];
+                ga = pool_type == DFD_POOL_AVGMAX ? 0.5f * d : 0.f;
+                gm = pool_type == DFD_POOL_AVGMAX ? 0.5f * d : d;
+            }
+            const float a = ga * inv;
+            f[j] = p == (long long)argmax[(size_t)n * C + c] ? a + gm : a;
+        }
+        stg16(dout + (size_t)t * C + v * 8, pack8<T>(f));
+    }
+}
 
 // ---- stem as a GEMM: im2col of the NCHW image in (ci, kh, kw) column order (== OIHW flattening), K padded to a multiple of 8.
 // One CTA per output row: the Cin x k input rows it needs are staged (zero-padded) in shared memory with coalesced reads,
@@ -380,6 +411,18 @@ int dfd_pool_bwd(const float* dpooled, void* dout, int N, long long hw, int C, i
     if (C % 8 || N <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_pool_bwd: C%8");
     long long total = (long long)N * hw * (C / 8);
     CD_T(dt, (pool_bwd_kernel<T><<<nblocks(total), 256, 0, (cudaStream_t)stream>>>(dpooled, (T*)dout, N, hw, C)));
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+int dfd_gpool_bwd(const float* dpooled, const int* argmax, void* dout, int N, long long hw, int C, int pool_type, int dt,
+                  void* stream) {
+    if (C % 8 || N <= 0 || hw <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_gpool_bwd: C%8, sizes");
+    if (!dpooled || !argmax) return dfd_set_error(DFD_ERR_ARG, "dfd_gpool_bwd: operands");
+    if (pool_type != DFD_POOL_MAX && pool_type != DFD_POOL_AVGMAX && pool_type != DFD_POOL_CATAVGMAX)
+        return dfd_set_error(DFD_ERR_ARG, "dfd_gpool_bwd: pool_type (avg: dfd_pool_bwd)");
+    long long total = (long long)N * hw * (C / 8);
+    CD_T(dt, (gpool_bwd_kernel<T><<<nblocks(total), 256, 0, (cudaStream_t)stream>>>(dpooled, argmax, (T*)dout, N, hw, C, pool_type)));
     DFD_LAUNCH_CHECK();
     return DFD_OK;
 }

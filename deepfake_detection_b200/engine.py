@@ -36,7 +36,7 @@ class _BN:
 class Engine:
     def __init__(self, arch, batch, height=None, width=None, num_classes=2, in_chans=3, dtype="bf16",
                  bn_momentum=0.1, bn_eps=1e-5, device=None, gemm_impl="tc", share_from=None, stem_impl="gemm",
-                 params_only=False, drop_rate=0.0, drop_path_rate=0.0, sync_bn=False):
+                 params_only=False, drop_rate=0.0, drop_path_rate=0.0, sync_bn=False, global_pool="avg"):
         # _plan_only: build the arenas and the call plan on the CPU for host-logic tests; nothing can be executed
         self._plan_only = device == "plan-only"
         if self._plan_only:
@@ -45,7 +45,7 @@ class Engine:
             raise _lib.NativeError("deepfake_detection_b200.Engine needs a CUDA device (H100, sm_90a); "
                                    "there is no CPU path")
         self.L = _lib.lib()
-        self.spec = spec = get_spec(arch, num_classes=num_classes, in_chans=in_chans)
+        self.spec = spec = get_spec(arch, num_classes=num_classes, in_chans=in_chans, global_pool=global_pool)
         self.cls_name = "classifier" if spec.family == "efficientnet" else "fc"
         self.device = torch.device(device if device is not None else "cuda:%d" % torch.cuda.current_device())
         self.N = int(batch)
@@ -80,8 +80,8 @@ class Engine:
         if share_from is not None:
             # a second plan (other batch size / resolution, e.g. the validation loader) over the SAME weights,
             # gradients and running statistics
-            if share_from.spec.arch != spec.arch or share_from.dt != self.dt:
-                raise ValueError("share_from: architecture / dtype mismatch")
+            if share_from.spec.arch != spec.arch or share_from.dt != self.dt or share_from.spec.global_pool != spec.global_pool:
+                raise ValueError("share_from: architecture / dtype / global_pool mismatch")
             share_from = self._shared_from = share_from.arena
             for a in ("p_off", "n_decay", "n_params", "param_names", "params32", "grads32", "params16", "b_off", "bn_names",
                       "buffers32", "nbt", "t_off", "paramsT16", "_ttable", "_ttable_count", "loss_scale_state", "flags",
@@ -628,14 +628,21 @@ class Engine:
         self.acts["conv_head"] = yh
         fwd.append(gemm(_ptr(x), P16("conv_head.weight"), _ptr(yh), Mf, F, spec.head_in, bnh))
         fwd.append(finalize(bnh, Mf))
-        self.pooled = torch.zeros(N, F, dtype=torch.float32, device=dev)
-        fwd.append(("dfd_pool", (_ptr(yh), bnh.scale, bnh.shift, _ptr(self.pooled), N, Hf * Wf, F, ACT_SWISH, dt,
-                             None, POOL_CHUNKS)))
+        P, pool_t = spec.pooled_features, _lib.POOL_TYPES[spec.global_pool]
+        self.pooled = torch.zeros(N, P, dtype=torch.float32, device=dev)
+        if pool_t == _lib.POOL_TYPES["avg"]:
+            fwd.append(("dfd_pool", (_ptr(yh), bnh.scale, bnh.shift, _ptr(self.pooled), N, Hf * Wf, F, ACT_SWISH, dt,
+                                     None, POOL_CHUNKS)))
+        else:
+            # max / avgmax / catavgmax: one pass gives the mean (dfd_pool's order), the max and its argmax for the backward
+            self.pool_argmax = torch.zeros(N, F, dtype=torch.int32, device=dev)
+            fwd.append(("dfd_global_pool", (_ptr(yh), bnh.scale, bnh.shift, _ptr(self.pooled), _ptr(self.pool_argmax), N,
+                                            Hf * Wf, F, ACT_SWISH, pool_t, dt, POOL_CHUNKS)))
         self.drop_masks = OrderedDict()
         if self.drop_rate > 0.0:
-            self.dropout_mask = torch.ones(N, F, dtype=torch.float32, device=dev)
-            masks.append((self.dropout_mask, N * F, 1, 1.0 - self.drop_rate))
-            fwd.append(("dfd_mul_f32_train", (_ptr(self.pooled), _ptr(self.dropout_mask), N * F)))
+            self.dropout_mask = torch.ones(N, P, dtype=torch.float32, device=dev)
+            masks.append((self.dropout_mask, N * P, 1, 1.0 - self.drop_rate))
+            fwd.append(("dfd_mul_f32_train", (_ptr(self.pooled), _ptr(self.dropout_mask), N * P)))
         for r_ in recs:
             if r_["dp_gate"] is not None:
                 self.drop_masks[r_["b"].name] = r_["dp_gate"]
@@ -651,18 +658,23 @@ class Engine:
         K = spec.num_classes
         self.logits = torch.zeros(N, K, dtype=torch.float32, device=dev)
         self.dlogits = torch.zeros(N, K, dtype=torch.float32, device=dev)
-        self.dpooled = torch.zeros(N, F, dtype=torch.float32, device=dev)
+        self.dpooled = torch.zeros(N, P, dtype=torch.float32, device=dev)
         self.target_i = torch.zeros(N, dtype=torch.int64, device=dev)
         self.target_f = torch.zeros(N, K, dtype=torch.float32, device=dev)
         self._head_in = x
 
         # ---- backward ----------------------------------------------------------------------------
         bwd.append(("dfd_head_bwd", (_ptr(self.dlogits), _ptr(self.pooled), P32("classifier.weight"),
-                                     G32("classifier.weight"), G32("classifier.bias"), _ptr(self.dpooled), N, F, K)))
+                                     G32("classifier.weight"), G32("classifier.bias"), _ptr(self.dpooled), N, P, K)))
         if self.drop_rate > 0.0:
-            bwd.append(("dfd_mul_f32", (_ptr(self.dpooled), _ptr(self.dropout_mask), N * F)))
-        bwd.append(("dfd_act_bwd", (None, _ptr(yh), bnh.scale, bnh.shift, bnh.mean, bnh.rstd, None, _ptr(self.dpooled),
-                                    mid_a, N, Hf * Wf, F, ACT_SWISH, dt, bnh.bs1, bnh.bs2, BF(bnh))))
+            bwd.append(("dfd_mul_f32", (_ptr(self.dpooled), _ptr(self.dropout_mask), N * P)))
+        if pool_t == _lib.POOL_TYPES["avg"]:
+            bwd.append(("dfd_act_bwd", (None, _ptr(yh), bnh.scale, bnh.shift, bnh.mean, bnh.rstd, None, _ptr(self.dpooled),
+                                        mid_a, N, Hf * Wf, F, ACT_SWISH, dt, bnh.bs1, bnh.bs2, BF(bnh))))
+        else:
+            bwd.append(("dfd_act_bwd_gpool", (_ptr(yh), bnh.scale, bnh.shift, bnh.mean, bnh.rstd, _ptr(self.dpooled),
+                                              _ptr(self.pool_argmax), mid_a, N, Hf * Wf, F, ACT_SWISH, pool_t, dt, bnh.bs1,
+                                              bnh.bs2, BF(bnh))))
         bwd.append(bwd_finalize(bnh, Mf))
         bwd.append(("dfd_bn_bwd_apply", (mid_a, _ptr(yh), None, bnh.cA, bnh.cB, bnh.cC, mid_b, N, Hf * Wf, F, dt)))
         cur = 0
@@ -873,12 +885,12 @@ class Engine:
         pw = _ptr(self.params32, self.p_off[self.cls_name + ".weight"][0])
         pb = _ptr(self.params32, self.p_off[self.cls_name + ".bias"][0])
         if with_loss:
-            _lib.call("dfd_head_fwd", _ptr(self.pooled), pw, pb, _ptr(self.logits), self.N, spec.num_features,
+            _lib.call("dfd_head_fwd", _ptr(self.pooled), pw, pb, _ptr(self.logits), self.N, spec.pooled_features,
                       spec.num_classes, None if soft else _ptr(self.target_i), _ptr(self.target_f) if soft else None,
                       float(smoothing), float(loss_scale), loss_scale_dev, _ptr(self.scalars), _ptr(self.scalars, 1),
                       _ptr(self.dlogits), st)
         else:
-            _lib.call("dfd_head_fwd", _ptr(self.pooled), pw, pb, _ptr(self.logits), self.N, spec.num_features,
+            _lib.call("dfd_head_fwd", _ptr(self.pooled), pw, pb, _ptr(self.logits), self.N, spec.pooled_features,
                       spec.num_classes, None, None, 0.0, 1.0, None, None, None, None, st)
 
     def backward(self, stream=None):

@@ -227,12 +227,18 @@ def build_resnet(e):
         recs.append(rec)
         x = out
     F, K = spec.num_features, spec.num_classes
-    e.pooled = torch.zeros(N, F, dtype=torch.float32, device=dev)
+    P, pool_t = spec.pooled_features, _lib.POOL_TYPES[spec.global_pool]
+    e.pooled = torch.zeros(N, P, dtype=torch.float32, device=dev)
     e.pool_partial = torch.zeros(8 * N * F, dtype=torch.float32, device=dev)
-    fwd.append(("dfd_pool", (_ptr(x), None, None, _ptr(e.pooled), N, Hf * Wf, F, ACT_NONE, dt, _ptr(e.pool_partial), 8)))
+    if pool_t == _lib.POOL_TYPES["avg"]:
+        fwd.append(("dfd_pool", (_ptr(x), None, None, _ptr(e.pooled), N, Hf * Wf, F, ACT_NONE, dt, _ptr(e.pool_partial), 8)))
+    else:
+        e.pool_argmax = torch.zeros(N, F, dtype=torch.int32, device=dev)
+        fwd.append(("dfd_global_pool", (_ptr(x), None, None, _ptr(e.pooled), _ptr(e.pool_argmax), N, Hf * Wf, F, ACT_NONE,
+                                        pool_t, dt, 8)))
     e.logits = torch.zeros(N, K, dtype=torch.float32, device=dev)
     e.dlogits = torch.zeros(N, K, dtype=torch.float32, device=dev)
-    e.dpooled = torch.zeros(N, F, dtype=torch.float32, device=dev)
+    e.dpooled = torch.zeros(N, P, dtype=torch.float32, device=dev)
     e.target_i = torch.zeros(N, dtype=torch.int64, device=dev)
     e.target_f = torch.zeros(N, K, dtype=torch.float32, device=dev)
 
@@ -277,8 +283,11 @@ def build_resnet(e):
         return ops
 
     bwd.append(("dfd_head_bwd", (_ptr(e.dlogits), _ptr(e.pooled), P32("fc.weight"), G32("fc.weight"), G32("fc.bias"),
-                                 _ptr(e.dpooled), N, F, K)))
-    bwd.append(("dfd_pool_bwd", (_ptr(e.dpooled), gA, N, Hf * Wf, F, dt)))
+                                 _ptr(e.dpooled), N, P, K)))
+    if pool_t == _lib.POOL_TYPES["avg"]:
+        bwd.append(("dfd_pool_bwd", (_ptr(e.dpooled), gA, N, Hf * Wf, F, dt)))
+    else:
+        bwd.append(("dfd_gpool_bwd", (_ptr(e.dpooled), _ptr(e.pool_argmax), gA, N, Hf * Wf, F, pool_t, dt)))
     # The gradient entering a block is kept as up to TWO tensors (main-path dx + identity-path gm of the block above): the
     # fused ReLU / BN-backward reduction adds them on the fly (dfd_relu_bn_bwd_reduce), which removes the materialised
     # residual add of every block without a downsample branch. DFD_NO_RELU_FUSE=1 restores the three separate passes.

@@ -74,7 +74,7 @@ def init_state_dict(spec, seed=None):
             last_bn.add(b.name + (".bn2.weight" if b.kind == "basic" else ".bn3.weight"))       # resnet.py:147-148,212-213
     for name, shape, role in state_entries(spec):
         if resnet and role in ("fc_w", "fc_b"):
-            r = 1.0 / math.sqrt(spec.num_features)
+            r = 1.0 / math.sqrt(spec.pooled_features)
             sd[name] = (torch.rand(shape, generator=g) * 2 - 1) * r
             continue
         if name in last_bn:
@@ -101,7 +101,7 @@ def init_state_dict(spec, seed=None):
 
 class NativeModel(nn.Module):
     def __init__(self, arch, num_classes=2, in_chans=3, dtype="bf16", bn_momentum=None, bn_eps=None, bn_tf=False,
-                 drop_rate=0.0, drop_path_rate=0.0, gemm_impl="tc", **unused):
+                 drop_rate=0.0, drop_path_rate=0.0, gemm_impl="tc", global_pool="avg", **unused):
         super().__init__()
         if bn_tf:       # efficientnet_blocks.py:13-30
             bn_momentum = 1 - 0.99 if bn_momentum is None else bn_momentum
@@ -119,7 +119,8 @@ class NativeModel(nn.Module):
         self.allow_local_grads = False
         self.sync_bn = False                           # set by ddp.convert_syncbn_model (train.py:388-394)
         self._reducer = None
-        self.spec = get_spec(arch, num_classes=num_classes, in_chans=in_chans)
+        self.global_pool = global_pool                 # SelectAdaptivePool2d type (efficientnet.py:297-300, resnet.py:407-409)
+        self.spec = get_spec(arch, num_classes=num_classes, in_chans=in_chans, global_pool=global_pool)
         if self.spec.family != "efficientnet" and (self.drop_rate or self.drop_path_rate):
             raise _lib.NativeError("drop_rate / drop_path_rate are implemented for the EfficientNet family only")
         self.default_cfg = dict(_DEFAULT_CFG, input_size=self.spec.input_size,
@@ -135,7 +136,7 @@ class NativeModel(nn.Module):
     def _engine_kwargs(self):
         return dict(num_classes=self.num_classes, in_chans=self.in_chans, dtype=self.dtype_name, bn_momentum=self.bn_momentum,
                     bn_eps=self.bn_eps, gemm_impl=self.gemm_impl, drop_rate=self.drop_rate, drop_path_rate=self.drop_path_rate,
-                    sync_bn=self.sync_bn)
+                    sync_bn=self.sync_bn, global_pool=self.global_pool)
 
     @property
     def engine(self):
@@ -235,7 +236,7 @@ class NativeModel(nn.Module):
     def get_classifier(self):
         """efficientnet.py:307-308 / resnet.py:426-427: the classifier as an nn.Linear whose tensors alias the arenas"""
         e = self.engine
-        fc = nn.Linear(self.spec.num_features, self.num_classes)
+        fc = nn.Linear(self.spec.pooled_features, self.num_classes)
         fc.weight = nn.Parameter(e.param_view(e.cls_name + ".weight"))
         fc.bias = nn.Parameter(e.param_view(e.cls_name + ".bias"))
         return fc
@@ -243,7 +244,8 @@ class NativeModel(nn.Module):
     def __deepcopy__(self, memo):
         """ModelEma deep-copies the model (utils.py:300): the copy owns fresh arenas holding the same state"""
         kw = dict(num_classes=self.num_classes, in_chans=self.in_chans, dtype=self.dtype_name, bn_momentum=self.bn_momentum,
-                  bn_eps=self.bn_eps, drop_rate=self.drop_rate, drop_path_rate=self.drop_path_rate, gemm_impl=self.gemm_impl)
+                  bn_eps=self.bn_eps, drop_rate=self.drop_rate, drop_path_rate=self.drop_path_rate, gemm_impl=self.gemm_impl,
+                  global_pool=self.global_pool)
         m = NativeModel(self.arch, **kw)
         m.training = self.training
         if self._primary is not None:
@@ -259,7 +261,6 @@ def create_model(model_name, pretrained=False, num_classes=1000, in_chans=3, che
         raise _lib.NativeError("pretrained weights need network access; load a checkpoint instead")
     if model_name not in SUPPORTED_ARCHS:
         raise RuntimeError("Unknown model (%s)" % model_name)       # factory.py:56
-    kwargs.pop("global_pool", None)
     model = NativeModel(model_name, num_classes=num_classes, in_chans=in_chans, **kwargs)
     if checkpoint_path:
         from .helpers import load_checkpoint
@@ -271,7 +272,6 @@ def create_deepfake_model_v4(model_name, pretrained=False, num_classes=1000, in_
                              strict=True, **kwargs):
     """dfd/timm/models/factory.py:190-252 (asserts the model name, :213)."""
     assert model_name in ["efficientnet_deepfake_v4"]
-    kwargs.pop("global_pool", None)
     model = NativeModel(model_name, num_classes=num_classes, in_chans=in_chans, **kwargs)
     if checkpoint_path:
         from .helpers import load_checkpoint

@@ -35,6 +35,12 @@ extern "C" {
 #define DFD_ACT_SWISH 1
 #define DFD_ACT_RELU 2
 
+/* global pool types (layers/adaptive_avgmax_pool.py:35-48); pooled width P = F for all but CATAVGMAX (P = 2F) */
+#define DFD_POOL_AVG 0
+#define DFD_POOL_MAX 1
+#define DFD_POOL_AVGMAX 2
+#define DFD_POOL_CATAVGMAX 3
+
 /* ---- runtime ---------------------------------------------------------------------------------------- */
 const char* dfd_last_error(void);
 int dfd_abi_version(void);
@@ -165,6 +171,11 @@ int dfd_maxpool_fwd(const void* x, void* out, void* argmax_u8, int N, int H, int
 int dfd_maxpool_bwd(const void* gy, const void* argmax_u8, void* gx, int N, int H, int W, int C, int dt, void* stream);
 int dfd_relu_bwd(const void* g, const void* out, void* gm, long long numel, int dt, void* stream);
 int dfd_pool_bwd(const float* dpooled, void* dout, int N, long long hw, int C, int dt, void* stream);
+/* backward of dfd_global_pool on a stored tensor (ResNet): dout[n,hw,c] = round16(g_avg[n,c] / HW + (hw == argmax[n,c]) *
+ * g_max[n,c]), with g_avg / g_max taken from dpooled [N, P] by pool_type (MAX: 0 / dpooled; AVGMAX: both 0.5 * dpooled;
+ * CATAVGMAX: dpooled[:, :C] / dpooled[:, C:]). pool_type != DFD_POOL_AVG (that is dfd_pool_bwd). */
+int dfd_gpool_bwd(const float* dpooled, const int* argmax, void* dout, int N, long long hw, int C, int pool_type, int dt,
+                  void* stream);
 
 /* ---- BatchNorm2d (train + eval), Swish, SE gating, residual, global pool and their backward:
  *      efficientnet_blocks.py:104-110,154,166,180-194,280-348; layers/activations.py:19-33;
@@ -181,6 +192,15 @@ int dfd_bn_act(const void* y, const float* scale, const float* shift, const floa
  * forward stays bit-reproducible); NULL / max_chunks <= 1: one CTA per image */
 int dfd_pool(const void* y, const float* scale, const float* shift, float* pooled, int n, long long hw, int C,
              int act, int dt, float* partial, int max_chunks, void* stream);
+/* Selectable global pool of a = act(scale*y + shift) (fp32 on load, never stored; scale / shift NULL: a = y) in one pass:
+ *   AVG: pooled[n,c] = mean_hw a        MAX: pooled[n,c] = max_hw a        AVGMAX: 0.5f * (mean + max)
+ *   CATAVGMAX: pooled[n, 0:C] = mean, pooled[n, C:2C] = max           (pooled is [n, P])
+ * argmax [n, C] int32 (optional) receives the hw index of the max under torch's adaptive_max_pool2d rule: a value replaces
+ * the running max when it is strictly greater or NaN (ties -> first index in row-major order, NaN propagates). The mean is
+ * summed in exactly dfd_pool's order and chunk geometry, so it is bit-identical to dfd_pool's result; chunk maxima are
+ * combined in chunk order, so max and argmax do not depend on the chunking. */
+int dfd_global_pool(const void* y, const float* scale, const float* shift, float* pooled, int* argmax, int n, long long hw,
+                    int C, int act, int pool_type, int dt, int max_chunks, void* stream);
 int dfd_bn_bwd_reduce(const void* g, const void* y, const void* out, const float* mean, const float* rstd, int n,
                       long long hw, int C, int dt, double* s1, double* s2, const void* fin, void* stream);
 /* ReLU backward (and the residual add of the block above: g2 optional) fused into the reduction (ResNet block tail):
@@ -197,6 +217,12 @@ int dfd_se_bwd_reduce(const void* da, const void* y, const float* scale, const f
 int dfd_act_bwd(const void* da, const void* y, const float* scale, const float* shift, const float* mean,
                 const float* rstd, const float* gate, const float* dpool, void* gu, int n, long long hw, int C,
                 int act, int dt, double* s1, double* s2, const void* fin, void* stream);
+/* dfd_act_bwd with no da and the gradient of dfd_global_pool instead of dpool (EfficientNet head, act = Swish):
+ *   gu = (g_avg[n,c] / hw + (hw == argmax[n,c]) * g_max[n,c]) * act'(u), g_avg / g_max from dpooled [n, P] as in
+ * dfd_gpool_bwd; the BN backward sums and `fin` as in dfd_act_bwd. pool_type != DFD_POOL_AVG. */
+int dfd_act_bwd_gpool(const void* y, const float* scale, const float* shift, const float* mean, const float* rstd,
+                      const float* dpooled, const int* argmax, void* gu, int n, long long hw, int C, int act, int pool_type,
+                      int dt, double* s1, double* s2, const void* fin, void* stream);
 int dfd_add_inplace(void* a, const void* b, long long numel, int dt, void* stream);
 
 /* ---- squeeze-excite FCs: SqueezeExcite.forward, efficientnet_blocks.py:104-110 ------------------------ */

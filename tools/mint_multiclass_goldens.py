@@ -44,14 +44,15 @@ def _pick(names, k):
     return [names[i] for i in sorted({round(j * (n - 1) / (k - 1)) for j in range(k)} | {n - 2, n - 1})]
 
 
-def mint_step_k(arch, batch, H, W, num_classes, n_steps=2, smoothing=0.0, opt_name="sgd", soft=False, tag=""):
+def mint_step_k(arch, batch, H, W, num_classes, n_steps=2, smoothing=0.0, opt_name="sgd", soft=False, tag="",
+                global_pool="avg"):
     from dfd.timm.loss import LabelSmoothingCrossEntropy, SoftTargetCrossEntropy
     from dfd.timm.models import create_model
     from dfd.timm.optim import create_optimizer
     from dfd.timm.utils import accuracy
     torch.manual_seed(0)
-    spec = get_spec(arch, num_classes=num_classes)
-    model = create_model(arch, num_classes=num_classes)
+    spec = get_spec(arch, num_classes=num_classes, global_pool=global_pool)
+    model = create_model(arch, num_classes=num_classes, global_pool=global_pool)
     model.load_state_dict(synth_state(spec, seed=7), strict=True)
     model.train()
     lr = 0.01 if opt_name == "sgd" else 1e-3
@@ -68,6 +69,8 @@ def mint_step_k(arch, batch, H, W, num_classes, n_steps=2, smoothing=0.0, opt_na
     pk, bk = _pick(list(params), 6), _pick([k for k in buffers if k.endswith("running_var")], 2)
     rec = dict(arch=arch, batch=batch, H=H, W=W, num_classes=num_classes, weight_seed=7, opt=opt_name, lr=lr,
                momentum=0.9, weight_decay=wd, smoothing=smoothing, soft=soft, torch=torch.__version__, steps=[])
+    if global_pool != "avg":
+        rec["global_pool"] = global_pool
     for step in range(n_steps):
         x, y = synth_batch(batch, 3, H, W, seed=1234 + step, soft=soft, num_classes=num_classes)
         out = model(x)
