@@ -127,8 +127,9 @@ def _bn_params(C, g):
     return scale, shift
 
 
-def check_dwconv(N, H, W, C, k, s, dtype=torch.bfloat16, affine=True, seed=0, fwd_impl="dfd_dwconv_fwd"):
-    """fwd + dgrad (both modes) + wgrad against F.conv2d autograd on the rounded operands."""
+def check_dwconv(N, H, W, C, k, s, dtype=torch.bfloat16, affine=True, seed=0, fwd_impl="dfd_dwconv_fwd", add=True):
+    """fwd + dgrad (both modes) + wgrad against F.conv2d autograd on the rounded operands. add (mode 0 only): the residual
+    gradient added to the input gradient, as in a DS block with a skip connection."""
     g = torch.Generator(device="cuda").manual_seed(seed)
     pad = (k - 1) // 2
     x = torch.randn(N, H, W, C, device="cuda", generator=g).to(dtype)
@@ -153,6 +154,24 @@ def check_dwconv(N, H, W, C, k, s, dtype=torch.bfloat16, affine=True, seed=0, fw
     ref = F.conv2d(a_q, wr, stride=s, padding=pad, groups=C)
     res = dict(fwd_max=maxerr_scaled(nchw(out.float()), ref.detach()), fwd_rel=relerr(nchw(out.float()), ref.detach()),
                nan=int(torch.isnan(out.float()).sum()))
+    # Element-wise bound of the forward (fwd_ulp <= 1). The kernel's Swish is u * sigmoid_fast(u) with
+    # sigmoid_fast = fmaf(tanh.approx(u/2), 0.5, 0.5) (common.cuh:97). tanh.approx.f32 has at most 2^-10.98 relative error and
+    # |tanh| <= 1, so the sigmoid is off by < 2^-11 ABSOLUTE and the kernel's activation a' by e = |u| 2^-11 (relative to a this
+    # is unbounded for negative u). Both a' and the reference's a are then rounded to the 16-bit type:
+    # |rnd(a') - rnd(a)| <= e + ulp(max(|a|, |a'|)) <= e + ulp_in (|a| + e), with ulp_in the largest relative ulp (2^-7 bf16,
+    # 2^-10 fp16). Summed over the taps, with the output half-ulp u_out (2^-8 bf16, 2^-11 fp16) and 2^-20 for both fp32
+    # accumulations of <= 25 taps (and the reference's own fp32 Swish):
+    #   |out - ref| <= u_out |ref| + (ulp_in + 2^-20) sum_taps |w a| + (1 + ulp_in) 2^-11 sum_taps |w u|
+    # The scaled 2^-7 (|ref| + rms) bound does not follow from this arithmetic and fails once cancelling sums are sampled 10^8
+    # times; a wrong tap, channel or tile is off by a whole |w a| term and fails this one.
+    u_out, ulp_in = (2.0 ** -8, 2.0 ** -7) if dtype == torch.bfloat16 else (2.0 ** -11, 2.0 ** -10)
+    with torch.no_grad():
+        mag = F.conv2d(a_q.detach().abs(), w.abs(), stride=s, padding=pad, groups=C)
+        bound = u_out * ref.detach().abs() + (ulp_in + 2.0 ** -20) * mag
+        if affine:
+            bound += (1 + ulp_in) * 2.0 ** -11 * F.conv2d(u.detach().abs(), w.abs(), stride=s, padding=pad, groups=C)
+        res["fwd_ulp"] = float(((nchw(out.float()) - ref.detach()).abs() / (bound + 1e-30)).max())
+        del mag, bound
     of = out.double()
     res["sum_rel"] = relerr(s1.sum(0), of.sum((0, 1, 2)))
     res["sq_rel"] = relerr(s2.sum(0), (of * of).sum((0, 1, 2)))
@@ -190,48 +209,138 @@ def check_dwconv(N, H, W, C, k, s, dtype=torch.bfloat16, affine=True, seed=0, fw
         c1, c2 = stat_buf(C), stat_buf(C)
         _lib.call("dfd_dwconv_bwd", P(gy), P(out), P(cA), P(cB), P(cC), P(w), P(x), P(scale), P(shift), P(mean), P(rstd), None,
                   P(gx2), P(dW2), N, H, W, C, k, s, DT[dtype], P(c1), P(c2), None, 0, None, st())
-        # order-deterministic mode: partials in fixed slots + ordered reduce; two runs agree bit for bit, and with the atomic
-        # flush to fp32 round-off
-        import struct
-        parts = _lib.lib().cdll.dfd_dwconv_bwd_parts(N, H, W, C, k, s)
-        cw = _lib.lib().cdll.dfd_dwconv_block_channels(C)
-        cbs = (C + cw - 1) // cw
-        ws = torch.full((cbs, parts, cw * k * k), float("nan"), device="cuda")
-        dW3 = [torch.zeros_like(w), torch.zeros_like(w)]
-        for t in dW3:
-            c3, c4 = stat_buf(C), stat_buf(C)
-            _lib.call("dfd_dwconv_bwd", P(gy), P(out), P(cA), P(cB), P(cC), P(w), P(x), P(scale), P(shift), P(mean), P(rstd), None,
-                      P(gx2), P(t), N, H, W, C, k, s, DT[dtype], P(c3), P(c4), P(ws), ws.numel() * 4, None, st())
-            raw = b"".join(struct.pack("<QQqqii", P(ws) + cb * parts * cw * k * k * 4, P(t) + cb * cw * k * k * 4,
-                                       min(cw, C - cw * cb) * k * k, cw * k * k, parts, 0) for cb in range(cbs))
-            table = torch.frombuffer(bytearray(raw), dtype=torch.uint8).cuda()
-            _lib.call("dfd_ordered_reduce", P(table), cbs, P(t), (cw * k * k // 4 + 7) // 8 if parts > 64 else 1, st())
-            torch.cuda.synchronize()
-        res["det_bitwise"] = bool(torch.equal(dW3[0], dW3[1]))
-        res["det_vs_atomic"] = relerr(dW3[0], dW2)
+        torch.cuda.synchronize()
         res["fused_gx_diff"] = float((gx2.float() - gx.float()).abs().max())
         res["fused_nan"] = int(torch.isnan(gx2.float()).sum())
         res["fused_wgrad_rel"] = relerr(dW2, wr.grad)
         res["fused_bs1_rel"] = relerr(c1.sum(0), gxd.sum((0, 1, 2)))
         res["fused_bs2_rel"] = relerr(c2.sum(0), (gxd * xhat).sum((0, 1, 2)))
+        det = _dwconv_bwd_det(lambda t, ws, nbytes, gxo, d1, d2: _lib.call(
+            "dfd_dwconv_bwd", P(gy), P(out), P(cA), P(cB), P(cC), P(w), P(x), P(scale), P(shift), P(mean), P(rstd), None,
+            P(gxo), P(t), N, H, W, C, k, s, DT[dtype], P(d1), P(d2), P(ws), nbytes, None, st()), w, dW2, gx, N, H, W, C, k, s, True)
+        stats = det.pop("stats")
+        res["det_bs1_rel"] = max(relerr(d1.sum(0), gxd.sum((0, 1, 2))) for d1, _ in stats)
+        res["det_bs2_rel"] = max(relerr(d2.sum(0), (gxd * xhat).sum((0, 1, 2))) for _, d2 in stats)
+        res.update(det)
     else:
-        add = torch.randn(N, H, W, C, device="cuda", generator=g).to(dtype)
-        _lib.call("dfd_dwconv_dgrad", P(gy), P(out), P(cA), P(cB), P(cC), P(w), None, None, None, None, None, P(add), P(gx), N, H,
+        addt = torch.randn(N, H, W, C, device="cuda", generator=g).to(dtype) if add else None
+        _lib.call("dfd_dwconv_dgrad", P(gy), P(out), P(cA), P(cB), P(cC), P(w), None, None, None, None, None, P(addt), P(gx), N, H,
                   W, C, k, s, 0, DT[dtype], None, None, st())
         torch.cuda.synchronize()
-        ref_gx = xr.grad + nchw(add.float())
+        ref_gx = xr.grad + nchw(addt.float()) if add else xr.grad
         res["dgrad_max"] = maxerr_scaled(nchw(gx.float()), ref_gx)
         res["dgrad_rel"] = relerr(nchw(gx.float()), ref_gx)
-        # fused pass, mode 0 (input consumed as is, residual gradient added)
+        # fused pass, mode 0 (input consumed as is, residual gradient added when given)
         gx2 = torch.full((N, H, W, C), float("nan"), device="cuda", dtype=dtype)
         dW2 = torch.zeros_like(w)
-        _lib.call("dfd_dwconv_bwd", P(gy), P(out), P(cA), P(cB), P(cC), P(w), P(x), None, None, None, None, P(add), P(gx2), P(dW2),
+        _lib.call("dfd_dwconv_bwd", P(gy), P(out), P(cA), P(cB), P(cC), P(w), P(x), None, None, None, None, P(addt), P(gx2), P(dW2),
                   N, H, W, C, k, s, DT[dtype], None, None, None, 0, None, st())
         torch.cuda.synchronize()
         res["fused_gx_diff"] = float((gx2.float() - gx.float()).abs().max())
         res["fused_nan"] = int(torch.isnan(gx2.float()).sum())
         res["fused_wgrad_rel"] = relerr(dW2, wr.grad)
+        det = _dwconv_bwd_det(lambda t, ws, nbytes, gxo, d1, d2: _lib.call(
+            "dfd_dwconv_bwd", P(gy), P(out), P(cA), P(cB), P(cC), P(w), P(x), None, None, None, None, P(addt), P(gxo), P(t),
+            N, H, W, C, k, s, DT[dtype], None, None, P(ws), nbytes, None, st()), w, dW2, gx, N, H, W, C, k, s, False)
+        det.pop("stats")
+        res.update(det)
     res["nan_b"] = int(torch.isnan(gx.float()).sum())
+    return res
+
+
+def _dwconv_bwd_det(launch, w, dW_atomic, gx_ref, N, H, W, C, k, s, with_stats):
+    """order-deterministic mode of dfd_dwconv_bwd (partials in fixed workspace slots + dfd_ordered_reduce, as the training plan
+    runs it), launched twice, each into its own NaN-filled input gradient: the weight gradients agree bit for bit, and with the
+    atomic flush to fp32 round-off; the input gradient equals the two-pass dfd_dwconv_dgrad's (gx_ref) bit for bit, with every
+    element written; also the workspace size in bytes, and (with_stats) each run's BatchNorm backward sums"""
+    import struct
+    parts = _lib.lib().cdll.dfd_dwconv_bwd_parts(N, H, W, C, k, s)
+    cw = _lib.lib().cdll.dfd_dwconv_block_channels(C)
+    cbs = (C + cw - 1) // cw
+    ws = torch.full((cbs, parts, cw * k * k), float("nan"), device="cuda")
+    dW3 = [torch.zeros_like(w), torch.zeros_like(w)]
+    gx_diff, gx_nan, stats = 0.0, 0, []
+    for t in dW3:
+        gxo = torch.full_like(gx_ref, float("nan"))
+        d1, d2 = (stat_buf(C), stat_buf(C)) if with_stats else (None, None)
+        launch(t, ws, ws.numel() * 4, gxo, d1, d2)
+        stats.append((d1, d2))
+        raw = b"".join(struct.pack("<QQqqii", P(ws) + cb * parts * cw * k * k * 4, P(t) + cb * cw * k * k * 4,
+                                   min(cw, C - cw * cb) * k * k, cw * k * k, parts, 0) for cb in range(cbs))
+        table = torch.frombuffer(bytearray(raw), dtype=torch.uint8).cuda()
+        _lib.call("dfd_ordered_reduce", P(table), cbs, P(t), (cw * k * k // 4 + 7) // 8 if parts > 64 else 1, st())
+        torch.cuda.synchronize()
+        gx_nan += int(torch.isnan(gxo.float()).sum())
+        gx_diff = max(gx_diff, float((gxo.float() - gx_ref.float()).abs().max()))
+        del gxo
+    return dict(det_bitwise=bool(torch.equal(dW3[0], dW3[1])), det_vs_atomic=relerr(dW3[0], dW_atomic), ws_bytes=ws.numel() * 4,
+                det_gx_diff=gx_diff, det_nan=gx_nan, stats=stats)
+
+
+def check_stem_gemm(N, Cin, H, W, Cout, k, s, pad, dtype=torch.bfloat16, seed=0, pack=1):
+    """the stem as the training plan runs it (stem_impl="gemm"): dfd_stem_im2col -> dfd_pad_weight -> the tensor-core GEMM with
+    the BatchNorm statistics (pack 1: dfd_gemm_tn; else dfd_gemm_tn_rowpack on the block-diagonal copy of the padded weight,
+    the plan's form for small Kp) -> order-deterministic dfd_gemm_wgrad into the Kp-padded gradient -> dfd_unpad_grad. im2col
+    exact against F.unfold; output and weight gradient against fp64 products of the same rounded operands."""
+    import struct
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    d = DT[dtype]
+    x = torch.randn(N, Cin, H, W, device="cuda", generator=g).to(dtype)
+    taps = Cin * k * k
+    Kp = (taps + 7) // 8 * 8
+    Ho, Wo = (H + 2 * pad - k) // s + 1, (W + 2 * pad - k) // s + 1
+    M = N * Ho * Wo
+    w = (torch.randn(Cout, taps, device="cuda", generator=g) / math.sqrt(taps)).to(dtype)
+    wpad = torch.full((Cout, Kp), float("nan"), device="cuda", dtype=dtype)
+    _lib.call("dfd_pad_weight", P(w), P(wpad), Cout, taps, Kp, d, st())
+    cols = torch.full((M, Kp), float("nan"), device="cuda", dtype=dtype)
+    _lib.call("dfd_stem_im2col", P(x), P(cols), N, Cin, H, W, k, s, pad, Kp, d, st())
+    y = torch.full((M, Cout), float("nan"), device="cuda", dtype=dtype)
+    s1, s2 = stat_buf(Cout), stat_buf(Cout)
+    if pack == 1:
+        _lib.call("dfd_gemm_tn", P(cols), P(wpad), P(y), M, Cout, Kp, d, P(s1), P(s2), None, st())
+    else:
+        Bd = torch.full((pack * Cout, pack * Kp), float("nan"), device="cuda", dtype=dtype)
+        table = torch.frombuffer(bytearray(struct.pack("<QQiiii", P(wpad), P(Bd), Cout, Kp, pack, 0)), dtype=torch.uint8).cuda()
+        _lib.call("dfd_blockdiag_weights", P(table), 1, d, st())
+        _lib.call("dfd_gemm_tn_rowpack", P(cols), P(Bd), P(y), M, Cout, Kp, pack, d, P(s1), P(s2), None, st())
+    torch.cuda.synchronize()
+    res = dict(wpad_diff=float((wpad[:, :taps].float() - w.float()).abs().max()), wpad_tail=float(wpad[:, taps:].float().abs().max()) if Kp > taps else 0.0,
+               cols_nan=int(torch.isnan(cols).sum()), cols_tail=float(cols[:, taps:].float().abs().max()) if Kp > taps else 0.0)
+    # im2col, exact; chunked over images so that the fp32 unfold stays small
+    diff = 0.0
+    per = max(1, (64 << 20) // (taps * Ho * Wo))
+    for n0 in range(0, N, per):
+        n1 = min(N, n0 + per)
+        ref = F.unfold(x[n0:n1].float(), k, padding=pad, stride=s).transpose(1, 2).reshape(-1, taps)
+        diff = max(diff, float((cols[n0 * Ho * Wo:n1 * Ho * Wo, :taps].float() - ref).abs().max()))
+        del ref
+    res["cols_diff"] = diff
+    ref_y = cols[:, :taps].double() @ w.double().t()
+    res.update(fwd_max=maxerr_scaled(y.float(), ref_y), nan=int(torch.isnan(y).sum()))
+    del ref_y
+    yd = y.double()
+    res["sum_rel"] = relerr(s1.sum(0), yd.sum(0))
+    res["sq_rel"] = relerr(s2.sum(0), (yd * yd).sum(0))
+    del yd
+    gy = (torch.randn(M, Cout, device="cuda", generator=g) * 0.1).to(dtype)
+    splits = _lib.lib().cdll.dfd_gemm_wgrad_splits(M, Cout, Kp)
+    ws = torch.full((splits, Cout, Kp), float("nan"), device="cuda")
+    gws = []
+    base = torch.randn(Cout, taps, device="cuda", generator=g)        # dfd_unpad_grad accumulates into the gradient arena
+    for _ in range(2):
+        gpad = torch.zeros(Cout, Kp, device="cuda")
+        gw = base.clone()
+        _lib.call("dfd_gemm_wgrad", P(gy), P(cols), P(gpad), M, Cout, Kp, d, P(ws), ws.numel() * 4, st())
+        table = torch.frombuffer(bytearray(struct.pack("<QQqqii", P(ws), P(gpad), Cout * Kp, Cout * Kp, splits, 0)), dtype=torch.uint8).cuda()
+        _lib.call("dfd_ordered_reduce", P(table), 1, P(gpad), min(1024, (Cout * Kp // 4 + 255) // 256), st())
+        _lib.call("dfd_unpad_grad", P(gpad), P(gw), Cout, taps, Kp, st())
+        torch.cuda.synchronize()
+        gws.append(gw)
+    res["wgrad_rel"] = relerr(gws[0].double() - base.double(), gy.double().t() @ cols[:, :taps].double())
+    res["wgrad_bitwise"] = bool(torch.equal(gws[0], gws[1]))
+    res["wgrad_nan"] = int(torch.isnan(gws[0]).sum())
+    res["splits"] = splits
     return res
 
 
@@ -349,6 +458,117 @@ def check_bn_chain(N, HW, C, dtype=torch.bfloat16, seed=0):
     res["reduce2_rel"] = relerr(c2.sum(0), (da.double() * xhat).sum((0, 1)))
     res["draw_rel"] = relerr(draw, (da.float().permute(0, 2, 1) * sw.squeeze(-1).detach()).sum(2))
     res["nan"] = int(torch.isnan(dy.float()).sum() + torch.isnan(a2.float()).sum())
+    return res
+
+
+ROW_KERNELS = ("dfd_bn_act", "dfd_act_bwd", "dfd_pool", "dfd_bn_bwd_reduce", "dfd_bn_bwd_apply", "dfd_se_bwd_reduce")
+
+
+def _act_ref(u, act):
+    """act(u) and act'(u) in fp64 (DFD_ACT_NONE / SWISH / RELU)"""
+    if act == 1:
+        s = torch.sigmoid(u)
+        return u * s, s * (1 + u * (1 - s))
+    if act == 2:
+        return u.clamp_min(0), (u > 0).double()
+    return u, torch.ones_like(u)
+
+
+def check_row_kernel(kernel, N, HW, C, args, ptrs, dtype=torch.bfloat16, seed=0):
+    """One launch of a per-row BatchNorm / activation / pool / SE kernel exactly as a plan issues it: `args` are its non-pointer
+    arguments after (n, hw, C) with the dtype left out, `ptrs` its pointer-presence mask ('p' / '0' per pointer argument, ABI
+    order; see tests/plan_launches.py), so the activation, residual mode and optional operands select the same instantiation.
+    Reference: fp64 on the same rounded operands, with u = scale*y + shift rounded to fp32 once (the kernel's fmaf)."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    d = DT[dtype]
+    has = lambda i: ptrs[i] == "p"
+    y = (torch.randn(N, HW, C, device="cuda", generator=g) * 1.5 + 0.3).to(dtype)
+    scale, shift = _bn_params(C, g)
+    mean = 0.1 * torch.randn(C, device="cuda", generator=g)
+    rstd = 1.0 + 0.1 * torch.rand(C, device="cuda", generator=g)
+    gate = torch.sigmoid(torch.randn(N, C, device="cuda", generator=g))
+    yd = y.double()
+    xhat = (yd - mean.double()) * rstd.double()
+    res = {}
+
+    def u_of(with_scale):
+        return (yd * scale.double() + shift.double()).float().double() if with_scale else yd
+
+    def sums(v):
+        return v.sum((0, 1)), (v * xhat).sum((0, 1))
+
+    if kernel == "dfd_bn_act":
+        act, res_mode = args[0], args[1]
+        r = torch.randn(N, HW, C, device="cuda", generator=g).to(dtype) if has(4) else None
+        out = torch.full_like(y, float("nan"))
+        _lib.call(kernel, P(y), P(scale) if has(1) else None, P(shift) if has(2) else None, P(gate) if has(3) else None,
+                  P(r), P(out), N, HW, C, act, res_mode, d, st())
+        torch.cuda.synchronize()
+        ref = _act_ref(u_of(has(1)), act)[0]
+        if has(3):
+            ref = ref * gate.double().unsqueeze(1)
+        if res_mode:
+            ref = ref + r.double()
+        if res_mode == 2:
+            ref = ref.clamp_min(0)
+        res.update(out_max=maxerr_scaled(out.float(), ref), nan=int(torch.isnan(out.float()).sum()))
+    elif kernel == "dfd_act_bwd":
+        act = args[0]
+        da = (torch.randn(N, HW, C, device="cuda", generator=g) * 0.1).to(dtype) if has(0) else None
+        dpool = torch.randn(N, C, device="cuda", generator=g) * 0.1 if has(7) else None
+        gu = torch.full_like(y, float("nan"))
+        s1, s2 = (stat_buf(C), stat_buf(C)) if has(9) else (None, None)
+        _lib.call(kernel, P(da), P(y), P(scale), P(shift), P(mean), P(rstd), P(gate) if has(6) else None, P(dpool), P(gu), N, HW, C,
+                  act, d, P(s1), P(s2), None, st())
+        torch.cuda.synchronize()
+        gin = torch.zeros_like(yd)
+        if has(0):
+            gin = da.double() * (gate.double().unsqueeze(1) if has(6) else 1.0)
+        if has(7):
+            gin = gin + dpool.double().unsqueeze(1) / HW
+        ref = gin * _act_ref(u_of(True), act)[1]
+        res.update(out_max=maxerr_scaled(gu.float(), ref), nan=int(torch.isnan(gu.float()).sum()))
+        if has(9):      # the BatchNorm backward sums of the STORED gradient
+            r1, r2 = sums(gu.double())
+            res.update(s1_rel=relerr(s1.sum(0), r1), s2_rel=relerr(s2.sum(0), r2))
+    elif kernel == "dfd_pool":
+        act, chunks = args[0], args[1]
+        pooled = [torch.full((N, C), float("nan"), device="cuda") for _ in range(2)]
+        for t in pooled:
+            _lib.call(kernel, P(y), P(scale) if has(1) else None, P(shift) if has(2) else None, P(t), N, HW, C, act, d, None, chunks, st())
+        torch.cuda.synchronize()
+        ref = _act_ref(u_of(has(1)), act)[0].mean(1)
+        res.update(pool_rel=relerr(pooled[0], ref), repro=bool(torch.equal(pooled[0], pooled[1])), nan=int(torch.isnan(pooled[0]).sum()))
+    elif kernel == "dfd_bn_bwd_reduce":
+        gr = (torch.randn(N, HW, C, device="cuda", generator=g) * 0.1).to(dtype)
+        out = torch.relu(torch.randn(N, HW, C, device="cuda", generator=g)).to(dtype) if has(2) else None
+        s1, s2 = stat_buf(C), stat_buf(C)
+        _lib.call(kernel, P(gr), P(y), P(out), P(mean), P(rstd), N, HW, C, d, P(s1), P(s2), None, st())
+        torch.cuda.synchronize()
+        gm = gr.double() * ((out.double() > 0).double() if has(2) else 1.0)
+        r1, r2 = sums(gm)
+        res.update(s1_rel=relerr(s1.sum(0), r1), s2_rel=relerr(s2.sum(0), r2), nan=0)
+    elif kernel == "dfd_bn_bwd_apply":
+        gr = (torch.randn(N, HW, C, device="cuda", generator=g) * 0.1).to(dtype)
+        out = torch.relu(torch.randn(N, HW, C, device="cuda", generator=g)).to(dtype) if has(2) else None
+        cA = 1.0 + 0.1 * torch.randn(C, device="cuda", generator=g)
+        cB = 0.05 * torch.randn(C, device="cuda", generator=g)
+        cC = 0.01 * torch.randn(C, device="cuda", generator=g)
+        dy = torch.full_like(y, float("nan"))
+        _lib.call(kernel, P(gr), P(y), P(out), P(cA), P(cB), P(cC), P(dy), N, HW, C, d, st())
+        torch.cuda.synchronize()
+        gm = gr.double() * ((out.double() > 0).double() if has(2) else 1.0)
+        ref = cA.double() * gm + cB.double() * yd + cC.double()
+        res.update(out_max=maxerr_scaled(dy.float(), ref), nan=int(torch.isnan(dy.float()).sum()))
+    elif kernel == "dfd_se_bwd_reduce":
+        da = (torch.randn(N, HW, C, device="cuda", generator=g) * 0.1).to(dtype)
+        draw = torch.full((N, C), float("nan"), device="cuda")
+        _lib.call(kernel, P(da), P(y), P(scale), P(shift), P(draw), N, HW, C, d, st())
+        torch.cuda.synchronize()
+        ref = (da.double() * _act_ref(u_of(True), 1)[0]).sum(1)
+        res.update(draw_rel=relerr(draw, ref), nan=int(torch.isnan(draw).sum()))
+    else:
+        raise KeyError(kernel)
     return res
 
 
