@@ -67,6 +67,10 @@ SIGNATURES = {
     "dfd_rng_masks": "pip" "p",
     "dfd_rng_tick": "p" "p",
     "dfd_mul_f32": "ppl" "p",
+    "dfd_drop_block_masks": "pip" "p",
+    "dfd_bn_act_drop": "pppppl" "ppp" "ili" "ii" "p",
+    "dfd_act_bwd_drop": "pppppp" "ppl" "p" "ili" "i" "pp" "p",
+    "dfd_relu_bn_bwd_reduce_drop": "ppppp" "ppl" "p" "p" "pp" "ili" "i" "pp" "p",
     "dfd_cast_arena": "pp" "li" "p",
     "dfd_check_finite": "p" "l" "pp",
     "dfd_update_loss_scale": "ppp" "i" "pp",

@@ -809,6 +809,217 @@ __global__ void add_inplace_kernel(T* __restrict__ a, const T* __restrict__ b, s
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// DropBlock (layers/drop.py:24-63) on the ResNet BatchNorm outputs, resnet.py:153-162,218-233: the block mask m (uint8 NHWC,
+// dfd_drop_block_masks) and the normalising scale s = numel / (sum m + 1e-7), evaluated as torch evaluates
+// `numel / tensor` (reciprocal, then the product) from the exact kept count in device memory - so one captured graph stays
+// valid across steps.  ms = m ? s : 0 multiplies the BN output u = scale*y + shift.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ float drop_block_scale(const unsigned long long* kept, long long numel) {
+    return __fmul_rn(__frcp_rn(__fadd_rn((float)*kept, 1e-7f)), (float)numel);
+}
+
+__device__ __forceinline__ void unpack_mask8(const uint2 raw, float s, float* ms) {
+#pragma unroll
+    for (int i = 0; i < 8; i++) ms[i] = ((i < 4 ? raw.x >> (8 * i) : raw.y >> (8 * (i - 4))) & 0xffu) ? s : 0.f;
+}
+
+// forward.  RES 0: out = relu(u * ms [* gate[n,c]]);  RES 2: out = relu(u * ms [* gate[n,c]] + res)   (block tail with
+// the drop-path gate, resnet.py:172-173,243-244)
+template <typename T, bool GATE, int RES>
+__global__ void bn_act_drop_kernel(const T* __restrict__ y, const float* __restrict__ scale, const float* __restrict__ shift,
+                                   const unsigned char* __restrict__ mask, const unsigned long long* __restrict__ kept,
+                                   long long numel, const float* __restrict__ gate, const T* __restrict__ res,
+                                   T* __restrict__ out, long long hw, int rows_per_block) {
+    const int V = blockDim.x, C = V * 8;
+    const int c0 = threadIdx.x * 8;
+    float sc[8], sh[8], gt[8];
+    ldg_f8(scale + c0, sc);
+    ldg_f8(shift + c0, sh);
+    ldg_f8(GATE ? gate + (size_t)blockIdx.y * C + c0 : nullptr, gt, 1.f);
+    const float s = drop_block_scale(kept, numel);
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    long long r1 = r0 + rows_per_block;
+    if (r1 > hw) r1 = hw;
+    const size_t img = (size_t)blockIdx.y * hw * C + c0;
+    constexpr int U = RES ? 2 : 4;
+    for (long long r = r0 + threadIdx.y; r < r1; r += (long long)U * blockDim.y) {
+        uint4 raw[U], rraw[U];
+        uint2 mraw[U];
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+            const long long rr = r + (long long)u * blockDim.y;
+            if (rr < r1) {
+                raw[u] = ldg16(y + img + (size_t)rr * C);
+                mraw[u] = __ldg(reinterpret_cast<const uint2*>(mask + img + (size_t)rr * C));
+                if (RES) rraw[u] = ldg16(res + img + (size_t)rr * C);
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+            const long long rr = r + (long long)u * blockDim.y;
+            if (rr >= r1) break;
+            float f[8], ms[8];
+            unpack8<T>(raw[u], f);
+            unpack_mask8(mraw[u], s, ms);
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                f[i] = fmaf(f[i], sc[i], sh[i]) * ms[i];
+                if (GATE) f[i] *= gt[i];
+            }
+            if (RES) {
+                float g[8];
+                unpack8<T>(rraw[u], g);
+#pragma unroll
+                for (int i = 0; i < 8; i++) f[i] += g[i];
+            }
+#pragma unroll
+            for (int i = 0; i < 8; i++) f[i] = fmaxf(f[i], 0.f);
+            stg16(out + img + (size_t)rr * C, pack8<T>(f));
+        }
+    }
+}
+
+// backward through a dropped BN + ReLU site: gu = round16(da * ms) * (u > 0), stored and reduced for the BN backward
+// (s1 += sum gu, s2 += sum gu * xhat), as act_bwd_kernel reduces the stored value
+template <typename T>
+__global__ void act_bwd_drop_kernel(const T* __restrict__ da, const T* __restrict__ y, const float* __restrict__ scale,
+                                    const float* __restrict__ shift, const float* __restrict__ mean,
+                                    const float* __restrict__ rstd, const unsigned char* __restrict__ mask,
+                                    const unsigned long long* __restrict__ kept, long long numel, T* __restrict__ gu,
+                                    long long hw, int rows_per_block, double* __restrict__ s1, double* __restrict__ s2) {
+    extern __shared__ float sm[];
+    const int V = blockDim.x, C = V * 8;
+    const int c0 = threadIdx.x * 8;
+    float sc[8], sh[8], mu[8], rs[8], a1[8], a2[8];
+    ldg_f8(scale + c0, sc);
+    ldg_f8(shift + c0, sh);
+    ldg_f8(mean + c0, mu);
+    ldg_f8(rstd + c0, rs);
+#pragma unroll
+    for (int i = 0; i < 8; i++) { a1[i] = 0.f; a2[i] = 0.f; mu[i] = -mu[i] * rs[i]; }
+    const float s = drop_block_scale(kept, numel);
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    long long r1 = r0 + rows_per_block;
+    if (r1 > hw) r1 = hw;
+    const size_t img = (size_t)blockIdx.y * hw * C + c0;
+    constexpr int U = 2;
+    for (long long r = r0 + threadIdx.y; r < r1; r += (long long)U * blockDim.y) {
+        uint4 draw_[U], yraw[U];
+        uint2 mraw[U];
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+            const long long rr = r + (long long)u * blockDim.y;
+            if (rr < r1) {
+                const size_t off = img + (size_t)rr * C;
+                draw_[u] = ldg16(da + off);
+                yraw[u] = ldg16(y + off);
+                mraw[u] = __ldg(reinterpret_cast<const uint2*>(mask + off));
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+            const long long rr = r + (long long)u * blockDim.y;
+            if (rr >= r1) break;
+            float d[8], f[8], ms[8];
+            unpack8<T>(draw_[u], d);
+            unpack8<T>(yraw[u], f);
+            unpack_mask8(mraw[u], s, ms);
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                const float uu = fmaf(f[i], sc[i], sh[i]);
+                const float o = uu > 0.f ? round_t<T>(d[i] * ms[i]) : 0.f;
+                d[i] = o;
+                a1[i] += o;
+                a2[i] = fmaf(o, fmaf(f[i], rs[i], mu[i]), a2[i]);      // xhat = (y - mean) * rstd
+            }
+            stg16(gu + img + (size_t)rr * C, pack8<T>(d));
+        }
+    }
+    double* p1 = stat_slot(s1, C);
+    double* p2 = stat_slot(s2, C);
+    reduce_rows_and_emit(sm, a1, [&](int c, float v) { atomicAdd(p1 + c, (double)v); });
+    reduce_rows_and_emit(sm, a2, [&](int c, float v) { atomicAdd(p2 + c, (double)v); });
+}
+
+// block tail backward with DropBlock and / or drop path: gm = round16(g + g2) * (out > 0) is stored unmasked (the identity /
+// downsample path's gradient); the main branch's last BN sees gd = round16(gm * ms * gate[n,c]), stored and reduced
+template <typename T, bool MASK, bool GATE>
+__global__ void relu_bn_bwd_reduce_drop_kernel(const T* __restrict__ g, const T* __restrict__ g2, const T* __restrict__ y,
+                                               const T* __restrict__ out, T* __restrict__ gm_out,
+                                               const unsigned char* __restrict__ mask,
+                                               const unsigned long long* __restrict__ kept, long long numel,
+                                               const float* __restrict__ gate, T* __restrict__ gd_out,
+                                               const float* __restrict__ mean, const float* __restrict__ rstd, long long hw,
+                                               int rows_per_block, double* __restrict__ s1, double* __restrict__ s2) {
+    extern __shared__ float sm[];
+    const int V = blockDim.x, C = V * 8;
+    const int c0 = threadIdx.x * 8;
+    float mu[8], rs[8], gt[8], a1[8], a2[8];
+#pragma unroll
+    for (int i = 0; i < 8; i++) { a1[i] = 0.f; a2[i] = 0.f; }
+    ldg_f8(mean + c0, mu);
+    ldg_f8(rstd + c0, rs);
+    ldg_f8(GATE ? gate + (size_t)blockIdx.y * C + c0 : nullptr, gt, 1.f);
+    const float s = MASK ? drop_block_scale(kept, numel) : 1.f;
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    long long r1 = r0 + rows_per_block;
+    if (r1 > hw) r1 = hw;
+    const size_t img = (size_t)blockIdx.y * hw * C + c0;
+    constexpr int U = 2;
+    for (long long r = r0 + threadIdx.y; r < r1; r += (long long)U * blockDim.y) {
+        uint4 graw[U], yraw[U], oraw[U], g2raw[U];
+        uint2 mraw[U];
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+            const long long rr = r + (long long)u * blockDim.y;
+            if (rr < r1) {
+                const size_t off = img + (size_t)rr * C;
+                graw[u] = ldg16(g + off);
+                yraw[u] = ldg16(y + off);
+                oraw[u] = ldg16(out + off);
+                if (g2) g2raw[u] = ldg16(g2 + off);
+                if (MASK) mraw[u] = __ldg(reinterpret_cast<const uint2*>(mask + off));
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+            const long long rr = r + (long long)u * blockDim.y;
+            if (rr >= r1) break;
+            const size_t off = img + (size_t)rr * C;
+            float gg[8], yy[8], oo[8], ms[8];
+            unpack8<T>(graw[u], gg);
+            unpack8<T>(yraw[u], yy);
+            unpack8<T>(oraw[u], oo);
+            if (g2) {
+                float hh[8];
+                unpack8<T>(g2raw[u], hh);
+#pragma unroll
+                for (int i = 0; i < 8; i++) gg[i] = round_t<T>(gg[i] + hh[i]);
+            }
+#pragma unroll
+            for (int i = 0; i < 8; i++) gg[i] = oo[i] > 0.f ? gg[i] : 0.f;
+            stg16(gm_out + off, pack8<T>(gg));
+            if (MASK) unpack_mask8(mraw[u], s, ms);
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                float o = gg[i];
+                if (MASK) o *= ms[i];
+                if (GATE) o *= gt[i];
+                o = round_t<T>(o);
+                gg[i] = o;
+                a1[i] += o;
+                a2[i] = fmaf(o, (yy[i] - mu[i]) * rs[i], a2[i]);
+            }
+            stg16(gd_out + off, pack8<T>(gg));
+        }
+    }
+    double* p1 = stat_slot(s1, C);
+    double* p2 = stat_slot(s2, C);
+    reduce_rows_and_emit(sm, a1, [&](int c, float v) { atomicAdd(p1 + c, (double)v); });
+    reduce_rows_and_emit(sm, a2, [&](int c, float v) { atomicAdd(p2 + c, (double)v); });
+}
+
 static size_t reduce_smem(const RowGeom& g) { return (size_t)g.block.x * 8 * g.block.y * sizeof(float); }
 
 }  // namespace
@@ -860,6 +1071,7 @@ int dfd_bn_act(const void* y, const float* scale, const float* shift, const floa
             case 2: LAUNCH(0, false, 2); break;
             case 10: LAUNCH(0, true, 0); break;        // drop-path scaling of a gradient (unit affine, per-sample gate)
             case 11: LAUNCH(0, true, 1); break;        // block tail with drop path: (scale*y + shift) * gate[n] + residual
+            case 12: LAUNCH(0, true, 2); break;        // ResNet block tail with drop path: relu((scale*y + shift) * gate[n] + residual)
             case 100: LAUNCH(1, false, 0); break;
             case 110: LAUNCH(1, true, 0); break;
             case 200: LAUNCH(2, false, 0); break;
@@ -1115,6 +1327,65 @@ int dfd_act_bwd_gpool(const void* y, const float* scale, const float* shift, con
         else act_bwd_kernel<T, 1, false, 256, 2, true><<<g.grid, g.block, smem_ab, st>>>(GARGS);
     });
 #undef GARGS
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+int dfd_bn_act_drop(const void* y, const float* scale, const float* shift, const unsigned char* mask,
+                    const unsigned long long* kept, long long numel, const float* gate, const void* res, void* out, int n,
+                    long long hw, int C, int res_mode, int dt, void* stream) {
+    if (C % 8 || C <= 0 || hw <= 0 || n <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_bn_act_drop: C%8, sizes");
+    if (res_mode != 0 && res_mode != 2) return dfd_set_error(DFD_ERR_ARG, "dfd_bn_act_drop: res_mode");
+    if ((res_mode != 0) != (res != nullptr)) return dfd_set_error(DFD_ERR_ARG, "dfd_bn_act_drop: res/res_mode");
+    if (!scale || !shift) return dfd_set_error(DFD_ERR_ARG, "dfd_bn_act_drop: operands");
+    // no mask (eval mode): the plain BN + ReLU or block tail, exactly as the undropped plan computes it
+    if (!mask) return dfd_bn_act(y, scale, shift, gate, res, out, n, hw, C, res_mode ? DFD_ACT_NONE : DFD_ACT_RELU, res_mode, dt, stream);
+    if (!kept || numel <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_bn_act_drop: kept count");
+    RowGeom g = make_geom(C, hw, n, DFD_SMS * 6, row_maxt(hw, false));
+    cudaStream_t st = (cudaStream_t)stream;
+#define LAUNCH(GATE, RES)                                                                                            \
+    bn_act_drop_kernel<T, GATE, RES><<<g.grid, g.block, 0, st>>>((const T*)y, scale, shift, mask, kept, numel, gate, \
+                                                                  (const T*)res, (T*)out, hw, g.rows_per_block)
+    DISPATCH_T(dt, {
+        if (res_mode == 0) { if (gate) LAUNCH(true, 0); else LAUNCH(false, 0); }
+        else { if (gate) LAUNCH(true, 2); else LAUNCH(false, 2); }
+    });
+#undef LAUNCH
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+int dfd_act_bwd_drop(const void* da, const void* y, const float* scale, const float* shift, const float* mean,
+                     const float* rstd, const unsigned char* mask, const unsigned long long* kept, long long numel, void* gu,
+                     int n, long long hw, int C, int dt, double* s1, double* s2, void* stream) {
+    if (C % 8 || C <= 0 || hw <= 0 || n <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_act_bwd_drop: C%8, sizes");
+    if (!da || !mask || !kept || numel <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_act_bwd_drop: operands");
+    RowGeom g = make_geom(C, hw, n, DFD_SMS * 6, row_maxt(hw, false));
+    cudaStream_t st = (cudaStream_t)stream;
+    DISPATCH_T(dt, (act_bwd_drop_kernel<T><<<g.grid, g.block, reduce_smem(g), st>>>((const T*)da, (const T*)y, scale, shift, mean, rstd,
+                                                                                    mask, kept, numel, (T*)gu, hw, g.rows_per_block, s1, s2)));
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+int dfd_relu_bn_bwd_reduce_drop(const void* g_, const void* g2, const void* y, const void* out, void* gm,
+                                const unsigned char* mask, const unsigned long long* kept, long long numel, const float* gate,
+                                void* gd, const float* mean, const float* rstd, int n, long long hw, int C, int dt, double* s1,
+                                double* s2, void* stream) {
+    if (C % 8 || C <= 0 || hw <= 0 || n <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_relu_bn_bwd_reduce_drop: C%8, sizes");
+    if (!out || !gm || !gd || (!mask && !gate)) return dfd_set_error(DFD_ERR_ARG, "dfd_relu_bn_bwd_reduce_drop: operands");
+    if (mask && (!kept || numel <= 0)) return dfd_set_error(DFD_ERR_ARG, "dfd_relu_bn_bwd_reduce_drop: kept count");
+    RowGeom g = make_geom(C, hw, n, DFD_SMS * 6, row_maxt(hw, false));
+    cudaStream_t st = (cudaStream_t)stream;
+#define LAUNCH(MASK, GATE)                                                                                                      \
+    relu_bn_bwd_reduce_drop_kernel<T, MASK, GATE><<<g.grid, g.block, reduce_smem(g), st>>>(                                      \
+        (const T*)g_, (const T*)g2, (const T*)y, (const T*)out, (T*)gm, mask, kept, numel, gate, (T*)gd, mean, rstd, hw,        \
+        g.rows_per_block, s1, s2)
+    DISPATCH_T(dt, {
+        if (mask) { if (gate) LAUNCH(true, true); else LAUNCH(true, false); }
+        else LAUNCH(false, true);
+    });
+#undef LAUNCH
     DFD_LAUNCH_CHECK();
     return DFD_OK;
 }

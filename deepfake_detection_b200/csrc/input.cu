@@ -87,6 +87,103 @@ __global__ void rng_masks_kernel(const MaskDesc* __restrict__ table, const long 
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// DropBlock block masks (drop_block_2d, dfd/timm/models/layers/drop.py:24-63), one site per grid row
+// ---------------------------------------------------------------------------------------------
+struct DropBlockDesc {
+    unsigned char* mask;        // [N, H, W, C] block mask: 1 kept, 0 dropped
+    float* noise;               // optional [N, H, W, C]: the uniform draws
+    unsigned long long* kept;   // number of ones in mask (zeroed before the launch)
+    double gamma;               // seed drop rate, as the reference computes it in double
+    int N, H, W, C;
+    int cb;                     // clipped block size (odd, <= DB_MAX_CB)
+    int stream;                 // generator stream id of the site
+    int _pad[2];
+};
+
+constexpr int DB_TILE = 16;     // output pixels per tile side
+constexpr int DB_CG = 32;       // channels per tile (consecutive bytes of an NHWC pixel)
+constexpr int DB_MAX_CB = 7;
+constexpr int DB_HALO = DB_TILE + DB_MAX_CB - 1;
+
+// One CTA walks tiles of [DB_TILE x DB_TILE pixels x DB_CG channels] of one image. It stages the seeds of the tile and its
+// halo in shared memory (each uniform is drawn once per tile), takes the min over the cb columns, then over the cb rows
+// (min of 0/1 = AND; pixels outside the map are ignored, as max_pool2d's implicit -inf padding is), and counts the ones.
+// seed = (2 - gamma - valid + u) >= 1 in the reference's fp32 order; valid follows the reference's [W, H] meshgrid reshaped
+// to [H, W]: pixel (h, w) reads entry f = h*W + w of the [W, H] grid, i.e. (i, j) = (f / H, f % H).
+__global__ void __launch_bounds__(256) drop_block_kernel(const DropBlockDesc* __restrict__ table,
+                                                         const long long* __restrict__ state) {
+    __shared__ unsigned char seeds[DB_HALO][DB_HALO][DB_CG];
+    __shared__ unsigned char rowmin[DB_HALO][DB_TILE][DB_CG];
+    __shared__ unsigned long long warp_cnt[8];
+    const DropBlockDesc d = table[blockIdx.y];
+    const unsigned long long seed = (unsigned long long)state[0], step = (unsigned long long)state[1];
+    const int H = d.H, W = d.W, C = d.C, cb = d.cb, r = cb / 2;
+    const float a = (float)(2.0 - d.gamma);
+    const int lo = cb / 2, hi_w = W - (cb - 1) / 2, hi_h = H - (cb - 1) / 2;
+    const int th_n = (H + DB_TILE - 1) / DB_TILE, tw_n = (W + DB_TILE - 1) / DB_TILE, cg_n = (C + DB_CG - 1) / DB_CG;
+    const long long ntiles = (long long)d.N * th_n * tw_n * cg_n;
+    const int c_l = threadIdx.x % DB_CG, p_l = threadIdx.x / DB_CG, p_step = blockDim.x / DB_CG;
+    unsigned long long cnt = 0;
+    for (long long t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const int cg = (int)(t % cg_n);
+        long long q = t / cg_n;
+        const int tw = (int)(q % tw_n); q /= tw_n;
+        const int th = (int)(q % th_n);
+        const int n = (int)(q / th_n);
+        const int h0 = th * DB_TILE, w0 = tw * DB_TILE, c = cg * DB_CG + c_l;
+        const int oh_n = min(DB_TILE, H - h0), ow_n = min(DB_TILE, W - w0);
+        const int hh_n = oh_n + cb - 1, ww_n = ow_n + cb - 1;
+        for (int p = p_l; p < hh_n * ww_n; p += p_step) {
+            const int hh = p / ww_n, ww = p - hh * ww_n;
+            const int h = h0 - r + hh, w = w0 - r + ww;
+            unsigned char s = 1;
+            if (h >= 0 && h < H && w >= 0 && w < W && c < C) {
+                const int f = h * W + w, i = f / H, j = f - (f / H) * H;
+                const bool valid = i >= lo && i < hi_w && j >= lo && j < hi_h;
+                // outside `valid` the seed is (a + u >= 1) with u >= 0: always kept when a >= 1, so no draw is needed there
+                // (the draws do not depend on which elements are drawn: with the noise output every element is drawn)
+                if (valid || a < 1.f || d.noise) {
+                    const unsigned long long idx = (((unsigned long long)n * H + h) * W + w) * C + c;
+                    const float u = uniform01(seed, step, (unsigned)d.stream, idx);
+                    const float v = __fadd_rn(__fsub_rn(a, valid ? 1.f : 0.f), u);
+                    s = v >= 1.f ? 1 : 0;
+                    if (d.noise && hh >= r && hh < r + oh_n && ww >= r && ww < r + ow_n) d.noise[idx] = u;
+                }
+            }
+            seeds[hh][ww][c_l] = s;
+        }
+        __syncthreads();
+        for (int p = p_l; p < hh_n * ow_n; p += p_step) {
+            const int hh = p / ow_n, ow = p - hh * ow_n;
+            unsigned char m = 1;
+            for (int k = 0; k < cb; k++) m &= seeds[hh][ow + k][c_l];
+            rowmin[hh][ow][c_l] = m;
+        }
+        __syncthreads();
+        if (c < C) {
+            for (int p = p_l; p < oh_n * ow_n; p += p_step) {
+                const int oh = p / ow_n, ow = p - oh * ow_n;
+                unsigned char m = 1;
+                for (int k = 0; k < cb; k++) m &= rowmin[oh + k][ow][c_l];
+                d.mask[(((size_t)n * H + h0 + oh) * W + w0 + ow) * C + c] = m;
+                cnt += m;
+            }
+        }
+        __syncthreads();
+    }
+    // exact count: integer sums do not depend on the order of the CTAs
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    if ((threadIdx.x & 31) == 0) warp_cnt[threadIdx.x >> 5] = cnt;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        unsigned long long s = 0;
+        for (int i = 0; i < (int)(blockDim.x >> 5); i++) s += warp_cnt[i];
+        if (s) atomicAdd(d.kept, s);
+    }
+}
+
 __global__ void rng_tick_kernel(long long* __restrict__ state) { state[1] += 1; }
 
 __global__ void mul_f32_kernel(float* __restrict__ a, const float* __restrict__ b, size_t n) {
@@ -130,6 +227,15 @@ int dfd_rng_masks(const void* table, int count, const long long* state, void* st
     if (count <= 0) return DFD_OK;
     if (!table || !state) return dfd_set_error(DFD_ERR_ARG, "dfd_rng_masks: operands");
     rng_masks_kernel<<<dim3(8, count), 256, 0, (cudaStream_t)stream>>>((const MaskDesc*)table, state);
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+// table: device array of DropBlockDesc (64 bytes each, see include/dfd_b200.h); every `kept` slot must be zero on entry
+int dfd_drop_block_masks(const void* table, int count, const long long* state, void* stream) {
+    if (count <= 0) return DFD_OK;
+    if (!table || !state || count > 65535) return dfd_set_error(DFD_ERR_ARG, "dfd_drop_block_masks: operands");
+    drop_block_kernel<<<dim3(4 * DFD_SMS, count), 256, 0, (cudaStream_t)stream>>>((const DropBlockDesc*)table, state);
     DFD_LAUNCH_CHECK();
     return DFD_OK;
 }

@@ -36,7 +36,7 @@ class _BN:
 class Engine:
     def __init__(self, arch, batch, height=None, width=None, num_classes=2, in_chans=3, dtype="bf16",
                  bn_momentum=0.1, bn_eps=1e-5, device=None, gemm_impl="tc", share_from=None, stem_impl="gemm",
-                 params_only=False, drop_rate=0.0, drop_path_rate=0.0, sync_bn=False, global_pool="avg"):
+                 params_only=False, drop_rate=0.0, drop_path_rate=0.0, sync_bn=False, global_pool="avg", drop_block_rate=0.0):
         # _plan_only: build the arenas and the call plan on the CPU for host-logic tests; nothing can be executed
         self._plan_only = device == "plan-only"
         if self._plan_only:
@@ -59,6 +59,8 @@ class Engine:
             raise ValueError("dtype %r: the native path computes in 'bf16' or 'fp16' (fp32 master weights)" % (dtype,))
         self.drop_rate = float(drop_rate)
         self.drop_path_rate = float(drop_path_rate)
+        # DropBlock of the ResNet family (layer3 / layer4, resnet.py:386-387); the EfficientNet plan has no DropBlock sites
+        self.drop_block_rate = float(drop_block_rate or 0.0)
         # synchronised BatchNorm (train.py:388-400 `convert_syncbn_model`): batch statistics and the BN-backward sums are
         # all-reduced over the process group between the kernel that produces them and the finalisation
         self.sync_bn = bool(sync_bn)
@@ -831,7 +833,7 @@ class Engine:
             elif name.endswith("_train"):
                 if not training:
                     continue
-            elif name == "dfd_bn_act" and any(isinstance(a, tuple) for a in args):
+            elif name in ("dfd_bn_act", "dfd_bn_act_drop") and any(isinstance(a, tuple) for a in args):
                 args = tuple((a[1] if training else None) if isinstance(a, tuple) else a for a in args)
             elif not training and name in ("dfd_gemm_tn", "dfd_gemm_tn_rowpack", "dfd_dwconv_fwd"):
                 args = tuple(args[:-3]) + (None, None, None)      # eval: no batch statistics, no finalisation

@@ -16,6 +16,7 @@ strided 3x3 is four parity-class implicit GEMMs (`dfd_conv_dgrad_s2_tc`) storing
 """
 import os
 import struct
+from collections import OrderedDict
 
 import torch
 
@@ -25,6 +26,33 @@ from .engine import ACT_NONE, ACT_RELU, _ptr
 
 def conv_out(h, k, s, p):
     return (h + 2 * p - k) // s + 1
+
+
+# DropBlock of the reference ResNet: DropBlock2d(rate, 7, gamma_scale) behind every main-branch BatchNorm of layer3 (gamma_scale
+# 0.25) and layer4 (1.0), resnet.py:386-387,403-404
+DROP_BLOCK_SIZE = 7
+DROP_BLOCK_GAMMA_SCALE = {"layer3": 0.25, "layer4": 1.0}
+DROP_BLOCK_STREAM0 = 1 << 20        # generator stream ids of the DropBlock sites (dfd_rng_masks' tables count from 0)
+
+
+def drop_block_geometry(name, H, W, rate, gamma_scale):
+    """(gamma, clipped block size) of drop_block_2d (layers/drop.py:36-42) on an H x W map, in the reference's double
+    arithmetic. The shapes on which the reference fails are refused: (W - 6)(H - 6) == 0 divides by zero, and an even clipped
+    block size makes the pooled mask one pixel larger than the map."""
+    cb = min(DROP_BLOCK_SIZE, min(W, H))
+    den = (W - DROP_BLOCK_SIZE + 1) * (H - DROP_BLOCK_SIZE + 1)
+    if den == 0:
+        raise ValueError("DropBlock at %s (%dx%d): (W - %d) * (H - %d) == 0, the reference divides by zero"
+                         % (name, H, W, DROP_BLOCK_SIZE - 1, DROP_BLOCK_SIZE - 1))
+    if cb % 2 == 0:
+        raise ValueError("DropBlock at %s (%dx%d): even block size %d, the reference's pooled mask does not match the map"
+                         % (name, H, W, cb))
+    return gamma_scale * rate * (W * H) / cb ** 2 / den, cb
+
+
+def drop_block_desc(mask, noise, kept, gamma, N, H, W, C, cb, stream):
+    """one 64-byte entry of the dfd_drop_block_masks table (pointers as integers, noise may be None)"""
+    return struct.pack("<QQQdiiiiiiii", mask, noise or 0, kept, gamma, N, H, W, C, cb, stream, 0, 0)
 
 
 def build_resnet(e):
@@ -130,7 +158,53 @@ def build_resnet(e):
 
     BF = (lambda bn: bn.bfin) if fused_fin else (lambda bn: None)
 
-    def bn_relu(y, bn, out, hw, C):
+    # ---- stochastic regularisation (training only): DropBlock sites, drop-path gates, classifier dropout ---------------
+    relu_fuse = not (fused_fin or os.environ.get("DFD_NO_RELU_FUSE"))
+    dp_rate, db_rate = e.drop_path_rate, e.drop_block_rate
+    if (e.drop_rate > 0.0 or dp_rate > 0.0 or db_rate > 0.0) and not relu_fuse:
+        raise _lib.NativeError("ResNet drop_rate / drop_path_rate / drop_block_rate need the default plan "
+                               "(not DFD_FUSED_FINALIZE or DFD_NO_RELU_FUSE)")
+    sites = OrderedDict()           # "<block>.bn<i>" -> (H, W, C, gamma, cb)
+    if db_rate > 0.0:
+        for b, h, w, ho, wo in shapes:
+            gs = DROP_BLOCK_GAMMA_SCALE.get(b.name.split(".")[0])
+            if gs is None:
+                continue
+            if b.kind == "basic":
+                dims = [("bn1", ho, wo, b.planes), ("bn2", ho, wo, b.cout)]
+            else:       # the stride is on conv2: bn1 runs at the block's input resolution
+                dims = [("bn1", h, w, b.planes), ("bn2", ho, wo, b.planes), ("bn3", ho, wo, b.cout)]
+            for bn_name, hh, ww, C in dims:
+                name = b.name + "." + bn_name
+                sites[name] = (hh, ww, C) + drop_block_geometry(name, hh, ww, db_rate, gs)
+    e.drop_block_masks = OrderedDict()      # site -> (uint8 mask [N, H, W, C], int64 kept count [1])
+    if sites:
+        e.drop_block_kept = torch.zeros(len(sites), dtype=torch.int64, device=dev)
+        raw = b""
+        for si, (name, (hh, ww, C, gamma, cb)) in enumerate(sites.items()):
+            m = torch.zeros(N, hh, ww, C, dtype=torch.uint8, device=dev)
+            e.drop_block_masks[name] = (m, e.drop_block_kept[si:si + 1])
+            raw += drop_block_desc(_ptr(m), None, _ptr(e.drop_block_kept, si), gamma, N, hh, ww, C, cb, DROP_BLOCK_STREAM0 + si)
+        e._drop_block_table = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(dev)
+    e.drop_block_sites = sites
+    e.drop_masks = OrderedDict()            # block -> drop-path gate [N, cout] (0 or 1 / keep per sample)
+    masks = []                              # dfd_rng_masks table: (tensor, rows, width, keep_prob)
+    if dp_rate > 0.0:
+        for b in spec.blocks:               # one DropPath(drop_path_rate) shared by every block, resnet.py:385
+            gate = torch.ones(N, b.cout, dtype=torch.float32, device=dev)
+            e.drop_masks[b.name] = gate
+            masks.append((gate, N, b.cout, 1.0 - dp_rate))
+
+    def site_args(name):
+        """(mask, kept, numel) operands of a DropBlock site"""
+        m, k = e.drop_block_masks[name]
+        return _ptr(m), _ptr(k), m.numel()
+
+    def bn_relu(y, bn, out, hw, C, site=None):
+        if site in sites:
+            m, k, numel = site_args(site)
+            return ("dfd_bn_act_drop", [_ptr(y), bn.scale, bn.shift, ("TRAIN_ONLY", m), k, numel, None, None, _ptr(out), N, hw, C,
+                                        0, dt])
         return ("dfd_bn_act", (_ptr(y), bn.scale, bn.shift, None, None, _ptr(out), N, hw, C, ACT_RELU, 0, dt))
 
     # ---- scratch -----------------------------------------------------------------------------------------
@@ -174,10 +248,10 @@ def build_resnet(e):
             y2 = e._alloc16(N, ho, wo, b.cout)
             fwd += conv3x3(_ptr(x), p + ".conv1.weight", _ptr(y1), h, w, b.cin, b.planes, b.stride, bn1)
             fwd.append(finalize(bn1, M2))
-            fwd.append(bn_relu(y1, bn1, a1, ho * wo, b.planes))
+            fwd.append(bn_relu(y1, bn1, a1, ho * wo, b.planes, p + ".bn1"))
             fwd += conv3x3(_ptr(a1), p + ".conv2.weight", _ptr(y2), ho, wo, b.planes, b.cout, 1, bn2)
             fwd.append(finalize(bn2, M2))
-            rec.update(y1=y1, a1=a1, ylast=y2, bnlast=bn2)
+            rec.update(y1=y1, a1=a1, ylast=y2, bnlast=bn2, site_last=p + ".bn2")
         else:
             bn1, bn2, bn3 = bns[p + ".bn1"], bns[p + ".bn2"], bns[p + ".bn3"]
             y1 = e._alloc16(N, h, w, b.planes)
@@ -187,13 +261,13 @@ def build_resnet(e):
             y3 = e._alloc16(N, ho, wo, b.cout)
             fwd.append(gemm(_ptr(x), P16(p + ".conv1.weight"), _ptr(y1), M1, b.planes, b.cin, bn1))
             fwd.append(finalize(bn1, M1))
-            fwd.append(bn_relu(y1, bn1, a1, h * w, b.planes))
+            fwd.append(bn_relu(y1, bn1, a1, h * w, b.planes, p + ".bn1"))
             fwd += conv3x3(_ptr(a1), p + ".conv2.weight", _ptr(y2), h, w, b.planes, b.planes, b.stride, bn2)
             fwd.append(finalize(bn2, M2))
-            fwd.append(bn_relu(y2, bn2, a2, ho * wo, b.planes))
+            fwd.append(bn_relu(y2, bn2, a2, ho * wo, b.planes, p + ".bn2"))
             fwd.append(gemm(_ptr(a2), P16(p + ".conv3.weight"), _ptr(y3), M2, b.cout, b.planes, bn3))
             fwd.append(finalize(bn3, M2))
-            rec.update(y1=y1, a1=a1, y2=y2, a2=a2, ylast=y3, bnlast=bn3)
+            rec.update(y1=y1, a1=a1, y2=y2, a2=a2, ylast=y3, bnlast=bn3, site_last=p + ".bn3")
         res = x
         if b.downsample:
             bnd = bns[p + ".downsample.1"]
@@ -220,8 +294,19 @@ def build_resnet(e):
             res = r
         out = e._alloc16(N, ho, wo, b.cout)
         bl = rec["bnlast"]
-        fwd.append(("dfd_bn_act", (_ptr(rec["ylast"]), bl.scale, bl.shift, None, _ptr(res), _ptr(out), N, ho * wo, b.cout,
-                                   ACT_NONE, 2, dt)))
+        gate = e.drop_masks.get(p)
+        rec["gate"] = gate
+        if rec["site_last"] in sites:
+            m, k, numel = site_args(rec["site_last"])
+            fwd.append(("dfd_bn_act_drop", [_ptr(rec["ylast"]), bl.scale, bl.shift, ("TRAIN_ONLY", m), k, numel,
+                                            ("TRAIN_ONLY", _ptr(gate)) if gate is not None else None, _ptr(res), _ptr(out), N,
+                                            ho * wo, b.cout, 2, dt]))
+        elif gate is not None:
+            fwd.append(("dfd_bn_act", [_ptr(rec["ylast"]), bl.scale, bl.shift, ("TRAIN_ONLY", _ptr(gate)), _ptr(res), _ptr(out),
+                                       N, ho * wo, b.cout, ACT_NONE, 2, dt]))
+        else:
+            fwd.append(("dfd_bn_act", (_ptr(rec["ylast"]), bl.scale, bl.shift, None, _ptr(res), _ptr(out), N, ho * wo, b.cout,
+                                       ACT_NONE, 2, dt)))
         e.acts[p + ".out"] = out
         rec["out"] = out
         recs.append(rec)
@@ -236,6 +321,23 @@ def build_resnet(e):
         e.pool_argmax = torch.zeros(N, F, dtype=torch.int32, device=dev)
         fwd.append(("dfd_global_pool", (_ptr(x), None, None, _ptr(e.pooled), _ptr(e.pool_argmax), N, Hf * Wf, F, ACT_NONE,
                                         pool_t, dt, 8)))
+    if e.drop_rate > 0.0:
+        # F.dropout on the pooled vector before fc (resnet.py:465-466), with a mask already divided by keep
+        e.dropout_mask = torch.ones(N, P, dtype=torch.float32, device=dev)
+        masks.append((e.dropout_mask, N * P, 1, 1.0 - e.drop_rate))
+        fwd.append(("dfd_mul_f32_train", (_ptr(e.pooled), _ptr(e.dropout_mask), N * P)))
+    # the step's masks are drawn at the head of the training forward, then the generator's step advances on the device
+    head = []
+    if sites:
+        head.append(("dfd_memset_async_train", (_ptr(e.drop_block_kept), 0, 8 * len(sites))))
+        head.append(("dfd_drop_block_masks_train", (_ptr(e._drop_block_table), len(sites), _ptr(e.rng_state))))
+    if masks:
+        raw = b"".join(struct.pack("<Qqifii", _ptr(t), rows, width, keep, si, 0) for si, (t, rows, width, keep) in enumerate(masks))
+        e._mask_table = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(dev)
+        head.append(("dfd_rng_masks_train", (_ptr(e._mask_table), len(masks), _ptr(e.rng_state))))
+    if head:
+        head.append(("dfd_rng_tick_train", (_ptr(e.rng_state),)))
+    fwd = head + fwd
     e.logits = torch.zeros(N, K, dtype=torch.float32, device=dev)
     e.dlogits = torch.zeros(N, K, dtype=torch.float32, device=dev)
     e.dpooled = torch.zeros(N, P, dtype=torch.float32, device=dev)
@@ -284,6 +386,8 @@ def build_resnet(e):
 
     bwd.append(("dfd_head_bwd", (_ptr(e.dlogits), _ptr(e.pooled), P32("fc.weight"), G32("fc.weight"), G32("fc.bias"),
                                  _ptr(e.dpooled), N, P, K)))
+    if e.drop_rate > 0.0:
+        bwd.append(("dfd_mul_f32", (_ptr(e.dpooled), _ptr(e.dropout_mask), N * P)))
     if pool_t == _lib.POOL_TYPES["avg"]:
         bwd.append(("dfd_pool_bwd", (_ptr(e.dpooled), gA, N, Hf * Wf, F, dt)))
     else:
@@ -291,7 +395,15 @@ def build_resnet(e):
     # The gradient entering a block is kept as up to TWO tensors (main-path dx + identity-path gm of the block above): the
     # fused ReLU / BN-backward reduction adds them on the fly (dfd_relu_bn_bwd_reduce), which removes the materialised
     # residual add of every block without a downsample branch. DFD_NO_RELU_FUSE=1 restores the three separate passes.
-    relu_fuse = not (fused_fin or os.environ.get("DFD_NO_RELU_FUSE"))
+    def relu_bwd(da, y, bn, gu, hw, C, site):
+        """gradient through BN output -> (DropBlock) -> ReLU, plus the BN backward sums"""
+        if site in sites:
+            m, k, numel = site_args(site)
+            return ("dfd_act_bwd_drop", (da, _ptr(y), bn.scale, bn.shift, bn.mean, bn.rstd, m, k, numel, gu, N, hw, C, dt,
+                                         bn.bs1, bn.bs2))
+        return ("dfd_act_bwd", (da, _ptr(y), bn.scale, bn.shift, bn.mean, bn.rstd, None, None, gu, N, hw, C, ACT_RELU, dt,
+                                bn.bs1, bn.bs2, BF(bn)))
+
     bufs = [gA, gB, gC, gD, gE, gF]
     dout, dout2 = gA, None
     for rec in reversed(recs):
@@ -303,19 +415,25 @@ def build_resnet(e):
         if not relu_fuse:
             bwd.append(("dfd_relu_bwd", (dout, _ptr(rec["out"]), gm, M2 * b.cout, dt)))
             bwd.append(("dfd_bn_bwd_reduce", (gm, _ptr(rec["ylast"]), None, bl.mean, bl.rstd, N, ho * wo, b.cout, dt, bl.bs1, bl.bs2, BF(bl))))
+        elif rec["site_last"] in sites or rec["gate"] is not None:
+            # gm goes unmasked to the identity / downsample path; the last BN sees gd = gm * (DropBlock) * (drop path) in t2
+            m, k, numel = site_args(rec["site_last"]) if rec["site_last"] in sites else (None, None, 0)
+            gate = _ptr(rec["gate"]) if rec["gate"] is not None else None
+            bwd.append(("dfd_relu_bn_bwd_reduce_drop", (dout, dout2, _ptr(rec["ylast"]), _ptr(rec["out"]), gm, m, k, numel, gate, t2,
+                                                        bl.mean, bl.rstd, N, ho * wo, b.cout, dt, bl.bs1, bl.bs2)))
         else:
             # gm = (dout + dout2) * (out > 0) is produced by the reduction itself (one pass over the block output instead of
             # the residual add, the ReLU backward and the reduction)
             bwd.append(("dfd_relu_bn_bwd_reduce", (dout, dout2, _ptr(rec["ylast"]), _ptr(rec["out"]), gm, bl.mean, bl.rstd, N, ho * wo,
                                                    b.cout, dt, bl.bs1, bl.bs2)))
+        gd = t2 if (rec["site_last"] in sites or rec["gate"] is not None) else gm
         bwd.append(bwd_finalize(bl, M2))
-        bwd.append(("dfd_bn_bwd_apply", (gm, _ptr(rec["ylast"]), None, bl.cA, bl.cB, bl.cC, t1, N, ho * wo, b.cout, dt)))
+        bwd.append(("dfd_bn_bwd_apply", (gd, _ptr(rec["ylast"]), None, bl.cA, bl.cB, bl.cC, t1, N, ho * wo, b.cout, dt)))
         if b.kind == "basic":
             bn1 = bns[p + ".bn1"]
             # conv2 (3x3 s1): dy2 = t1 -> da1 = t2
             bwd += conv3x3_bwd(p + ".conv2.weight", t1, M2, b.planes, b.cout, rec["a1"], ho, wo, 1, t2)
-            bwd.append(("dfd_act_bwd", (t2, _ptr(rec["y1"]), bn1.scale, bn1.shift, bn1.mean, bn1.rstd, None, None, t1, N,
-                                        ho * wo, b.planes, ACT_RELU, dt, bn1.bs1, bn1.bs2, BF(bn1))))
+            bwd.append(relu_bwd(t2, rec["y1"], bn1, t1, ho * wo, b.planes, p + ".bn1"))
             bwd.append(bwd_finalize(bn1, M2))
             bwd.append(("dfd_bn_bwd_apply", (t1, _ptr(rec["y1"]), None, bn1.cA, bn1.cB, bn1.cC, t2, N, ho * wo, b.planes, dt)))
             # conv1 (3x3 stride s): dy1 = t2 -> dx = t3 [M1, cin]
@@ -325,14 +443,12 @@ def build_resnet(e):
             # conv3 (1x1): dy3 = t1 -> da2 = t2
             bwd.append(gemm(t1, T16(p + ".conv3.weight"), t2, M2, b.planes, b.cout))
             bwd.append(e._wgrad(t1, _ptr(rec["a2"]), G32(p + ".conv3.weight"), M2, b.cout, b.planes))
-            bwd.append(("dfd_act_bwd", (t2, _ptr(rec["y2"]), bn2.scale, bn2.shift, bn2.mean, bn2.rstd, None, None, t1, N,
-                                        ho * wo, b.planes, ACT_RELU, dt, bn2.bs1, bn2.bs2, BF(bn2))))
+            bwd.append(relu_bwd(t2, rec["y2"], bn2, t1, ho * wo, b.planes, p + ".bn2"))
             bwd.append(bwd_finalize(bn2, M2))
             bwd.append(("dfd_bn_bwd_apply", (t1, _ptr(rec["y2"]), None, bn2.cA, bn2.cB, bn2.cC, t2, N, ho * wo, b.planes, dt)))
             # conv2 (3x3 stride s): dy2 = t2 -> da1 = t1 [M1, planes]
             bwd += conv3x3_bwd(p + ".conv2.weight", t2, M2, b.planes, b.planes, rec["a1"], h, w, b.stride, t1)
-            bwd.append(("dfd_act_bwd", (t1, _ptr(rec["y1"]), bn1.scale, bn1.shift, bn1.mean, bn1.rstd, None, None, t2, N,
-                                        h * w, b.planes, ACT_RELU, dt, bn1.bs1, bn1.bs2, BF(bn1))))
+            bwd.append(relu_bwd(t1, rec["y1"], bn1, t2, h * w, b.planes, p + ".bn1"))
             bwd.append(bwd_finalize(bn1, M1))
             bwd.append(("dfd_bn_bwd_apply", (t2, _ptr(rec["y1"]), None, bn1.cA, bn1.cB, bn1.cC, t1, N, h * w, b.planes, dt)))
             # conv1 (1x1): dy1 = t1 -> dx = t3 [M1, cin]
@@ -395,7 +511,10 @@ def build_resnet(e):
     e._upload_fin_descs()
 
     def base_name(n):
-        return n[:-9] if n.endswith("_evalonly") else n
+        for suf in ("_evalonly", "_train"):
+            if n.endswith(suf):
+                return n[:-len(suf)]
+        return n
 
     for n, a in fwd + bwd:
         codes = _lib.SIGNATURES[base_name(n)]

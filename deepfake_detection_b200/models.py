@@ -101,7 +101,7 @@ def init_state_dict(spec, seed=None):
 
 class NativeModel(nn.Module):
     def __init__(self, arch, num_classes=2, in_chans=3, dtype="bf16", bn_momentum=None, bn_eps=None, bn_tf=False,
-                 drop_rate=0.0, drop_path_rate=0.0, gemm_impl="tc", global_pool="avg", **unused):
+                 drop_rate=0.0, drop_path_rate=0.0, gemm_impl="tc", global_pool="avg", drop_block_rate=None, **unused):
         super().__init__()
         if bn_tf:       # efficientnet_blocks.py:13-30
             bn_momentum = 1 - 0.99 if bn_momentum is None else bn_momentum
@@ -115,14 +115,13 @@ class NativeModel(nn.Module):
         self.gemm_impl = gemm_impl
         self.drop_rate = float(drop_rate)              # efficientnet.py:346-347 (classifier dropout)
         self.drop_path_rate = float(drop_path_rate)    # efficientnet_builder.py:322-323 (linear ramp over the blocks)
+        self.drop_block_rate = float(drop_block_rate or 0.0)   # ResNet layer3 / layer4 DropBlock, resnet.py:386-387
         self.max_plans = 4                             # execution plans kept alive (LRU); each owns an activation arena
         self.allow_local_grads = False
         self.sync_bn = False                           # set by ddp.convert_syncbn_model (train.py:388-394)
         self._reducer = None
         self.global_pool = global_pool                 # SelectAdaptivePool2d type (efficientnet.py:297-300, resnet.py:407-409)
         self.spec = get_spec(arch, num_classes=num_classes, in_chans=in_chans, global_pool=global_pool)
-        if self.spec.family != "efficientnet" and (self.drop_rate or self.drop_path_rate):
-            raise _lib.NativeError("drop_rate / drop_path_rate are implemented for the EfficientNet family only")
         self.default_cfg = dict(_DEFAULT_CFG, input_size=self.spec.input_size,
                                 first_conv="conv_stem" if self.spec.family == "efficientnet" else "conv1",
                                 classifier="classifier" if self.spec.family == "efficientnet" else "fc")
@@ -136,7 +135,7 @@ class NativeModel(nn.Module):
     def _engine_kwargs(self):
         return dict(num_classes=self.num_classes, in_chans=self.in_chans, dtype=self.dtype_name, bn_momentum=self.bn_momentum,
                     bn_eps=self.bn_eps, gemm_impl=self.gemm_impl, drop_rate=self.drop_rate, drop_path_rate=self.drop_path_rate,
-                    sync_bn=self.sync_bn, global_pool=self.global_pool)
+                    sync_bn=self.sync_bn, global_pool=self.global_pool, drop_block_rate=self.drop_block_rate)
 
     @property
     def engine(self):
@@ -245,7 +244,7 @@ class NativeModel(nn.Module):
         """ModelEma deep-copies the model (utils.py:300): the copy owns fresh arenas holding the same state"""
         kw = dict(num_classes=self.num_classes, in_chans=self.in_chans, dtype=self.dtype_name, bn_momentum=self.bn_momentum,
                   bn_eps=self.bn_eps, drop_rate=self.drop_rate, drop_path_rate=self.drop_path_rate, gemm_impl=self.gemm_impl,
-                  global_pool=self.global_pool)
+                  global_pool=self.global_pool, drop_block_rate=self.drop_block_rate)
         m = NativeModel(self.arch, **kw)
         m.training = self.training
         if self._primary is not None:

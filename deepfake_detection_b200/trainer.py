@@ -21,10 +21,11 @@ class Trainer:
     def __init__(self, arch, batch, height=None, width=None, dtype="bf16", opt="sgd", lr=0.01, momentum=0.9,
                  weight_decay=1e-4, opt_eps=1e-8, smoothing=0.0, num_classes=2, in_chans=3, bn_momentum=0.1,
                  bn_eps=1e-5, use_graph=True, gemm_impl="tc", process_group=None, bucket_mb=4.0, loss_scale=None,
-                 scale_window=2000, drop_rate=0.0, drop_path_rate=0.0, opt_alpha=0.9, global_pool="avg"):
+                 scale_window=2000, drop_rate=0.0, drop_path_rate=0.0, opt_alpha=0.9, global_pool="avg",
+                 drop_block_rate=0.0):
         self.engine = Engine(arch, batch, height, width, num_classes=num_classes, in_chans=in_chans, dtype=dtype,
                              bn_momentum=bn_momentum, bn_eps=bn_eps, gemm_impl=gemm_impl, drop_rate=drop_rate,
-                             drop_path_rate=drop_path_rate, global_pool=global_pool)
+                             drop_path_rate=drop_path_rate, global_pool=global_pool, drop_block_rate=drop_block_rate)
         self.optimizer = ArenaOptimizer(self.engine, opt=opt, lr=lr, momentum=momentum, weight_decay=weight_decay,
                                         eps=opt_eps, alpha=opt_alpha)
         self.smoothing = float(smoothing)

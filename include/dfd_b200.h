@@ -272,6 +272,28 @@ int dfd_input_normalize(const void* x_u8, const float* mean255, const float* std
 int dfd_rng_masks(const void* table, int count, const long long* state, void* stream);
 int dfd_rng_tick(long long* state, void* stream);
 int dfd_mul_f32(float* a, const float* b, long long n, void* stream);
+/* DropBlock block masks of drop_block_2d (layers/drop.py:24-63), one launch for every site of the step.
+ * table: device array of { unsigned char* mask; float* noise; unsigned long long* kept; double gamma; int N, H, W, C;
+ * int cb; int stream; int _pad[2]; } (64 bytes). mask [N, H, W, C] = the min-pool over cb x cb (cb odd, <= 7) of the seeds
+ * (2 - gamma - valid + u >= 1, u uniform per element); kept (zero on entry) receives the number of ones; noise (optional)
+ * receives u. state: the [seed, step] of dfd_rng_masks; stream ids must differ from that table's. */
+int dfd_drop_block_masks(const void* table, int count, const long long* state, void* stream);
+/* DropBlock on the ResNet BatchNorm outputs (resnet.py:153-162,218-233): ms = mask ? numel / (float(*kept) + 1e-7) : 0.
+ * res_mode 0: out = relu((scale*y + shift) * ms [* gate[n,c]]); res_mode 2: out = relu((scale*y + shift) * ms [* gate[n,c]]
+ * + res). mask == NULL: dfd_bn_act with ReLU (res_mode 0) or the block tail (res_mode 2) */
+int dfd_bn_act_drop(const void* y, const float* scale, const float* shift, const unsigned char* mask,
+                    const unsigned long long* kept, long long numel, const float* gate, const void* res, void* out, int n,
+                    long long hw, int C, int res_mode, int dt, void* stream);
+/* gu = round16(da * ms) * (scale*y + shift > 0), stored, and the BN backward sums of gu */
+int dfd_act_bwd_drop(const void* da, const void* y, const float* scale, const float* shift, const float* mean,
+                     const float* rstd, const unsigned char* mask, const unsigned long long* kept, long long numel, void* gu,
+                     int n, long long hw, int C, int dt, double* s1, double* s2, void* stream);
+/* dfd_relu_bn_bwd_reduce for a block tail with DropBlock (mask) and / or drop path (gate [n, C]): gm = round16(g + g2) *
+ * (out > 0) is stored unmasked; gd = round16(gm * ms * gate[n,c]) is stored and reduced */
+int dfd_relu_bn_bwd_reduce_drop(const void* g, const void* g2, const void* y, const void* out, void* gm,
+                                const unsigned char* mask, const unsigned long long* kept, long long numel, const float* gate,
+                                void* gd, const float* mean, const float* rstd, int n, long long hw, int C, int dt, double* s1,
+                                double* s2, void* stream);
 
 /* ---- optimizers over the flat fp32 parameter arena: create_optimizer, optim_factory.py:26-100;
  *      RMSpropTF rmsprop_tf.py:57-122; AdamW adamw.py:55-117; apex AMP loss scaling train.py:353,632-634 ---- */
