@@ -97,6 +97,10 @@ class Engine:
             self.rng_state = torch.zeros(2, dtype=torch.int64, device=self.device)
             self.rng_state[0] = torch.initial_seed() & 0x7FFFFFFFFFFFFFFF          # follows torch.manual_seed (train.py:299)
             self._derived_dirty = False
+            # bumped whenever a plan registers a derived weight layout (block-diagonal copy, padded stem weight, packed k x k
+            # weights): a CUDA graph captured around the optimizer's refresh holds the old table pointers and entry counts and
+            # must be re-captured (Trainer._graph_signature)
+            self.layout_gen = 0
             # bumped whenever weights or BN running statistics change (load, a training forward, EMA / distribute_bn): an
             # eval-mode plan recomputes its per-channel scale / shift vectors only when this moved (see forward)
             self.state_version = 0
@@ -349,6 +353,7 @@ class Engine:
             reg[key] = torch.zeros(pack * Nn * pack * K, dtype=self.tdtype, device=self.device)
             o._bd_table = None
             o._derived_dirty = True
+            o.layout_gen += 1
         return _ptr(reg[key])
 
     def refresh_weight_layouts(self, stream):
@@ -378,6 +383,7 @@ class Engine:
         if key not in reg:
             reg[key] = torch.zeros(Cout * Kp, dtype=self.tdtype, device=self.device)
             o._derived_dirty = True
+            o.layout_gen += 1
         self.stem_wpad = reg[key]
         self.stem_gpad = torch.zeros(Cout * Kp, dtype=torch.float32, device=self.device)
         self.stem_cols = self._alloc16(M, Kp)

@@ -80,6 +80,7 @@ def build_resnet(e):
         ar._rtable = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(dev)
         ar._rtable_count = len(pk_off)
         ar._derived_dirty = True
+        ar.layout_gen += 1
     e.wpack16, e.wpackT16, e.wpackD16 = ar.wpack16, ar.wpackT16, ar.wpackD16
     # two regions: a BasicBlock has two 3x3 convolutions whose packed gradients wait for the block's single ordered reduce
     gperm_max = max([O * I * k * k for (_, O, I, k) in pk_off.values()] + [8])

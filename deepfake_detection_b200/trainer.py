@@ -89,8 +89,10 @@ class Trainer:
                       self.scale_window, _ptr(e.loss_scale_state, 1), st)
 
     def _graph_signature(self, soft):
-        # the learning rate is NOT part of the key: it is read from device memory by the update kernels
-        return (soft, self.smoothing, self.optimizer.hyper_signature())
+        # the learning rate is NOT part of the key: it is read from device memory by the update kernels. The layout generation
+        # is: a later plan over the same arena (another batch size) can register derived weight layouts, which replaces the
+        # block-diagonal table the captured refresh points to and adds copies only a new capture refreshes
+        return (soft, self.smoothing, self.optimizer.hyper_signature(), self.engine.arena.layout_gen)
 
     def step_resident(self, soft=False):
         """One full train step on the batch already resident in engine.x_in / target_i|target_f."""
