@@ -60,6 +60,14 @@ SIGNATURES = {
     "dfd_sgd_step": "ppp" "l" "fffi" "f" "ppp" "i" "p" "p",
     "dfd_adam_step": "pppp" "l" "fffff" "ii" "f" "ppp" "i" "pp" "p",
     "dfd_rmsprop_tf_step": "pppp" "l" "fffff" "f" "ppp" "i" "p" "p",
+    "dfd_radam_step": "pppp" "l" "fddff" "f" "ppp" "i" "ppp" "p",
+    "dfd_adadelta_step": "pppp" "l" "ffff" "f" "ppp" "i" "p" "p",
+    "dfd_rmsprop_step": "pppp" "l" "fffff" "f" "ppp" "i" "p" "p",
+    "dfd_tensor_sumsq": "ppip" "i" "pp" "f" "pp" "p",
+    "dfd_novograd_prepare": "ppppp" "p" "i" "ff" "p" "p",
+    "dfd_novograd_step": "ppp" "pi" "pp" "fddf" "f" "ppp" "i" "pp" "p",
+    "dfd_nvnovograd_prepare": "ppp" "i" "ff" "p" "p",
+    "dfd_nvnovograd_step": "ppp" "pi" "p" "fff" "f" "ppp" "i" "p" "p",
     "dfd_opt_tick": "pp" "p",
     "dfd_set_floats": "pi" "ffffffff" "p",
     "dfd_ema_update": "ppl" "ppi" "f" "p",

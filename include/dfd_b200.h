@@ -310,6 +310,46 @@ int dfd_adam_step(float* p, const float* g, float* m, float* v, long long n, flo
 int dfd_rmsprop_tf_step(float* p, const float* g, float* sq, float* mom, long long n, float lr, float alpha,
                         float eps, float wd, float momentum, float grad_scale, const float* gscale_dev, const int* skip,
                         void* p16, int dt, const float* lr_dev, void* stream);
+/* ---- the other optimizers of create_optimizer (csrc/optim_ext.cu), same conventions; step_dev is required where named ---- */
+/* RAdam, dfd/timm/optim/radam.py:10-82 (factory optim_factory.py:57-59): exp_avg m, exp_avg_sq v; N_sma and the step size from
+ * *step_dev and *lr0_dev (group 0's lr: the reference caches them in self.buffer, shared by all groups, :54-70), in double;
+ * decoupled decay p -= wd * lr * p first (:73-74) with the range's own lr; N_sma < 5: p -= step_size * m (:79-80) */
+int dfd_radam_step(float* p, const float* g, float* m, float* v, long long n, float lr, double b1, double b2, float eps,
+                   float wd, float grad_scale, const float* gscale_dev, const int* skip, void* p16, int dt,
+                   const float* lr_dev, const float* lr0_dev, const int* step_dev, void* stream);
+/* torch.optim.Adadelta(rho, eps, weight_decay) as built by optim_factory.py:63-65: square_avg sq, acc_delta acc, L2 decay */
+int dfd_adadelta_step(float* p, const float* g, float* sq, float* acc, long long n, float lr, float rho, float eps, float wd,
+                      float grad_scale, const float* gscale_dev, const int* skip, void* p16, int dt, const float* lr_dev,
+                      void* stream);
+/* torch.optim.RMSprop(alpha, eps, momentum, weight_decay), optim_factory.py:66-69: square_avg sq from zeros, eps outside the
+ * sqrt, momentum_buffer mom (may be NULL when momentum == 0), lr applied at the weight update */
+int dfd_rmsprop_step(float* p, const float* g, float* sq, float* mom, long long n, float lr, float alpha, float eps, float wd,
+                     float momentum, float grad_scale, const float* gscale_dev, const int* skip, void* p16, int dt,
+                     const float* lr_dev, void* stream);
+/* Layer-wise norms of NovoGrad / NvNovoGrad (novograd.py:35,59; nvnovograd.py:94): sumsq[t] = sum over tensor t of
+ * (g * grad_scale * *gscale_dev)^2. table: device array of { long long off; int len; int tensor; } (16 bytes), chunks of one
+ * tensor each, in arena order; chunk0[t] .. chunk0[t+1] are tensor t's chunks (n_tensors + 1 ints); partial: n_chunks
+ * doubles of scratch. Partials in fixed slots, fp64, added in a fixed order: bit-reproducible. Nothing written if *skip. */
+int dfd_tensor_sumsq(const float* g, const void* table, int n_chunks, const int* chunk0, int n_tensors, double* partial,
+                     float* sumsq, float grad_scale, const float* gscale_dev, const int* skip, void* stream);
+/* NovoGrad, dfd/timm/optim/novograd.py:12-77, per-tensor part (one CTA): v, grad_ema [n_tensors]; state[0] = initialised flag
+ * (the first applied step re-initialises every tensor, :30-46, and restarts *step_dev at 1), state[1] = this step
+ * initialised; coef [2 * n_tensors] for dfd_novograd_step. ||g/(sqrt(grad_ema)+eps)||^2 is ||g||^2/(sqrt(grad_ema)+eps)^2. */
+int dfd_novograd_prepare(const float* sumsq, float* v, float* grad_ema, float* coef, int* state, int* step_dev, int n_tensors,
+                         float b2, float eps, const int* skip, void* stream);
+/* NovoGrad elementwise part over the chunks [table, table + n_chunks) of one range: m, then p -= lr sqrt(1-b2^t)/(1-b1^t) m
+ * (:65-72); wd is the constructor's decay (self._wd, :20,41,69) */
+int dfd_novograd_step(float* p, const float* g, float* m, const void* table, int n_chunks, const float* coef, const int* state,
+                      float lr, double b1, double b2, float wd, float grad_scale, const float* gscale_dev, const int* skip,
+                      void* p16, int dt, const float* lr_dev, const int* step_dev, void* stream);
+/* NvNovoGrad, dfd/timm/optim/nvnovograd.py:13-117, per tensor: exp_avg_sq = sumsq while it is 0, EMA after (:96-99);
+ * denom = sqrt(exp_avg_sq) + eps */
+int dfd_nvnovograd_prepare(const float* sumsq, float* exp_avg_sq, float* denom, int n_tensors, float b2, float eps,
+                           const int* skip, void* stream);
+/* NvNovoGrad elementwise part: exp_avg = b1 exp_avg + g / denom + wd p (the group's decay), p -= lr exp_avg (:108-115) */
+int dfd_nvnovograd_step(float* p, const float* g, float* m, const void* table, int n_chunks, const float* denom, float lr,
+                        float b1, float wd, float grad_scale, const float* gscale_dev, const int* skip, void* p16, int dt,
+                        const float* lr_dev, void* stream);
 /* *step_dev += 1 unless *skip (fp16 overflow): a skipped step does not advance Adam's bias correction (apex semantics) */
 int dfd_opt_tick(int* step_dev, const int* skip, void* stream);
 /* dst[0..n) = v0..v(n-1), n <= 8: host scalars (learning rates) to device memory, values carried in the launch itself */
