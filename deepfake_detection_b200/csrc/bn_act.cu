@@ -170,8 +170,16 @@ __global__ void bn_finalize_kernel(const double* __restrict__ dsum, const double
         running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * mean;
         running_var[c] = (1.f - momentum) * running_var[c] + momentum * (float)unb;
     } else {
-        mean = running_mean[c];
-        var = running_var[c];
+        // eval: the folded constants rounded once from fp64, so each is within half an fp32 ulp of torch's exact
+        // gamma / sqrt(rv + eps) and beta - rm * scale (rsqrtf plus a Newton step in fp32 was up to 1.7 ulp off rstd, and
+        // shift inherited scale's error); this runs once per weight state, off the training step's critical path
+        const double r = 1.0 / sqrt((double)running_var[c] + (double)eps);
+        const double s = (double)gamma[c] * r;
+        scale[c] = (float)s;
+        shift[c] = (float)((double)beta[c] - (double)running_mean[c] * s);
+        mean_out[c] = running_mean[c];
+        rstd_out[c] = (float)r;
+        return;
     }
     float rstd = rsqrtf(var + eps);
     // rsqrtf is 2 ulp; refine once so that eval-mode folding matches torch's 1/sqrt to fp32 round-off

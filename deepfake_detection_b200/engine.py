@@ -814,6 +814,33 @@ class Engine:
     # ------------------------------------------------------------------------------------------
     # execution
     # ------------------------------------------------------------------------------------------
+    def launch_args(self, name, args, training):
+        """the C-ABI arguments (stream excluded) that the planned op `name` runs with in training or eval mode, or None when
+        the op does not run in that mode. Eval mode: BatchNorm finalises from the running statistics (training = 0, no batch
+        sums), producers write no batch statistics, `_train` ops and ("TRAIN_ONLY", ptr) operands drop out. Training: an
+        `_evalonly` finalisation is done by its producer's last CTA, and a synchronised BatchNorm counts every rank's elements."""
+        if name == "dfd_bn_finalize_sync":
+            args = list(args)
+            if training:
+                args[2] = args[2] * self.sync_world          # global element count behind the summed statistics
+            name = "dfd_bn_finalize"
+        if name.startswith("dfd_bn_finalize"):
+            if training and name.endswith("_evalonly"):
+                return None
+            args = tuple((1 if training else 0) if a == "TRAINING" else a for a in args)
+            if not training:
+                args = (None, None) + args[2:]
+        elif name.endswith("_train"):
+            if not training:
+                return None
+        elif name in ("dfd_bn_act", "dfd_bn_act_drop") and any(isinstance(a, tuple) for a in args):
+            args = tuple((a[1] if training else None) if isinstance(a, tuple) else a for a in args)
+        elif not training and name in ("dfd_gemm_tn", "dfd_gemm_tn_rowpack", "dfd_dwconv_fwd"):
+            args = tuple(args[:-3]) + (None, None, None)      # eval: no batch statistics, no finalisation
+        elif not training and name in ("dfd_gemm_tn_mma", "dfd_stem_fwd"):
+            args = tuple(args[:-2]) + (None, None)
+        return args
+
     def _run(self, ops, stream, training=None, skip_finalize=False):
         if self._plan_only:
             raise _lib.NativeError("plan-only engine cannot execute (no CUDA device)")
@@ -824,27 +851,11 @@ class Engine:
                     import torch.distributed as dist
                     dist.all_reduce(args[0], op=dist.ReduceOp.SUM if args[1] == "sum" else dist.ReduceOp.AVG)
                 continue
-            if name == "dfd_bn_finalize_sync":
-                args = list(args)
-                if training:
-                    args[2] = args[2] * self.sync_world          # global element count behind the summed statistics
-                name = "dfd_bn_finalize"
-            if name.startswith("dfd_bn_finalize"):
-                # `_evalonly`: in training the producing kernel's last CTA finalised this BatchNorm already
-                if skip_finalize or (training and name.endswith("_evalonly")):
-                    continue
-                args = tuple((1 if training else 0) if a == "TRAINING" else a for a in args)
-                if not training:
-                    args = (None, None) + args[2:]
-            elif name.endswith("_train"):
-                if not training:
-                    continue
-            elif name in ("dfd_bn_act", "dfd_bn_act_drop") and any(isinstance(a, tuple) for a in args):
-                args = tuple((a[1] if training else None) if isinstance(a, tuple) else a for a in args)
-            elif not training and name in ("dfd_gemm_tn", "dfd_gemm_tn_rowpack", "dfd_dwconv_fwd"):
-                args = tuple(args[:-3]) + (None, None, None)      # eval: no batch statistics, no finalisation
-            elif not training and name in ("dfd_gemm_tn_mma", "dfd_stem_fwd"):
-                args = tuple(args[:-2]) + (None, None)
+            if skip_finalize and name.startswith("dfd_bn_finalize"):
+                continue
+            args = self.launch_args(name, args, training)
+            if args is None:
+                continue
             rc = fn(*args, stream)
             _lib.N_CALLS[0] += 1
             if rc != 0:

@@ -127,9 +127,10 @@ def _bn_params(C, g):
     return scale, shift
 
 
-def check_dwconv(N, H, W, C, k, s, dtype=torch.bfloat16, affine=True, seed=0, fwd_impl="dfd_dwconv_fwd", add=True):
+def check_dwconv(N, H, W, C, k, s, dtype=torch.bfloat16, affine=True, seed=0, fwd_impl="dfd_dwconv_fwd", add=True, stats=True):
     """fwd + dgrad (both modes) + wgrad against F.conv2d autograd on the rounded operands. add (mode 0 only): the residual
-    gradient added to the input gradient, as in a DS block with a skip connection."""
+    gradient added to the input gradient, as in a DS block with a skip connection. stats=False: also the eval form of the
+    forward (no statistics, no finalisation), which must store the same output bit for bit (`nostats_mismatch`)."""
     g = torch.Generator(device="cuda").manual_seed(seed)
     pad = (k - 1) // 2
     x = torch.randn(N, H, W, C, device="cuda", generator=g).to(dtype)
@@ -142,6 +143,14 @@ def check_dwconv(N, H, W, C, k, s, dtype=torch.bfloat16, affine=True, seed=0, fw
     _lib.call(fwd_impl, P(x), P(scale) if affine else None, P(shift) if affine else None, P(w), P(out), N, H, W, C,
               k, s, act, DT[dtype], P(s1), P(s2), None, st())
     torch.cuda.synchronize()
+    nostats = {}
+    if not stats:
+        out_e = torch.full_like(out, float("nan"))
+        _lib.call(fwd_impl, P(x), P(scale) if affine else None, P(shift) if affine else None, P(w), P(out_e), N, H, W, C,
+                  k, s, act, DT[dtype], None, None, None, st())
+        torch.cuda.synchronize()
+        nostats["nostats_mismatch"] = int((out_e.view(torch.int16) != out.view(torch.int16)).sum())
+        del out_e
     # reference (fp32, same rounding points: activated input rounded to `dtype`)
     xr = nchw(x.float()).requires_grad_(True)
     if affine:
@@ -153,7 +162,7 @@ def check_dwconv(N, H, W, C, k, s, dtype=torch.bfloat16, affine=True, seed=0, fw
     wr = w.clone().requires_grad_(True)
     ref = F.conv2d(a_q, wr, stride=s, padding=pad, groups=C)
     res = dict(fwd_max=maxerr_scaled(nchw(out.float()), ref.detach()), fwd_rel=relerr(nchw(out.float()), ref.detach()),
-               nan=int(torch.isnan(out.float()).sum()))
+               nan=int(torch.isnan(out.float()).sum()), **nostats)
     # Element-wise bound of the forward (fwd_ulp <= 1). The kernel's Swish is u * sigmoid_fast(u) with
     # sigmoid_fast = fmaf(tanh.approx(u/2), 0.5, 0.5) (common.cuh:97). tanh.approx.f32 has at most 2^-10.98 relative error and
     # |tanh| <= 1, so the sigmoid is off by < 2^-11 ABSOLUTE and the kernel's activation a' by e = |u| 2^-11 (relative to a this
@@ -756,11 +765,19 @@ def check_se_fused(N, HW, C, Cse, dtype=torch.bfloat16, seed=0):
     return out
 
 
-def check_head(N, Fdim, smoothing=0.0, soft=False, seed=0):
+def check_head(N, Fdim, smoothing=0.0, soft=False, seed=0, with_loss=True):
+    """with_loss=False: the logits-only launch of Engine.head(False) (validate, test_img), with no target, loss, count or
+    dlogits operand; only the logits are returned"""
     g = torch.Generator(device="cuda").manual_seed(seed)
     pooled = torch.randn(N, Fdim, device="cuda", generator=g)
     W = (torch.randn(2, Fdim, device="cuda", generator=g) / math.sqrt(Fdim)).requires_grad_(True)
     b = (0.1 * torch.randn(2, device="cuda", generator=g)).requires_grad_(True)
+    if not with_loss:
+        logits = torch.full((N, 2), float("nan"), device="cuda")
+        _lib.call("dfd_head_fwd", P(pooled), P(W), P(b), P(logits), N, Fdim, 2, None, None, 0.0, 1.0, None, None, None, None, st())
+        torch.cuda.synchronize()
+        ref = pooled.double() @ W.detach().double().t() + b.detach().double()
+        return dict(logits_rel=relerr(logits, ref), nan=int(torch.isnan(logits).sum()))
     y = torch.randint(0, 2, (N,), device="cuda", generator=g)
     tf = torch.softmax(torch.randn(N, 2, device="cuda", generator=g), -1)
     logits = torch.zeros(N, 2, device="cuda")
@@ -787,6 +804,41 @@ def check_head(N, Fdim, smoothing=0.0, soft=False, seed=0):
     return dict(logits_rel=relerr(logits, z.detach()), loss_rel=abs(float(acc[0]) - float(loss)) / abs(float(loss)),
                 correct_diff=abs(float(acc[1]) - correct), dlogits_rel=relerr(dlog, z.grad), dW_rel=relerr(dW, W.grad),
                 db_rel=relerr(db, b.grad), dpooled_rel=relerr(dpooled, pr.grad))
+
+
+def _ulp32(x):
+    """the fp32 ulp at each value of the fp64 tensor x (normal range)"""
+    _, e = torch.frexp(x.abs())
+    return torch.ldexp(torch.ones_like(x), e - 24)
+
+
+def check_bn_finalize_eval(C, eps=1e-5, momentum=0.1, seed=0):
+    """dfd_bn_finalize in eval form, as Engine.launch_args issues it (training = 0, no batch sums): the folded BatchNorm from
+    the running statistics against fp64. Returns the errors in fp32 ulps of the fp64 values: rstd of 1/sqrt(rv + eps) (eps as
+    the fp32 argument the kernel receives), scale of gamma * rstd, and shift over ulp(beta) + ulp(rm * scale) of
+    beta - rm * scale; whether mean is the running mean exactly, and whether the running statistics and num_batches_tracked
+    kept every bit. The running variances span 1e-4 .. 1e2 so that rsqrt meets many exponents."""
+    import numpy as np
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    gamma = 1.0 + 0.2 * torch.randn(C, device="cuda", generator=g)
+    beta = 0.3 * torch.randn(C, device="cuda", generator=g)
+    rm = 0.5 * torch.randn(C, device="cuda", generator=g)
+    rv = 10.0 ** (6.0 * torch.rand(C, device="cuda", generator=g) - 4.0)
+    nbt = torch.full((1,), 5, dtype=torch.int64, device="cuda")
+    rm0, rv0 = rm.clone(), rv.clone()
+    scale, shift, mean, rstd = (torch.full((C,), float("nan"), device="cuda") for _ in range(4))
+    _lib.call("dfd_bn_finalize", None, None, 1000.0, P(gamma), P(beta), P(rm), P(rv), P(nbt), momentum, eps, 0, C, P(scale),
+              P(shift), P(mean), P(rstd), st())
+    torch.cuda.synchronize()
+    r_ref = 1.0 / torch.sqrt(rv.double() + float(np.float32(eps)))
+    sc_ref = gamma.double() * r_ref
+    sh_ref = beta.double() - rm.double() * sc_ref
+    return dict(rstd_ulp=float(((rstd.double() - r_ref).abs() / _ulp32(r_ref)).max()),
+                scale_ulp=float(((scale.double() - sc_ref).abs() / _ulp32(sc_ref)).max()),
+                shift_ulp=float(((shift.double() - sh_ref).abs() / (_ulp32(beta.double()) + _ulp32(rm.double() * sc_ref))).max()),
+                mean_exact=bool(torch.equal(mean, rm0)),
+                state_kept=bool(torch.equal(rm, rm0) and torch.equal(rv, rv0) and int(nbt) == 5),
+                nan=int(sum(torch.isnan(t).sum() for t in (scale, shift, mean, rstd))))
 
 
 def check_optimizer(kind, n=10007, steps=3, dtype=torch.bfloat16, seed=0):

@@ -50,18 +50,39 @@ def _split(name, args):
     return Launch(name, tuple(shape), ptrs)
 
 
-@functools.lru_cache(maxsize=None)
-def plan_launches(tag):
-    """OrderedDict Launch -> number of times the training step (forward + backward) issues it, for one configuration"""
+@functools.lru_cache(maxsize=2)         # the training and the eval harvest of one plan share its engine
+def _plan_engine(tag, batch, dtype):
     from deepfake_detection_b200.engine import Engine
-    _, arch, batch, res, dtype, kw = next(c for c in CONFIGS if c[0] == tag)
-    eng = Engine(arch, batch, res, res, device="plan-only", dtype=dtype, **kw)
+    _, arch, b, res, dt, kw = next(c for c in CONFIGS if c[0] == tag)
+    return Engine(arch, batch or b, res, res, device="plan-only", dtype=dtype or dt, **kw)
+
+
+@functools.lru_cache(maxsize=None)
+def plan_launches(tag, batch=None, training=True, dtype=None):
+    """OrderedDict Launch -> number of times one step issues it, for one configuration (at another batch / 16-bit type when
+    given). Training: the forward and backward plan as built. Eval: the forward ops as Engine.launch_args rewrites them for
+    eval mode, then the logits-only head (Engine.head(False))."""
+    eng = _plan_engine(tag, batch, dtype)
     out = OrderedDict()
-    for _, name, args in list(eng.fwd_ops) + list(eng.bwd_ops):
+
+    def add(la):
+        out[la] = out.get(la, 0) + 1
+
+    for _, name, args in list(eng.fwd_ops) + (list(eng.bwd_ops) if training else []):
         if name.startswith("ALLREDUCE"):
             continue
-        la = _split(base_name(name), args)
-        out[la] = out.get(la, 0) + 1
+        if not training:
+            args = eng.launch_args(name, args, False)
+            if args is None:
+                continue
+        add(_split(base_name(name), args))
+    if not training:
+        real = _lib.call
+        _lib.call = lambda name, *args: add(_split(name, args[:-1]))          # the stream last
+        try:
+            eng.head(False, stream=0)
+        finally:
+            _lib.call = real
     return out
 
 
@@ -179,8 +200,9 @@ def dw_cpw(C):
     return _lib.lib().cdll.dfd_dwconv_block_channels(C) // 2
 
 
-def _case_of(la, dtype):
-    """(check, kwargs, n_full, dispatch class) exercising this launch; kwargs at the full batch"""
+def _case_of(la, dtype, plan=None):
+    """(check, kwargs, n_full, dispatch class) exercising this launch; kwargs at the full batch. `plan`: the launches of the
+    plan that issues it (default: the shipped training plans)"""
     k, s = la.kernel, la.shape
     if k == "dfd_gemm_tn":
         M, N, K = s[0], s[1], s[2]
@@ -201,6 +223,8 @@ def _case_of(la, dtype):
         # the backward with it (the plan's add-less mode-0 launches have cases of their own)
         add = not affine and (k == "dfd_dwconv_fwd" or la.ptrs[11] == "p")
         kw = dict(N=N, H=H, W=W, C=C, k=kk, s=st, affine=affine, add=add)
+        if k == "dfd_dwconv_fwd" and la.ptrs[5] == "0":        # the eval form: no batch statistics, no finalisation
+            kw["stats"] = False
         if k == "dfd_dwconv_fwd":
             return "dwconv", kw, N, ("dw_fwd", dw_cpw(C), dw_tile(H, W, kk, st), kk, st, affine)
         kw["ws_bytes"] = s[7]
@@ -219,11 +243,13 @@ def _case_of(la, dtype):
         return "conv1x1_dgrad_add", dict(N=N, H=H, W=W, Cin=Cin, Cout=Cout, stride=st), N, ("c1x1", st)
     if k == "dfd_stem_im2col":
         N, Cin, H, W, kk, st, pad, Kp = s[:8]
-        cout, pack = _stem_gemm_form(N, Cin, H, W, kk, st, pad, Kp)
+        cout, pack = _stem_gemm_form(N, Cin, H, W, kk, st, pad, Kp, plan)
         return "stem_gemm", dict(N=N, Cin=Cin, H=H, W=W, Cout=cout, k=kk, s=st, pad=pad, pack=pack), N, ("stem", Cin, kk, pack)
     if k == "dfd_unpad_grad":            # the stem case of the configuration that issues it
-        tag = next(t for t, *_ in CONFIGS if config_dtype(t) == dtype and la in plan_launches(t))
-        return _case_of(next(x for x in plan_launches(tag) if x.kernel == "dfd_stem_im2col"), dtype)
+        if plan is None:
+            tag = next(t for t, *_ in CONFIGS if config_dtype(t) == dtype and la in plan_launches(t))
+            plan = plan_launches(tag)
+        return _case_of(next(x for x in plan if x.kernel == "dfd_stem_im2col"), dtype, plan)
     if CHECKED.get(k) == "row":
         # every non-pointer argument after (n, hw, C) but the dtype (the last one, except before dfd_pool's chunk count)
         n_dt = {"dfd_pool": 4}.get(k, len(s) - 1)
@@ -238,15 +264,23 @@ def _case_of(la, dtype):
     if k == "dfd_head_bwd":
         assert s[2] == 2, la                 # the 2-class head of the shipped configurations (check_head)
         return "head", dict(N=s[0], F=s[1]), None, None
+    if k == "dfd_head_fwd":                  # logits only (validate / test_img): no target, loss, count or dlogits
+        assert s[2] == 2 and la.ptrs == "pppp" + "0" * 6, la
+        return "head_fwd", dict(N=s[0], F=s[1]), None, None
+    if k == "dfd_bn_finalize":               # eval form: scale / shift from the running statistics
+        assert s[3] == 0 and la.ptrs[:2] == "00", la
+        return "bn_finalize_eval", dict(C=s[4]), None, None
     raise KeyError(k)
 
 
-def _stem_gemm_form(N, Cin, H, W, k, s, pad, Kp):
+def _stem_gemm_form(N, Cin, H, W, k, s, pad, Kp, plan=None):
     """(Cout, pack) of the stem GEMM the plan runs on these columns: pack 1 = dfd_gemm_tn, else dfd_gemm_tn_rowpack"""
     M = N * ((H + 2 * pad - k) // s + 1) * ((W + 2 * pad - k) // s + 1)
-    for tag, *_ in CONFIGS:
-        for la in plan_launches(tag):
-            if la.kernel in ("dfd_gemm_tn", "dfd_gemm_tn_rowpack") and la.shape[0] == M and la.shape[2] == Kp and la.ptrs[3] == "p":
+    # the first such GEMM in plan order is the stem's (it follows the im2col); an eval plan's writes no statistics
+    for launches in ([plan] if plan is not None else [plan_launches(tag) for tag, *_ in CONFIGS]):
+        for la in launches:
+            if la.kernel in ("dfd_gemm_tn", "dfd_gemm_tn_rowpack") and la.shape[0] == M and la.shape[2] == Kp and \
+                    (la.ptrs[3] == "p" or plan is not None):
                 return la.shape[1], (la.shape[3] if la.kernel == "dfd_gemm_tn_rowpack" else 1)
     raise KeyError((N, Cin, H, k))
 

@@ -54,8 +54,12 @@ def _check_wgrad(kw, dt):
 
 
 def _check_dwconv(kw, dt):
-    r = _gc().check_dwconv(kw["N"], kw["H"], kw["W"], kw["C"], kw["k"], kw["s"], dtype=TDT[dt], affine=kw["affine"], add=kw["add"])
+    """stats=False (the eval form of the forward): also the stats-less launch, bit for bit the output of the stats run"""
+    stats = kw.get("stats", True)
+    r = _gc().check_dwconv(kw["N"], kw["H"], kw["W"], kw["C"], kw["k"], kw["s"], dtype=TDT[dt], affine=kw["affine"], add=kw["add"],
+                           stats=stats)
     assert r["nan"] == 0 and r["nan_b"] == 0 and r["fused_nan"] == 0 and r["det_nan"] == 0, str(r)
+    assert stats or r["nostats_mismatch"] == 0, str(r)
     if dt == "fp16":      # test_dwconv_fp16's bounds
         assert r["fwd_rel"] < 2e-3 and r["dgrad_rel"] < 4e-3 and r["wgrad_rel"] < RED, str(r)
     else:
