@@ -35,6 +35,8 @@ SIGNATURES = {
     "dfd_dwconv_bwd": "ppppp" "pppppp" "ppp" "iiiiii" "i" "pp" "pl" "p" "p",
     "dfd_dwconv_bwd_parts": "iiiiii",
     "dfd_dwconv_block_channels": "i",
+    "dfd_dwconv_fwd_pad": "ppppp" "iiiiiiii" "ii" "ppp" "p",
+    "dfd_dwconv_bwd_pad": "ppppp" "pppppp" "ppp" "iiiiiiii" "i" "pp" "pl" "p" "p",
     "dfd_stem_fwd": "ppp" "iiiiiiii" "i" "ppp",
     "dfd_stem_wgrad": "ppppppp" "iiiiiiii" "i" "p",
     "dfd_colstats": "p" "ili" "i" "ppp",
@@ -93,6 +95,7 @@ SIGNATURES = {
     "dfd_pool_bwd": "pp" "ili" "i" "p",
     "dfd_gpool_bwd": "ppp" "ili" "ii" "p",
     "dfd_stem_im2col": "pp" "iiiiiiii" "i" "p",
+    "dfd_stem_im2col_pad": "pp" "iiiiiiiii" "i" "p",
     "dfd_pad_weight": "pp" "iii" "i" "p",
     "dfd_unpad_grad": "pp" "iii" "p",
 }

@@ -12,6 +12,8 @@ BASELINE.json names; it builds no modules and owns no tensors.
   * SE width `make_divisible(block_in_chs * 0.25, 1)`: efficientnet_blocks.py:46-47,98
   * B0/B4 generator (stem 32, head 1280, 7 stages): dfd/timm/models/efficientnet.py:760-803,1078,1132
   * deepfake_v4 (stem 128, head 128, x2.0 / x3.1): efficientnet.py:806-851,1186-1192
+  * tf_efficientnet_b0..b7 (+ _ap, _ns): the B0 generator with pad_type='same', efficientnet.py:1265-1530; TF "SAME"
+    padding of the stride-2 convolutions, layers/padding.py `pad_same` / layers/conv2d_same.py
   * ResNet-18/50 layout: dfd/timm/models/resnet.py:115-260,280-468,472,523
 """
 import math
@@ -39,6 +41,16 @@ def round_channels(channels, multiplier=1.0, divisor=8, channel_min=None):
 
 def conv_out(h, k, s, p):
     return (h + 2 * p - k) // s + 1
+
+
+def same_pad(i, k, s):
+    """TF "SAME" padding of one axis of extent i (layers/padding.py get_same_padding / pad_same):
+    (begin, end, output extent). The total is max((ceil(i/s) - 1)*s + k - i, 0); the begin side (top / left) gets half of
+    it rounded down. At stride 1 (k odd) and over an odd extent at stride 2 that is the symmetric (k-1)/2; over an even
+    extent at stride 2 the begin side gets one element less."""
+    out = -(-i // s)
+    total = max((out - 1) * s + k - i, 0)
+    return total // 2, total - total // 2, out
 
 
 # ----------------------------------------------------------------------------------------------
@@ -76,6 +88,7 @@ class EfficientNetSpec:
     input_size: Tuple[int, int, int]
     family: str = "efficientnet"
     global_pool: str = "avg"
+    pad_type: str = ""           # '' (symmetric (k-1)/2) or 'same' (TF "SAME" on the stride-2 stem and depthwise convs)
 
     @property
     def pooled_features(self):
@@ -210,6 +223,11 @@ def _base_spec(arch, num_classes, in_chans):
         # efficientnet.py:806-851: stem_size=128, num_features=round_channels(128, 2.0)
         return _efficientnet_spec(arch, 2.0, 3.1, 128, round_channels(128, 2.0, 8, None), in_chans,
                                   num_classes, (in_chans, 600, 600))
+    if arch in TF_ARCHS:
+        cm, dm, res = _TF_SCALING[int(arch[len("tf_efficientnet_b")])]
+        spec = _efficientnet_spec(arch, cm, dm, 32, round_channels(1280, cm, 8, None), in_chans, num_classes, (3, res, res))
+        spec.pad_type = "same"
+        return spec
     if arch == "resnet18":
         return _resnet_spec(arch, "basic", (2, 2, 2, 2), in_chans, num_classes, (3, 224, 224))
     if arch == "resnet50":
@@ -218,6 +236,38 @@ def _base_spec(arch, num_classes, in_chans):
 
 
 SUPPORTED_ARCHS = ("efficientnet_b0", "efficientnet_b4", "efficientnet_deepfake_v4", "resnet18", "resnet50")
+
+# TensorFlow-ported EfficientNets (efficientnet.py:1265-1530): the B0 generator with TF "SAME" padding and BatchNorm eps 1e-3.
+# _ap (AdvProp) and _ns (Noisy Student) share the plain variant's layers; only their default_cfg differs (models.py).
+# size -> (channel multiplier, depth multiplier, default resolution), efficientnet.py:112-195,1268-1350
+_TF_SCALING = {0: (1.0, 1.0, 224), 1: (1.0, 1.1, 240), 2: (1.1, 1.2, 260), 3: (1.2, 1.4, 300),
+               4: (1.4, 1.8, 380), 5: (1.6, 2.2, 456), 6: (1.8, 2.6, 528), 7: (2.0, 3.1, 600)}
+TF_ARCHS = tuple("tf_efficientnet_b%d%s" % (i, suf) for suf in ("", "_ap", "_ns") for i in range(8))
+# default_cfg pool_size / crop_pct per size (efficientnet.py:112-195)
+TF_POOL_CROP = {0: ((7, 7), 0.875), 1: ((8, 8), 0.882), 2: ((9, 9), 0.890), 3: ((10, 10), 0.904),
+                4: ((12, 12), 0.922), 5: ((15, 15), 0.934), 6: ((17, 17), 0.942), 7: ((19, 19), 0.949)}
+
+
+def conv_pads(spec, H, W):
+    """The padded convolutions of an EfficientNet spec at input H x W, in forward order: [(layer, k, stride, h, w,
+    pad_top, pad_left, ho, wo)] for 'conv_stem' and every '<block>.conv_dw'. pad_type '' pads (k-1)/2 on every side;
+    'same' pads as TF "SAME" (same_pad) per axis. The output extents agree either way."""
+    out = []
+
+    def add(name, k, s, h, w):
+        if spec.pad_type == "same":
+            pt, _, ho = same_pad(h, k, s)
+            pl, _, wo = same_pad(w, k, s)
+        else:
+            pt = pl = (k - 1) // 2
+            ho, wo = conv_out(h, k, s, pt), conv_out(w, k, s, pl)
+        out.append((name, k, s, h, w, pt, pl, ho, wo))
+        return ho, wo
+
+    h, w = add("conv_stem", 3, 2, H, W)
+    for b in spec.blocks:
+        h, w = add(b.name + ".conv_dw", b.k, b.stride, h, w)
+    return out
 
 
 # ----------------------------------------------------------------------------------------------

@@ -276,11 +276,11 @@ __global__ void gpool_bwd_kernel(const float* __restrict__ dpooled, const int* _
 // ---- stem as a GEMM: im2col of the NCHW image in (ci, kh, kw) column order (== OIHW flattening), K padded to a multiple of 8.
 // One CTA per output row: the Cin x k input rows it needs are staged (zero-padded) in shared memory with coalesced reads,
 // then every thread assembles 16-byte column groups from it (a per-thread 2-byte gather from global is request-bound).
+// pad_t / pad_l: zero rows above / columns left of the image; WP: staged (padded) row width, >= (Wo - 1) * s + k.
 template <typename T>
-__global__ void stem_im2col_kernel(const T* __restrict__ x, T* __restrict__ cols, int N, int Cin, int H, int W, int k, int s,
-                                   int pad, int Ho, int Wo, int Kp) {
+__device__ __forceinline__ void stem_im2col_body(const T* __restrict__ x, T* __restrict__ cols, int N, int Cin, int H, int W,
+                                                 int k, int s, int pad_t, int pad_l, int WP, int Ho, int Wo, int Kp) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    const int WP = W + 2 * pad;                      // padded row
     const int taps = Cin * k * k;
     T* rows = reinterpret_cast<T*>(smem_raw);        // [Cin][k][WP]
     int* offs = reinterpret_cast<int*>(smem_raw + (((size_t)Cin * k * WP * sizeof(T) + 15) & ~(size_t)15));   // [Kp]
@@ -289,7 +289,7 @@ __global__ void stem_im2col_kernel(const T* __restrict__ x, T* __restrict__ cols
     for (int i = threadIdx.x; i < Cin * k * WP; i += blockDim.x) {
         const int px = i % WP, r = i / WP;           // r = ci * k + kh
         const int kh = r % k, ci = r / k;
-        const int iy = oy * s - pad + kh, ix = px - pad;
+        const int iy = oy * s - pad_t + kh, ix = px - pad_l;
         rows[i] = (iy >= 0 && iy < H && ix >= 0 && ix < W) ? img[((size_t)ci * H + iy) * W + ix] : from_f<T>(0.f);
     }
     for (int t = threadIdx.x; t < Kp; t += blockDim.x) {
@@ -314,6 +314,18 @@ __global__ void stem_im2col_kernel(const T* __restrict__ x, T* __restrict__ cols
         }
         stg16(out + (size_t)ox * Kp + g * 8, *reinterpret_cast<const uint4*>(vals));
     }
+}
+// symmetric padding (the EfficientNet and ResNet stems)
+template <typename T>
+__global__ void stem_im2col_kernel(const T* __restrict__ x, T* __restrict__ cols, int N, int Cin, int H, int W, int k, int s,
+                                   int pad, int Ho, int Wo, int Kp) {
+    stem_im2col_body(x, cols, N, Cin, H, W, k, s, pad, pad, W + 2 * pad, Ho, Wo, Kp);
+}
+// TF "SAME" padding (dfd_stem_im2col_pad)
+template <typename T>
+__global__ void stem_im2col_same_kernel(const T* __restrict__ x, T* __restrict__ cols, int N, int Cin, int H, int W, int k,
+                                        int s, int pad_t, int pad_l, int WP, int Ho, int Wo, int Kp) {
+    stem_im2col_body(x, cols, N, Cin, H, W, k, s, pad_t, pad_l, WP, Ho, Wo, Kp);
 }
 // 16-bit weight [O][taps] -> [O][Kp] (zero padded), and the inverse for the fp32 gradient (accumulating)
 template <typename T>
@@ -427,15 +439,37 @@ int dfd_gpool_bwd(const float* dpooled, const int* argmax, void* dout, int N, lo
     return DFD_OK;
 }
 
-int dfd_stem_im2col(const void* x_nchw, void* cols, int N, int Cin, int H, int W, int k, int stride, int pad, int Kp, int dt,
-                    void* stream) {
+static int stem_im2col(const void* x_nchw, void* cols, int N, int Cin, int H, int W, int k, int stride, int pad_t, int pad_l,
+                       int Ho, int Wo, int WP, int Kp, int dt, void* stream) {
     if (Kp % 8 || Kp < Cin * k * k) return dfd_set_error(DFD_ERR_ARG, "dfd_stem_im2col: Kp");
-    int Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
-    size_t smem = (((size_t)Cin * k * (W + 2 * pad) * 2 + 15) & ~(size_t)15) + (size_t)Kp * sizeof(int);
+    size_t smem = (((size_t)Cin * k * WP * 2 + 15) & ~(size_t)15) + (size_t)Kp * sizeof(int);
     if (smem > 48 * 1024) return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_stem_im2col: input rows exceed shared memory");
-    CD_T(dt, (stem_im2col_kernel<T><<<N * Ho, 256, smem, (cudaStream_t)stream>>>((const T*)x_nchw, (T*)cols, N, Cin, H, W, k, stride, pad, Ho, Wo, Kp)));
+    // symmetric pads (every ResNet / EfficientNet stem, and a TF "SAME" stem over odd extents) run the symmetric kernel
+    if (pad_t == pad_l && WP == W + 2 * pad_t && Ho == (H + 2 * pad_t - k) / stride + 1 && Wo == (W + 2 * pad_t - k) / stride + 1) {
+        CD_T(dt, (stem_im2col_kernel<T><<<N * Ho, 256, smem, (cudaStream_t)stream>>>((const T*)x_nchw, (T*)cols, N, Cin, H, W, k, stride, pad_t, Ho, Wo, Kp)));
+    } else {
+        CD_T(dt, (stem_im2col_same_kernel<T><<<N * Ho, 256, smem, (cudaStream_t)stream>>>((const T*)x_nchw, (T*)cols, N, Cin, H, W, k, stride, pad_t, pad_l, WP, Ho, Wo, Kp)));
+    }
     DFD_LAUNCH_CHECK();
     return DFD_OK;
+}
+
+int dfd_stem_im2col(const void* x_nchw, void* cols, int N, int Cin, int H, int W, int k, int stride, int pad, int Kp, int dt,
+                    void* stream) {
+    int Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
+    return stem_im2col(x_nchw, cols, N, Cin, H, W, k, stride, pad, pad, Ho, Wo, W + 2 * pad, Kp, dt, stream);
+}
+
+// TF "SAME" padding: Ho = ceil(H / stride), Wo = ceil(W / stride), pad_t rows above and pad_l columns left of the image,
+// the rest of each total pad max((ceil(i/s) - 1) * s + k - i, 0) below / right (layers/padding.py `pad_same`)
+int dfd_stem_im2col_pad(const void* x_nchw, void* cols, int N, int Cin, int H, int W, int k, int stride, int pad_t, int pad_l,
+                        int Kp, int dt, void* stream) {
+    if (stride <= 0 || N <= 0 || H <= 0 || W <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_stem_im2col_pad: sizes");
+    const int Ho = (H + stride - 1) / stride, Wo = (W + stride - 1) / stride;
+    const int tot_h = (Ho - 1) * stride + k - H, tot_w = (Wo - 1) * stride + k - W;
+    if (pad_t != (tot_h > 0 ? tot_h / 2 : 0) || pad_l != (tot_w > 0 ? tot_w / 2 : 0))
+        return dfd_set_error(DFD_ERR_ARG, "dfd_stem_im2col_pad: pads are the begin sides of TF SAME padding");
+    return stem_im2col(x_nchw, cols, N, Cin, H, W, k, stride, pad_t, pad_l, Ho, Wo, (Wo - 1) * stride + k, Kp, dt, stream);
 }
 
 int dfd_pad_weight(const void* src, void* dst, int O, int taps, int Kp, int dt, void* stream) {

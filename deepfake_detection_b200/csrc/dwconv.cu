@@ -1,7 +1,9 @@
 // Depthwise k x k convolution (k in {3,5}, stride in {1,2}) forward, input-gradient and weight-gradient,
 // NHWC 16-bit activations, fp32 accumulation.   Reference: nn.Conv2d(groups=C) built by
 // dfd/timm/models/layers/create_conv2d.py:11-30 at dfd/timm/models/efficientnet_blocks.py:152-153,283-285
-// with symmetric padding (k-1)//2 (layers/padding.py:12-14).
+// with symmetric padding (k-1)//2 (layers/padding.py:12-14), or, through the `_pad` entry points, with the TensorFlow
+// "SAME" padding of the tf_efficientnet_* models (Conv2dSame, layers/conv2d_same.py): at stride 2 over an even extent the
+// begin side (top / left) gets one element less, (k-1)/2 - 1, and the output extent stays ceil(H/2).
 //
 // Design: these layers are HBM-bound with k*k-fold reuse of every input element, and the preceding
 // BN + Swish is fused into the load, so:
@@ -33,7 +35,7 @@ constexpr int DW_MAX_SMEM = 200 * 1024;
 
 
 struct DwGeom {
-    int N, H, W, C, Ho, Wo, pad;
+    int N, H, W, C, Ho, Wo, pad;     // pad: the symmetric (k-1)/2 (TF "SAME" pads: template parameters DT / DL below)
     int TH, TW;              // output tile (TW multiple of 8)
     int IH, IW;              // staged input tile
     int tiles_x, tiles_y;
@@ -165,7 +167,7 @@ __device__ __forceinline__ void stage_grad_tile(uint32_t* tile, const T* __restr
 
 // stride-2 input gradient of one strip of P input columns (ix0 even) in input row `sy` (relative to the even tile
 // origin): ga[p] = sum over taps with (sy+pad-kh) and (p+pad-kw) even of dy[(sy+pad-kh)/2, (sx+p+pad-kw)/2] * w[kh,kw].
-// The compact dy tile starts at (y0/2 - 1, x0/2 - 1).
+// The compact dy tile starts at (y0/2 - 1, x0/2 - 1). Symmetric padding only (the diagnostic split kernel).
 template <typename T, int K>
 __device__ __forceinline__ void strip_dgrad_s2(const uint32_t* __restrict__ tile, int IW, int sy, int sx, int lane,
                                                const float (&w)[K * K][2], float (&acc)[P][2]) {
@@ -243,7 +245,8 @@ __device__ __forceinline__ void reduce_warps_emit(float* sm, float a, float b, F
 // ---------------------------------------------------------------------------------------------
 // forward
 // ---------------------------------------------------------------------------------------------
-template <typename T, int K, int S, int ACT, bool AFFINE, int NT, int CPW = 32>
+// DT / DL: the top / left pad is g.pad - DT / g.pad - DL (TF "SAME" over an even extent at stride 2: DT, DL = 1)
+template <typename T, int K, int S, int ACT, bool AFFINE, int NT, int CPW = 32, int DT = 0, int DL = 0>
 __global__ void __launch_bounds__(NT)
 dwconv_fwd_kernel(const T* __restrict__ x, const float* __restrict__ scale, const float* __restrict__ shift,
                   const float* __restrict__ wgt, T* __restrict__ out, double* __restrict__ dsum,
@@ -257,7 +260,7 @@ dwconv_fwd_kernel(const T* __restrict__ x, const float* __restrict__ scale, cons
     const int c0 = blockIdx.y * (2 * CPW), n = blockIdx.z;
     const int oy0 = ty * g.TH, ox0 = tx * g.TW;
     const T* img = x + (size_t)n * g.H * g.W * g.C;
-    stage_input_tile<T, ACT, AFFINE, CPW>(tile, img, g.H, g.W, g.C, c0, oy0 * S - g.pad, ox0 * S - g.pad, g.IH, g.IW, scale, shift);
+    stage_input_tile<T, ACT, AFFINE, CPW>(tile, img, g.H, g.W, g.C, c0, oy0 * S - (g.pad - DT), ox0 * S - (g.pad - DL), g.IH, g.IW, scale, shift);
 
     const int ch = c0 + cp * 2;
     const bool chv = ch < g.C;
@@ -505,14 +508,17 @@ dwconv_wgrad_kernel(const T* __restrict__ x, const float* __restrict__ scale, co
 // sigmoid of the input pixel serves both a and swish'.  A CTA walks images blockIdx.z, +gridDim.z, ... so that its
 // k*k weight-gradient partials (registers) are reduced and flushed once, not once per image.
 // ---------------------------------------------------------------------------------------------
-template <typename T, int K, bool WG, int P, int CPW = 32>
+// PT / PL: the zero rows above / columns left of the image, (K-1)/2 (symmetric) or (K-1)/2 - 1 (TF "SAME" over an even
+// extent). Either way the taps that reach input row sy read dy rows (sy + PT - kh)/2 >= -1 and <= (TH+1)/2 - 1 of the tile
+// (columns likewise): the compact tile at (y0/2 - 1, x0/2 - 1) with (TH+1)/2 + 2 rows and TW/2 + 2 columns covers both
+// pads; only the tap parity classes change.
+template <typename T, int K, bool WG, int P, int CPW = 32, int PT = (K - 1) / 2, int PL = (K - 1) / 2>
 __device__ __forceinline__ void strip_bwd_s2(const uint32_t* __restrict__ tile, int IW, int sy, int sx, int lane,
                                              const float (&w)[K * K][2], float (&acc)[P][2],
                                              const float (&av)[P][2], float (&wacc)[K * K][2]) {
-    constexpr int PAD = (K - 1) / 2;
 #pragma unroll
     for (int kh = 0; kh < K; kh++) {
-        const int q = sy + PAD - kh;
+        const int q = sy + PT - kh;
         if (q & 1) continue;                          // warp-uniform: the sub-strips of a warp sit on rows of one parity
         const int row = (q >> 1) + 1;
         const uint32_t* rp = tile + (row * IW + (sx >> 1)) * CPW + lane;
@@ -523,7 +529,7 @@ __device__ __forceinline__ void strip_bwd_s2(const uint32_t* __restrict__ tile, 
         for (int p = 0; p < P; p++) {
 #pragma unroll
             for (int kw = 0; kw < K; kw++) {
-                const int e = p + PAD - kw;
+                const int e = p + PL - kw;
                 if (((e % 2) + 2) % 2 == 0) {
                     const int col = (e + 2) / 2;
                     acc[p][0] = fmaf(vv[col].x, w[kh * K + kw][0], acc[p][0]);
@@ -564,7 +570,8 @@ __device__ __forceinline__ void strip_bwd_s1(const uint32_t* __restrict__ tile, 
 
 // MODE 1: xin is the pre-BN expand output (a = swish(scale*xin + shift), gx = ga * swish', BN-backward sums);
 // MODE 0: xin is the block input itself (DS block): a = xin, gx = ga (+ add).
-template <typename T, int K, int S, bool AFFINE, int MODE, int NT, int P, int CPW = 32>
+// DT / DL (stride 2 only): the top / left pad is (K-1)/2 - DT / (K-1)/2 - DL (see strip_bwd_s2).
+template <typename T, int K, int S, bool AFFINE, int MODE, int NT, int P, int CPW = 32, int DT = 0, int DL = 0>
 #ifndef DW_BWD_OCC3
 #define DW_BWD_OCC3 4
 #endif
@@ -686,7 +693,7 @@ dwconv_bwd_kernel(const T* __restrict__ gy, const T* __restrict__ yout, const fl
 #pragma unroll
             for (int p = 0; p < P; p++) { acc[p][0] = 0.f; acc[p][1] = 0.f; }
             if (S == 1) strip_bwd_s1<T, K, P, CPW>(tile, g.IW, sy, sx, cp, w, acc, av, wacc);
-            else strip_bwd_s2<T, K, true, P, CPW>(tile, g.IW, sy, sx, cp, w, acc, av, wacc);
+            else strip_bwd_s2<T, K, true, P, CPW, (K - 1) / 2 - DT, (K - 1) / 2 - DL>(tile, g.IW, sy, sx, cp, w, acc, av, wacc);
             if (chv) {
                 const uint32_t off0 = (uint32_t)((iy * g.W + ix) * g.C + ch);
 #pragma unroll
@@ -780,7 +787,7 @@ static int dw_cpw(int C) {
 static int fill_geom(DwGeom& g, int N, int H, int W, int C, int K, int S, bool input_space, int cpw = 32) {
     // input_space: tiles partition the INPUT pixels (dgrad); the staged tile is then dy: shifted (S=1) or compact (S=2)
     g.N = N; g.H = H; g.W = W; g.C = C; g.pad = (K - 1) / 2;
-    g.Ho = (H + 2 * g.pad - K) / S + 1;
+    g.Ho = (H + 2 * g.pad - K) / S + 1;           // == ceil(H / S): also the extent of TF "SAME" padding
     g.Wo = (W + 2 * g.pad - K) / S + 1;
     int th_dim = input_space ? H : g.Ho, tw_dim = input_space ? W : g.Wo;
     int eff_s = input_space ? 1 : S;
@@ -856,15 +863,39 @@ extern "C" {
 
 // out[N,Ho,Wo,C] = dwconv(act_in(scale*x + shift)); scale == NULL: x is consumed as is (act_in must be 0).
 // dsum/dsq (optional): per-channel sum / sum of squares of the rounded outputs (fp64, accumulated).
-int dfd_dwconv_fwd(const void* x, const float* scale, const float* shift, const float* w, void* out, int N, int H,
-                   int W, int C, int k, int stride, int act_in, int dt, double* dsum, double* dsq, const void* fin,
-                   void* stream) {
+// dt_ / dl_: the top / left pad is (k-1)/2 - dt_ / (k-1)/2 - dl_ (TF "SAME", stride 2)
+static int dw_fwd(const void* x, const float* scale, const float* shift, const float* w, void* out, int N, int H, int W,
+                  int C, int k, int stride, int dt_, int dl_, int act_in, int dt, double* dsum, double* dsq,
+                  const void* fin, void* stream) {
     if (C % 8 || N <= 0 || H <= 0 || W <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_dwconv_fwd: sizes");
     if (!scale && act_in != DFD_ACT_NONE) return dfd_set_error(DFD_ERR_ARG, "dfd_dwconv_fwd: act without BN");
     if (scale && act_in != DFD_ACT_SWISH) return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_dwconv_fwd: BN input implies Swish");
     DwGeom g;
     const int cpw = dw_cpw(C);
     int smem = fill_geom(g, N, H, W, C, k, stride, false, cpw);
+    // TF "SAME" pads: the staged halo (IH x IW) does not depend on the pads, only the tile origin moves. Instantiated for what
+    // a plan launches: the stride-2 depthwise conv of an inverted-residual block (BN + Swish input) at the default CTA size
+    if (dt_ || dl_) {
+        if (stride != 2 || !scale || dw_nt(k) != (k == 5 ? 128 : 256))
+            return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_dwconv_fwd_pad: asymmetric pads need stride 2, a BN + Swish input and the default CTA size");
+        dim3 grid(g.tiles_x * g.tiles_y, (C + 2 * cpw - 1) / (2 * cpw), N);
+        cudaStream_t st = (cudaStream_t)stream;
+#define FWP1(K_, CPW_, DT_, DL_) do { constexpr int NT = K_ == 5 ? 128 : 256;                                                  \
+        DW_LAUNCH((dwconv_fwd_kernel<T, K_, 2, DFD_ACT_SWISH, true, NT, CPW_, DT_, DL_>), grid, smem, st, (const T*)x, scale, shift, w, \
+                  (T*)out, dsum, dsq, (const BnFinDesc*)fin, g); } while (0)
+#define FWP2(K_, DT_, DL_) do { if (cpw == 32) FWP1(K_, 32, DT_, DL_); else if (cpw == 16) FWP1(K_, 16, DT_, DL_); else FWP1(K_, 8, DT_, DL_); } while (0)
+#define FWP(K_) do { if (dt_ && dl_) FWP2(K_, 1, 1); else if (dt_) FWP2(K_, 1, 0); else FWP2(K_, 0, 1); } while (0)
+        DW_DISPATCH_T(dt, {
+            if (k == 3) FWP(3);
+            else if (k == 5) FWP(5);
+            else return dfd_set_error(DFD_ERR_UNSUPPORTED, "depthwise conv: k in {3,5}, stride in {1,2}");
+        });
+#undef FWP
+#undef FWP2
+#undef FWP1
+        DFD_LAUNCH_CHECK();
+        return DFD_OK;
+    }
     // one CTA per (tile, 2*cpw channels, image): walking several images per CTA (as the fused backward does) was slower
     // here on the GPU this code was first tuned on (not re-measured on the H100) - the forward has no per-CTA state worth amortising and loses the overlap between resident CTAs
     dim3 grid(g.tiles_x * g.tiles_y, (C + 2 * cpw - 1) / (2 * cpw), N);
@@ -879,6 +910,29 @@ int dfd_dwconv_fwd(const void* x, const float* scale, const float* shift, const 
 #undef FW
     DFD_LAUNCH_CHECK();
     return DFD_OK;
+}
+
+// TF "SAME" padding check of the `_pad` entry points: stride 1 takes the symmetric (k-1)/2 only; stride 2 also takes
+// (k-1)/2 - 1 on a side whose extent is even (the output extent is ceil(extent / 2) either way)
+static bool dw_pad_ok(int pad, int extent, int k, int stride) {
+    const int sym = (k - 1) / 2;
+    return pad == sym || (stride == 2 && pad == sym - 1 && extent % 2 == 0);
+}
+
+int dfd_dwconv_fwd(const void* x, const float* scale, const float* shift, const float* w, void* out, int N, int H,
+                   int W, int C, int k, int stride, int act_in, int dt, double* dsum, double* dsq, const void* fin,
+                   void* stream) {
+    return dw_fwd(x, scale, shift, w, out, N, H, W, C, k, stride, 0, 0, act_in, dt, dsum, dsq, fin, stream);
+}
+
+// dfd_dwconv_fwd with the zero rows above (pad_t) and columns left (pad_l) of the image given: TF "SAME" padding
+int dfd_dwconv_fwd_pad(const void* x, const float* scale, const float* shift, const float* w, void* out, int N, int H,
+                       int W, int C, int k, int stride, int pad_t, int pad_l, int act_in, int dt, double* dsum, double* dsq,
+                       const void* fin, void* stream) {
+    if (!dw_pad_ok(pad_t, H, k, stride) || !dw_pad_ok(pad_l, W, k, stride))
+        return dfd_set_error(DFD_ERR_ARG, "dfd_dwconv_fwd_pad: pads are (k-1)/2, or (k-1)/2 - 1 at stride 2 over an even extent");
+    const int sym = (k - 1) / 2;
+    return dw_fwd(x, scale, shift, w, out, N, H, W, C, k, stride, sym - pad_t, sym - pad_l, act_in, dt, dsum, dsq, fin, stream);
 }
 
 // Input gradient of the depthwise conv.
@@ -955,10 +1009,12 @@ int dfd_dwconv_bwd_parts(int N, int H, int W, int C, int k, int stride) {
     return tiles * gz;
 }
 
-int dfd_dwconv_bwd(const void* gy, const void* yout, const float* cA, const float* cB, const float* cC,
-                   const float* w, const void* xin, const float* scale, const float* shift, const float* mean,
-                   const float* rstd, const void* add, void* gx, float* dW, int N, int H, int W, int C, int k,
-                   int stride, int dt, double* s1, double* s2, void* ws, long long ws_bytes, const void* fin, void* stream) {
+// dt_ / dl_: the top / left pad is (k-1)/2 - dt_ / (k-1)/2 - dl_ (stride 2 only, see strip_bwd_s2)
+static int dw_bwd(const void* gy, const void* yout, const float* cA, const float* cB, const float* cC,
+                  const float* w, const void* xin, const float* scale, const float* shift, const float* mean,
+                  const float* rstd, const void* add, void* gx, float* dW, int N, int H, int W, int C, int k,
+                  int stride, int dt_, int dl_, int dt, double* s1, double* s2, void* ws, long long ws_bytes, const void* fin,
+                  void* stream) {
     if (C % 8 || N <= 0 || H <= 0 || W <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_dwconv_bwd: sizes");
     if (!xin || !dW) return dfd_set_error(DFD_ERR_ARG, "dfd_dwconv_bwd: operands");
     if (scale && (!shift || !mean || !rstd || !s1 || !s2)) return dfd_set_error(DFD_ERR_ARG, "dfd_dwconv_bwd: mode 1 operands");
@@ -992,6 +1048,26 @@ int dfd_dwconv_bwd(const void* gy, const void* yout, const float* cA, const floa
         else DW_LAUNCH((dwconv_bwd_kernel<T, K_, S_, AFF, MODE_, NT, 8>), grid, smem, st, BWARGS);                            \
     } while (0)
 #define BW(K_, S_) do { if (scale) { if (cA) BW1(K_, S_, true, 1); else BW1(K_, S_, false, 1); } else { if (cA) BW1(K_, S_, true, 0); else BW1(K_, S_, false, 0); } } while (0)
+    // TF "SAME" pads (one side one element short): instantiated for what a plan launches - the stride-2 depthwise stage of an
+    // inverted-residual block (BN + Swish input, BN backward folded into dy) at the default strip width of each kernel size
+#define BWP1(K_, DT_, DL_) do {                                                                                               \
+        constexpr int PD = K_ == 3 ? 4 : 8;                                                                                   \
+        if (cpw == 16) DW_LAUNCH((dwconv_bwd_kernel<T, K_, 2, true, 1, NT, PD, 16, DT_, DL_>), grid, smem, st, BWARGS);       \
+        else if (cpw == 8) DW_LAUNCH((dwconv_bwd_kernel<T, K_, 2, true, 1, NT, PD, 8, DT_, DL_>), grid, smem, st, BWARGS);    \
+        else DW_LAUNCH((dwconv_bwd_kernel<T, K_, 2, true, 1, NT, PD, 32, DT_, DL_>), grid, smem, st, BWARGS);                 \
+    } while (0)
+#define BWP(K_) do { if (dt_ && dl_) BWP1(K_, 1, 1); else if (dt_) BWP1(K_, 1, 0); else BWP1(K_, 0, 1); } while (0)
+    if (dt_ || dl_) {
+        if (stride != 2 || !scale || !cA)
+            return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_dwconv_bwd_pad: asymmetric pads need stride 2, a BN + Swish input and cA");
+        DW_DISPATCH_T(dt, {
+            if (k == 3) BWP(3);
+            else if (k == 5) BWP(5);
+            else return dfd_set_error(DFD_ERR_UNSUPPORTED, "depthwise conv: k in {3,5}, stride in {1,2}");
+        });
+        DFD_LAUNCH_CHECK();
+        return DFD_OK;
+    }
     DW_DISPATCH_T(dt, {
         if (k == 3 && stride == 1) BW(3, 1);
         else if (k == 3 && stride == 2) BW(3, 2);
@@ -999,11 +1075,35 @@ int dfd_dwconv_bwd(const void* gy, const void* yout, const float* cA, const floa
         else if (k == 5 && stride == 2) BW(5, 2);
         else return dfd_set_error(DFD_ERR_UNSUPPORTED, "depthwise conv: k in {3,5}, stride in {1,2}");
     });
+#undef BWP
+#undef BWP1
 #undef BW
 #undef BW1
 #undef BWARGS
     DFD_LAUNCH_CHECK();
     return DFD_OK;
+}
+
+int dfd_dwconv_bwd(const void* gy, const void* yout, const float* cA, const float* cB, const float* cC,
+                   const float* w, const void* xin, const float* scale, const float* shift, const float* mean,
+                   const float* rstd, const void* add, void* gx, float* dW, int N, int H, int W, int C, int k,
+                   int stride, int dt, double* s1, double* s2, void* ws, long long ws_bytes, const void* fin, void* stream) {
+    return dw_bwd(gy, yout, cA, cB, cC, w, xin, scale, shift, mean, rstd, add, gx, dW, N, H, W, C, k, stride, 0, 0, dt, s1, s2,
+                  ws, ws_bytes, fin, stream);
+}
+
+// dfd_dwconv_bwd of a stage padded with pad_t rows above and pad_l columns left of the image (TF "SAME", as in
+// dfd_dwconv_fwd_pad); the workspace layout and dfd_dwconv_bwd_parts do not depend on the pads
+int dfd_dwconv_bwd_pad(const void* gy, const void* yout, const float* cA, const float* cB, const float* cC,
+                       const float* w, const void* xin, const float* scale, const float* shift, const float* mean,
+                       const float* rstd, const void* add, void* gx, float* dW, int N, int H, int W, int C, int k,
+                       int stride, int pad_t, int pad_l, int dt, double* s1, double* s2, void* ws, long long ws_bytes,
+                       const void* fin, void* stream) {
+    if (!dw_pad_ok(pad_t, H, k, stride) || !dw_pad_ok(pad_l, W, k, stride))
+        return dfd_set_error(DFD_ERR_ARG, "dfd_dwconv_bwd_pad: pads are (k-1)/2, or (k-1)/2 - 1 at stride 2 over an even extent");
+    const int sym = (k - 1) / 2;
+    return dw_bwd(gy, yout, cA, cB, cC, w, xin, scale, shift, mean, rstd, add, gx, dW, N, H, W, C, k, stride, sym - pad_t,
+                  sym - pad_l, dt, s1, s2, ws, ws_bytes, fin, stream);
 }
 
 }  // extern "C"

@@ -17,7 +17,7 @@ from collections import OrderedDict
 import torch
 
 from . import _lib
-from .arch import get_spec, is_no_decay, param_entries, state_entries
+from .arch import conv_pads, get_spec, is_no_decay, param_entries, state_entries
 
 ACT_NONE, ACT_SWISH, ACT_RELU = _lib.ACT_NONE, _lib.ACT_SWISH, _lib.ACT_RELU
 POOL_CHUNKS = 8          # row chunks per image of the pooling kernels when the batch alone cannot fill the GPU
@@ -256,9 +256,9 @@ class Engine:
         self._red_pending.append((off, dW, Cout * Kw, Cout * Kw, splits))
         return ("dfd_conv_wgrad_tc", [dY, X, dW, N, H, W, Cin, Cout, k, stride, self.dt, ("WS", off), nbytes])
 
-    def _dw_bwd(self, args, N, H, W, C, k, stride, fin=None):
+    def _dw_bwd(self, args, N, H, W, C, k, stride, fin=None, name="dfd_dwconv_bwd"):
         if os.environ.get("DFD_NONDET"):
-            return ("dfd_dwconv_bwd", list(args) + [None, 0, fin])
+            return (name, list(args) + [None, 0, fin])
         parts = self.L.cdll.dfd_dwconv_bwd_parts(N, H, W, C, k, stride)
         cw = self.L.cdll.dfd_dwconv_block_channels(C)          # channels per CTA: 64, or 32 / 16 for C = 32, 96 / 144
         cbs = (C + cw - 1) // cw
@@ -267,7 +267,7 @@ class Engine:
         for cb in range(cbs):
             n = min(cw, C - cw * cb) * k * k
             self._red_pending.append((off + cb * parts * cw * k * k * 4, dW + cb * cw * k * k * 4, n, cw * k * k, parts))
-        return ("dfd_dwconv_bwd", list(args) + [("WS", off), nbytes, fin])
+        return (name, list(args) + [("WS", off), nbytes, fin])
 
     def _ws_take(self, nbytes):
         off = getattr(self, "_ws_bytes", 0)
@@ -448,6 +448,17 @@ class Engine:
             blocks.append((b, h, w, ho, wo))
             h, w = ho, wo
         Hf, Wf = h, w
+        # (top, left) pad of the stem and of every depthwise conv at this plan's extents. TF "SAME" padding (pad_type
+        # 'same') is one short on the begin side of a stride-2 layer over an even extent; only such layers are planned
+        # through the `_pad` kernels, every other layer issues exactly the launches of the symmetric models
+        self.conv_pads = conv_pads(spec, self.H, self.W)
+        pads = {name: (pt, pl) for name, k, s_, h_, w_, pt, pl, ho_, wo_ in self.conv_pads}
+        asym = lambda name, k: pads[name] != ((k - 1) // 2, (k - 1) // 2)
+        if asym("conv_stem", 3) and self.stem_impl != "gemm":
+            raise ValueError("stem_impl=%r: TF 'SAME' padding of the stem is planned through dfd_stem_im2col_pad (stem_impl='gemm')"
+                             % (self.stem_impl,))
+        if os.environ.get("DFD_DW_SPLIT_BWD") and any(asym(b.name + ".conv_dw", b.k) for b in spec.blocks):
+            raise ValueError("DFD_DW_SPLIT_BWD: the split depthwise backward has no TF 'SAME' padding variant")
 
         # ---- BN bookkeeping arenas ---------------------------------------------------------------
         bn_specs = [("bn1", spec.stem)]
@@ -548,7 +559,11 @@ class Engine:
         bn = self.bns["bn1"]
         if self.stem_impl == "gemm":
             taps, Kp = self._stem_gemm_setup("conv_stem.weight", spec.stem, 3, N * Hs * Ws)
-            fwd.append(("dfd_stem_im2col", (_ptr(self.x_in), _ptr(self.stem_cols), N, spec.in_chans, self.H, self.W, 3, 2, 1, Kp, dt)))
+            if asym("conv_stem", 3):
+                fwd.append(("dfd_stem_im2col_pad", (_ptr(self.x_in), _ptr(self.stem_cols), N, spec.in_chans, self.H, self.W, 3, 2)
+                            + pads["conv_stem"] + (Kp, dt)))
+            else:
+                fwd.append(("dfd_stem_im2col", (_ptr(self.x_in), _ptr(self.stem_cols), N, spec.in_chans, self.H, self.W, 3, 2, 1, Kp, dt)))
             fwd.append(gemm(_ptr(self.stem_cols), _ptr(self.stem_wpad), _ptr(y0), N * Hs * Ws, spec.stem, Kp, bn))
         else:
             fwd.append(("dfd_stem_fwd", (_ptr(self.x_in), P32("conv_stem.weight"), _ptr(y0), N, spec.in_chans, self.H, self.W,
@@ -581,9 +596,11 @@ class Engine:
                 dw_in, dw_bn, bn_mid, bn_out, pw_name = x, None, self.bns[p + ".bn1"], self.bns[p + ".bn2"], ".conv_pw"
             y2 = self._alloc16(N, ho, wo, b.cmid)
             self.acts[p + ".conv_dw"] = y2
-            fwd.append(("dfd_dwconv_fwd", (_ptr(dw_in), dw_bn.scale if dw_bn else None, dw_bn.shift if dw_bn else None,
-                                           P32(p + ".conv_dw.weight"), _ptr(y2), N, h, w, b.cmid, b.k, b.stride,
-                                           ACT_SWISH if dw_bn else ACT_NONE, dt, bn_mid.fsum, bn_mid.fsq, FF(bn_mid))))
+            dw_pad = pads[p + ".conv_dw"] if asym(p + ".conv_dw", b.k) else ()
+            fwd.append(("dfd_dwconv_fwd" + ("_pad" if dw_pad else ""),
+                        (_ptr(dw_in), dw_bn.scale if dw_bn else None, dw_bn.shift if dw_bn else None,
+                         P32(p + ".conv_dw.weight"), _ptr(y2), N, h, w, b.cmid, b.k, b.stride) + dw_pad +
+                        (ACT_SWISH if dw_bn else ACT_NONE, dt, bn_mid.fsum, bn_mid.fsq, FF(bn_mid))))
             fwd.append(finalize(bn_mid, M2))
             gate_ptr = None
             if b.cse:
@@ -625,7 +642,8 @@ class Engine:
             fwd.append(("dfd_bn_act", [_ptr(y3), bn_out.scale, bn_out.shift, ("TRAIN_ONLY", _ptr(dp_gate)) if dp_gate is not None else None,
                                        _ptr(x) if b.has_residual else None,
                                        _ptr(out), N, ho * wo, b.cout, ACT_NONE, 1 if b.has_residual else 0, dt]))
-            rec.update(y2=y2, a2=a2, y3=y3, out=out, dw_bn=dw_bn, bn_mid=bn_mid, bn_out=bn_out, pw_name=pw_name, dp_gate=dp_gate)
+            rec.update(y2=y2, a2=a2, y3=y3, out=out, dw_bn=dw_bn, bn_mid=bn_mid, bn_out=bn_out, pw_name=pw_name, dp_gate=dp_gate,
+                       dw_pad=dw_pad)
             recs.append(rec)
             x = out
         # head
@@ -744,10 +762,12 @@ class Engine:
                                                      bn_mid.cC, G32(p + ".conv_dw.weight"), N, h, w, b.cmid, b.k, b.stride, dt)))
                 else:
                     # input gradient (through bn1 + Swish) and weight gradient in one pass over the dy tile
+                    dw_pad = rec["dw_pad"]
                     bwd.append(self._dw_bwd((mid_b, _ptr(y2), bn_mid.cA, bn_mid.cB, bn_mid.cC, P32(p + ".conv_dw.weight"),
                                              _ptr(y1), dw_bn.scale, dw_bn.shift, dw_bn.mean, dw_bn.rstd, None, mid_a,
-                                             G32(p + ".conv_dw.weight"), N, h, w, b.cmid, b.k, b.stride, dt,
-                                             dw_bn.bs1, dw_bn.bs2), N, h, w, b.cmid, b.k, b.stride, BF(dw_bn)))
+                                             G32(p + ".conv_dw.weight"), N, h, w, b.cmid, b.k, b.stride) + dw_pad +
+                                            (dt, dw_bn.bs1, dw_bn.bs2), N, h, w, b.cmid, b.k, b.stride, BF(dw_bn),
+                                            name="dfd_dwconv_bwd" + ("_pad" if dw_pad else "")))
                 bwd.append(bwd_finalize(dw_bn, M1))
                 bwd.append(("dfd_bn_bwd_apply", (mid_a, _ptr(y1), None, dw_bn.cA, dw_bn.cB, dw_bn.cC, mid_b, N, h * w, b.cmid, dt)))
                 bwd.append(gemm(mid_b, T16(p + ".conv_pw.weight"), t2, M1, b.cin, b.cmid))
@@ -761,7 +781,9 @@ class Engine:
                 bwd.append(("dfd_dwconv_wgrad", (_ptr(xin), None, None, mid_b, _ptr(y2), bn_mid.cA, bn_mid.cB, bn_mid.cC,
                                                  G32(p + ".conv_dw.weight"), N, h, w, b.cmid, b.k, b.stride, dt)))
             else:
-                # DS block: the depthwise conv reads the block input as is (mode 0 of the fused pass)
+                # DS block: the depthwise conv reads the block input as is (mode 0 of the fused pass); stride 1 in every
+                # EfficientNet, so its padding is symmetric under TF "SAME" too
+                assert not rec["dw_pad"], p
                 bwd.append(self._dw_bwd((mid_b, _ptr(y2), bn_mid.cA, bn_mid.cB, bn_mid.cC, P32(p + ".conv_dw.weight"),
                                          _ptr(xin), None, None, None, None, dout if b.has_residual else None, t2,
                                          G32(p + ".conv_dw.weight"), N, h, w, b.cmid, b.k, b.stride, dt, None, None),
@@ -835,7 +857,7 @@ class Engine:
                 return None
         elif name in ("dfd_bn_act", "dfd_bn_act_drop") and any(isinstance(a, tuple) for a in args):
             args = tuple((a[1] if training else None) if isinstance(a, tuple) else a for a in args)
-        elif not training and name in ("dfd_gemm_tn", "dfd_gemm_tn_rowpack", "dfd_dwconv_fwd"):
+        elif not training and name in ("dfd_gemm_tn", "dfd_gemm_tn_rowpack", "dfd_dwconv_fwd", "dfd_dwconv_fwd_pad"):
             args = tuple(args[:-3]) + (None, None, None)      # eval: no batch statistics, no finalisation
         elif not training and name in ("dfd_gemm_tn_mma", "dfd_stem_fwd"):
             args = tuple(args[:-2]) + (None, None)

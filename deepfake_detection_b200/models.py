@@ -18,11 +18,12 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .arch import SUPPORTED_ARCHS, get_spec, state_entries
+from .arch import SUPPORTED_ARCHS, TF_ARCHS, TF_POOL_CROP, get_spec, state_entries
 from .engine import Engine
 
 _DEFAULT_CFG = dict(num_classes=1000, pool_size=(7, 7), crop_pct=0.875, interpolation="bicubic",
                     mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225))
+_INCEPTION_MEAN_STD = dict(mean=(0.5, 0.5, 0.5), std=(0.5, 0.5, 0.5))      # the AdvProp (_ap) checkpoints' normalisation
 
 
 class _NativeForward(torch.autograd.Function):
@@ -106,6 +107,8 @@ class NativeModel(nn.Module):
         if bn_tf:       # efficientnet_blocks.py:13-30
             bn_momentum = 1 - 0.99 if bn_momentum is None else bn_momentum
             bn_eps = 1e-3 if bn_eps is None else bn_eps
+        if arch in TF_ARCHS:
+            bn_eps = 1e-3       # the tf_* entrypoints overwrite kwargs['bn_eps'] (efficientnet.py:1267), a caller's value included
         self.arch = arch
         self.num_classes = num_classes
         self.in_chans = in_chans
@@ -125,6 +128,11 @@ class NativeModel(nn.Module):
         self.default_cfg = dict(_DEFAULT_CFG, input_size=self.spec.input_size,
                                 first_conv="conv_stem" if self.spec.family == "efficientnet" else "conv1",
                                 classifier="classifier" if self.spec.family == "efficientnet" else "fc")
+        if arch in TF_ARCHS:        # efficientnet.py:112-195
+            pool_size, crop_pct = TF_POOL_CROP[int(arch[len("tf_efficientnet_b")])]
+            self.default_cfg.update(pool_size=pool_size, crop_pct=crop_pct)
+            if arch.endswith("_ap"):
+                self.default_cfg.update(_INCEPTION_MEAN_STD)
         self._engines = OrderedDict()
         self._primary = None
         self._pending_state = None
@@ -258,7 +266,7 @@ def create_model(model_name, pretrained=False, num_classes=1000, in_chans=3, che
     """dfd/timm/models/factory.py:8-64 for the architectures on the native hot path."""
     if pretrained:
         raise _lib.NativeError("pretrained weights need network access; load a checkpoint instead")
-    if model_name not in SUPPORTED_ARCHS:
+    if model_name not in SUPPORTED_ARCHS and model_name not in TF_ARCHS:
         raise RuntimeError("Unknown model (%s)" % model_name)       # factory.py:56
     model = NativeModel(model_name, num_classes=num_classes, in_chans=in_chans, **kwargs)
     if checkpoint_path:

@@ -111,6 +111,19 @@ int dfd_dwconv_bwd_parts(int N, int H, int W, int C, int k, int stride);
 /* channels per CTA of the depthwise kernels for a layer of C channels (64, or 32 / 16 where 64-channel blocks would leave a
  * fifth or more of the lanes idle): the slot width and the channel-block size of the ws layout above */
 int dfd_dwconv_block_channels(int C);
+/* TF "SAME" padding (Conv2dSame, layers/conv2d_same.py; the tf_efficientnet_* models): dfd_dwconv_fwd / dfd_dwconv_bwd with
+ * pad_t zero rows above and pad_l zero columns left of the image. Each is (k-1)/2, or (k-1)/2 - 1 at stride 2 over an even
+ * extent; the output extent is ceil(extent / stride) either way (the end side gets the rest). The asymmetric backward takes
+ * the stride-2 stage of an inverted-residual block only (scale and cA non-NULL). Symmetric pads run exactly the kernels of
+ * the entry points above. */
+int dfd_dwconv_fwd_pad(const void* x, const float* scale, const float* shift, const float* w, void* out, int N, int H,
+                       int W, int C, int k, int stride, int pad_t, int pad_l, int act_in, int dt, double* dsum, double* dsq,
+                       const void* fin, void* stream);
+int dfd_dwconv_bwd_pad(const void* gy, const void* yout, const float* cA, const float* cB, const float* cC,
+                       const float* w, const void* xin, const float* scale, const float* shift, const float* mean,
+                       const float* rstd, const void* add, void* gx, float* dW, int N, int H, int W, int C, int k,
+                       int stride, int pad_t, int pad_l, int dt, double* s1, double* s2, void* ws, long long ws_bytes,
+                       const void* fin, void* stream);
 
 /* ---- stem convolution: conv_stem 3x3 s2 (efficientnet.py:275,321) / conv1 7x7 s2 (resnet.py:379,451) ---- */
 int dfd_stem_fwd(const void* x_nchw, const float* w, void* out_nhwc, int N, int Cin, int H, int W, int Cout, int k,
@@ -123,6 +136,10 @@ int dfd_stem_wgrad(const void* x_nchw, const void* g, const void* y, const float
  * Kp % 8 == 0; weights padded to [Cout, Kp]; fp32 gradient un-padded (accumulating) into the OIHW arena */
 int dfd_stem_im2col(const void* x_nchw, void* cols, int N, int Cin, int H, int W, int k, int stride, int pad, int Kp, int dt,
                     void* stream);
+/* the same with TF "SAME" padding: Ho = ceil(H/stride), Wo = ceil(W/stride); pad_t / pad_l must be the begin sides,
+ * total // 2 of total = max((ceil(i/s) - 1)*s + k - i, 0) (layers/padding.py) */
+int dfd_stem_im2col_pad(const void* x_nchw, void* cols, int N, int Cin, int H, int W, int k, int stride, int pad_t, int pad_l,
+                        int Kp, int dt, void* stream);
 int dfd_pad_weight(const void* src16, void* dst16, int O, int taps, int Kp, int dt, void* stream);
 int dfd_unpad_grad(const float* g_padded, float* g_accum, int O, int taps, int Kp, void* stream);
 
