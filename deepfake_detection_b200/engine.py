@@ -7,17 +7,26 @@ This is the host side of the hot path (dfd/runners/train.py:610-649): given an a
   * builds, once, the ordered list of C-ABI calls ("plan") for forward, backward and the optimizer, and
   * replays the plan on the caller's current CUDA stream (optionally captured into a CUDA graph).
 
+The family's plan builder (engine_efficientnet.build_efficientnet, engine_resnet.build_resnet) lays out the activations
+and lists the ops; the conventions every plan shares (BatchNorm statistics and finalisation, the mask generators, the
+deterministic weight-gradient reduce, validation against the ABI table) are the plan helpers of this class.
+
+A plan op is (name, args). `base_name(name)` is the C-ABI entry point it calls: `<entry>_train` runs in training mode
+only, `<entry>_evalonly` in eval mode only and `dfd_bn_finalize_sync` finalises the summed statistics of all ranks. In
+args, ("TRAIN_ONLY", ptr) is an operand that is NULL in eval mode, "TRAINING" is the mode flag (1 / 0) and ("WS", off)
+a slot of the deterministic-reduce workspace, resolved when the plan is finished.
+
 PyTorch is used for device memory and streams only; there is no PyTorch compute on the hot path and no CPU
 fallback: constructing an Engine without a CUDA device or without libdfd_b200.so raises.
 """
-import ctypes
 import os
+import struct
 from collections import OrderedDict
 
 import torch
 
 from . import _lib
-from .arch import conv_pads, get_spec, is_no_decay, param_entries, state_entries
+from .arch import get_spec, is_no_decay, param_entries, state_entries
 
 ACT_NONE, ACT_SWISH, ACT_RELU = _lib.ACT_NONE, _lib.ACT_SWISH, _lib.ACT_RELU
 POOL_CHUNKS = 8          # row chunks per image of the pooling kernels when the batch alone cannot fill the GPU
@@ -25,6 +34,14 @@ POOL_CHUNKS = 8          # row chunks per image of the pooling kernels when the 
 
 def _ptr(t, off_elems=0):
     return t.data_ptr() + off_elems * t.element_size()
+
+
+def base_name(name):
+    """the C-ABI entry point of the plan op `name`"""
+    for suf in ("_train", "_evalonly", "_sync"):
+        if name.endswith(suf):
+            return name[:-len(suf)]
+    return name
 
 
 class _BN:
@@ -70,6 +87,20 @@ class Engine:
             if dist.is_available() and dist.is_initialized():
                 self.sync_world = dist.get_world_size()
             self.sync_bn = self.sync_world > 1
+        if self.sync_bn and spec.family == "resnet":
+            raise _lib.NativeError("sync_bn over %d ranks: the ResNet plan has no synchronised BatchNorm (only the "
+                                   "EfficientNet plan all-reduces its batch statistics)" % self.sync_world)
+        # DFD_NONDET=1: weight gradients flushed with atomics instead of the ordered reduce (see _wgrad)
+        self._nondet = bool(os.environ.get("DFD_NONDET"))
+        # BatchNorm finalisation by the last CTA of the statistics-producing kernel (descriptors, csrc/bn_finalize.cuh)
+        # instead of one-block launches: implemented and tested, but off by default: every CTA pays a __threadfence + a
+        # same-address ticket atomic before it may retire (the depthwise kernels run ~14k short CTAs), and the one finalising
+        # CTA walks C channels with a fraction of the threads of the standalone launch. DFD_FUSED_FINALIZE=1: every
+        # producer, forward and backward; =gemm: only the EfficientNet BatchNorms whose statistics come from the persistent
+        # tensor-core GEMM (one CTA per SM: the ticket is free there). Never with synchronised BatchNorm.
+        ff_mode = os.environ.get("DFD_FUSED_FINALIZE", "")
+        self._fused_fin = ff_mode not in ("", "0", "gemm") and not self.sync_bn
+        self._fused_gemm = (self._fused_fin or ff_mode == "gemm") and not self.sync_bn
         self.bn_momentum = float(bn_momentum)
         self.bn_eps = float(bn_eps)
         self.gemm_impl = gemm_impl
@@ -164,7 +195,6 @@ class Engine:
                 self.t_off[n] = (toff, s[0], s[1])
                 toff += (s[0] * s[1] + 7) // 8 * 8
         self.paramsT16 = torch.zeros(max(toff, 8), dtype=self.tdtype, device=dev)
-        import struct
         raw = b"".join(struct.pack("<QQii", _ptr(self.params16, self.p_off[n][0]), _ptr(self.paramsT16, o), O, I)
                        for n, (o, O, I) in self.t_off.items())
         self._ttable = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(dev)
@@ -238,7 +268,7 @@ class Engine:
     def _wgrad(self, G, X, dW, M, Nw, Kw):
         if self._wgrad_name != "dfd_gemm_wgrad":
             return (self._wgrad_name, (G, X, dW, M, Nw, Kw, self.dt))
-        if os.environ.get("DFD_NONDET"):
+        if self._nondet:
             return ("dfd_gemm_wgrad", (G, X, dW, M, Nw, Kw, self.dt, None, 0))
         splits = self.L.cdll.dfd_gemm_wgrad_splits(M, Nw, Kw)
         off, nbytes = self._ws_take(splits * Nw * Kw * 4)
@@ -249,7 +279,7 @@ class Engine:
         """implicit-GEMM weight gradient of a dense k x k convolution (H, W = input extents) into the packed
         [Cout][kh][kw][Cin] fp32 buffer"""
         Kw = k * k * Cin
-        if os.environ.get("DFD_NONDET"):
+        if self._nondet:
             return ("dfd_conv_wgrad_tc", (dY, X, dW, N, H, W, Cin, Cout, k, stride, self.dt, None, 0))
         splits = self.L.cdll.dfd_conv_wgrad_splits(N, H, W, Cin, Cout, k, stride)
         off, nbytes = self._ws_take(splits * Cout * Kw * 4)
@@ -257,7 +287,7 @@ class Engine:
         return ("dfd_conv_wgrad_tc", [dY, X, dW, N, H, W, Cin, Cout, k, stride, self.dt, ("WS", off), nbytes])
 
     def _dw_bwd(self, args, N, H, W, C, k, stride, fin=None, name="dfd_dwconv_bwd"):
-        if os.environ.get("DFD_NONDET"):
+        if self._nondet:
             return (name, list(args) + [None, 0, fin])
         parts = self.L.cdll.dfd_dwconv_bwd_parts(N, H, W, C, k, stride)
         cw = self.L.cdll.dfd_dwconv_block_channels(C)          # channels per CTA: 64, or 32 / 16 for C = 32, 96 / 144
@@ -282,7 +312,6 @@ class Engine:
             del pend[:]
 
     def _patch_workspace(self, ops):
-        import struct
         self._flush_reduce(ops)
         total = getattr(self, "_ws_bytes", 0)
         if not total:
@@ -329,7 +358,6 @@ class Engine:
     # the optimizer refreshes them once per step for every plan that shares the weights.
     def _upload_fin_descs(self):
         """fill the BatchNorm finalisation descriptors once the plan knows every layer's element count"""
-        import struct
         n = len(self.bns)
         raw = bytearray(2 * n * 128)
         for bn in self.bns.values():
@@ -362,7 +390,6 @@ class Engine:
         _lib.call("dfd_transpose_weights", _ptr(o._ttable), o._ttable_count, o.dt, stream)
         reg = getattr(o, "_bd_reg", None)
         if reg and getattr(o, "_bd_table", None) is None:
-            import struct
             raw = b"".join(struct.pack("<QQiiii", B, _ptr(t), Nn, K, pack, 0) for (B, Nn, K, pack), t in reg.items())
             o._bd_table = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(o.device)
         if getattr(o, "_rtable_count", 0):
@@ -427,393 +454,79 @@ class Engine:
 
 
     def _build(self):
-        if self.spec.family == "resnet":
-            from .engine_resnet import build_resnet
-            return build_resnet(self)
-        spec, N, dev, L = self.spec, self.N, self.device, self.L
-        S = L.stat_slots
-        self._keep = []
-        self.acts = {}
-        fwd, bwd = [], []
-        bn_list = []
+        from .engine_efficientnet import build_efficientnet
+        from .engine_resnet import build_resnet
+        (build_resnet if self.spec.family == "resnet" else build_efficientnet)(self)
 
-        # ---- pass 1: shapes --------------------------------------------------------------------
-        Hs = (self.H + 2 - 3) // 2 + 1
-        Ws = (self.W + 2 - 3) // 2 + 1
-        blocks = []
-        h, w = Hs, Ws
-        for b in spec.blocks:
-            ho = (h + 2 * b.pad - b.k) // b.stride + 1
-            wo = (w + 2 * b.pad - b.k) // b.stride + 1
-            blocks.append((b, h, w, ho, wo))
-            h, w = ho, wo
-        Hf, Wf = h, w
-        # (top, left) pad of the stem and of every depthwise conv at this plan's extents. TF "SAME" padding (pad_type
-        # 'same') is one short on the begin side of a stride-2 layer over an even extent; only such layers are planned
-        # through the `_pad` kernels, every other layer issues exactly the launches of the symmetric models
-        self.conv_pads = conv_pads(spec, self.H, self.W)
-        pads = {name: (pt, pl) for name, k, s_, h_, w_, pt, pl, ho_, wo_ in self.conv_pads}
-        asym = lambda name, k: pads[name] != ((k - 1) // 2, (k - 1) // 2)
-        if asym("conv_stem", 3) and self.stem_impl != "gemm":
-            raise ValueError("stem_impl=%r: TF 'SAME' padding of the stem is planned through dfd_stem_im2col_pad (stem_impl='gemm')"
-                             % (self.stem_impl,))
-        if os.environ.get("DFD_DW_SPLIT_BWD") and any(asym(b.name + ".conv_dw", b.k) for b in spec.blocks):
-            raise ValueError("DFD_DW_SPLIT_BWD: the split depthwise backward has no TF 'SAME' padding variant")
+    # ---- plan helpers shared by the family builders ---------------------------------------------------------------------
+    def _stats(self, bn, fuse=False):
+        """a forward producer's (sum, sum of squares, finalisation descriptor) operands for `bn`, all training-only (NULL in
+        eval mode). With `fuse` the producer's last CTA finalises `bn` in training, and its finalise op runs in eval only."""
+        if bn is None:
+            return None, None, None
+        bn.fused = fuse
+        return ("TRAIN_ONLY", bn.fsum), ("TRAIN_ONLY", bn.fsq), ("TRAIN_ONLY", bn.fin) if fuse else None
 
-        # ---- BN bookkeeping arenas ---------------------------------------------------------------
-        bn_specs = [("bn1", spec.stem)]
-        for b in spec.blocks:
-            if b.kind == "ir":
-                bn_specs += [(b.name + ".bn1", b.cmid), (b.name + ".bn2", b.cmid), (b.name + ".bn3", b.cout)]
-            else:
-                bn_specs += [(b.name + ".bn1", b.cmid), (b.name + ".bn2", b.cout)]
-        bn_specs.append(("bn2", spec.num_features))
-        self._alloc_bn(bn_specs)
+    def _gemm(self, A, B, C, M, Nn, K, bn=None, fuse=False, rowpack=True):
+        """C [M, Nn] = A [M, K] . B [Nn, K]^T (+ the batch statistics of `bn` over C); `fuse`: see _stats"""
+        if self.gemm_impl != "tc":
+            return ("dfd_gemm_tn_mma", (A, B, C, None, M, Nn, K, self.dt) + self._stats(bn)[:2])
+        fs, fq, fin = self._stats(bn, fuse)
+        pack = self._row_pack(M, K) if rowpack else 1
+        if pack > 1:
+            return ("dfd_gemm_tn_rowpack", (A, self._blockdiag(B, Nn, K, pack), C, M, Nn, K, pack, self.dt, fs, fq, fin))
+        return ("dfd_gemm_tn", (A, B, C, M, Nn, K, self.dt, fs, fq, fin))
 
-        P32 = lambda n: _ptr(self.params32, self.p_off[n][0])
-        G32 = lambda n: _ptr(self.grads32, self.p_off[n][0])
-        P16 = lambda n: _ptr(self.params16, self.p_off[n][0])
-        T16 = lambda n: _ptr(self.paramsT16, self.t_off[n][0])
-        dt = self.dt
-        mom, eps = self.bn_momentum, self.bn_eps
+    def _finalize(self, bn, count):
+        """ops that finalise `bn` over `count` elements per rank: batch statistics -> scale / shift and the running
+        statistics in training, running statistics -> scale / shift in eval (once per weight state, see forward).
+        Synchronised BatchNorm finalises the SUM of every rank's statistics against the global count (torch SyncBatchNorm)."""
+        bn.count = count
+        args = [bn.fsum, bn.fsq, float(count), bn.gamma, bn.beta, bn.rm, bn.rv, bn.nbt, self.bn_momentum, self.bn_eps,
+                "TRAINING", bn.C, bn.scale, bn.shift, bn.mean, bn.rstd]
+        if self.sync_bn:
+            return [("ALLREDUCE_train", (self.stats[bn.stat_off:bn.stat_off + 2 * self.L.stat_slots * bn.C], "sum")),
+                    ("dfd_bn_finalize_sync", args)]
+        return [("dfd_bn_finalize" + ("_evalonly" if bn.fused else ""), args)]
 
-        # BatchNorm finalisation by the last CTA of the statistics-producing kernel (descriptors, csrc/bn_finalize.cuh) instead of
-        # 98 one-block launches: implemented and tested, but off by default: every CTA pays a __threadfence + a same-address
-        # ticket atomic before it may retire (the depthwise kernels run ~14k short CTAs), and the one finalising CTA walks C
-        # channels with a fraction of the threads of the standalone launch. Off unless DFD_FUSED_FINALIZE=1.
-        # DFD_FUSED_FINALIZE=gemm: only the BatchNorms whose statistics come from the persistent tensor-core GEMM (one CTA per
-        # SM: the ticket is free there) are finalised by their producer; =1: every producer, forward and backward.
-        ff_mode = os.environ.get("DFD_FUSED_FINALIZE", "")
-        fused_fin = ff_mode not in ("", "0", "gemm") and not self.sync_bn
-        fused_gemm = (fused_fin or ff_mode == "gemm") and not self.sync_bn
+    def _bwd_finalize(self, bn, count):
+        """ops that turn the backward sums of `bn` into the coefficients of dy (none when the producer's last CTA does it).
+        Synchronised BatchNorm averages (sum g, sum g*xhat) over the ranks and keeps the LOCAL count: the coefficients then use
+        the global means, and dgamma / dbeta receive global_sum / world - what the DDP gradient mean of the per-rank sums gives."""
+        bn.count = count
+        op = ("dfd_bn_bwd_finalize", (bn.bs1, bn.bs2, float(count), bn.gamma, bn.mean, bn.rstd, bn.dgamma, bn.dbeta,
+                                      bn.cA, bn.cB, bn.cC, bn.C))
+        if self.sync_bn:
+            S = self.L.stat_slots
+            return [("ALLREDUCE", (self.stats[bn.stat_off + 2 * S * bn.C:bn.stat_off + 4 * S * bn.C], "avg")), op]
+        return [] if self._fused_fin else [op]
 
-        def gemm(A, B, C, M, Nn, K, bn=None):
-            fs, fq = (bn.fsum, bn.fsq) if bn is not None else (None, None)
-            if self.gemm_impl == "tc":
-                fin = bn.fin if (bn is not None and fused_gemm) else None
-                if bn is not None:
-                    bn.fused = fin is not None
-                pack = self._row_pack(M, K)
-                if pack > 1:
-                    return ("dfd_gemm_tn_rowpack", (A, self._blockdiag(B, Nn, K, pack), C, M, Nn, K, pack, dt, fs, fq, fin))
-                return ("dfd_gemm_tn", (A, B, C, M, Nn, K, dt, fs, fq, fin))
-            return ("dfd_gemm_tn_mma", (A, B, C, None, M, Nn, K, dt, fs, fq))
+    def _bfin(self, bn):
+        """the finalisation descriptor a backward producer of `bn`'s sums takes (NULL: a dfd_bn_bwd_finalize op follows)"""
+        return bn.bfin if self._fused_fin else None
 
-        def finalize(bn, count):
-            # Training: the producing kernel's last CTA finalises (descriptor bn.fin), this op is skipped (see _run); it runs
-            # in eval mode (running statistics -> scale / shift, once per weight state) and when the producer cannot finalise.
-            bn.count = count
-            if self.sync_bn:
-                # SUM of every rank's statistics, finalised against the GLOBAL element count (torch SyncBatchNorm semantics)
-                fwd.append(("ALLREDUCE_train", (self.stats[bn.stat_off:bn.stat_off + 2 * S * bn.C], "sum")))
-                return ("dfd_bn_finalize_sync", [bn.fsum, bn.fsq, float(count), bn.gamma, bn.beta, bn.rm, bn.rv, bn.nbt, mom, eps,
-                                                 "TRAINING", bn.C, bn.scale, bn.shift, bn.mean, bn.rstd])
-            return ("dfd_bn_finalize" + ("_evalonly" if bn.fused else ""),
-                    [bn.fsum, bn.fsq, float(count), bn.gamma, bn.beta, bn.rm, bn.rv, bn.nbt, mom, eps,
-                     "TRAINING", bn.C, bn.scale, bn.shift, bn.mean, bn.rstd])
-
-        def bwd_finalize(bn, count):
-            bn.count = count
-            if self.sync_bn:
-                # MEAN over the ranks of (sum g, sum g*xhat) with the LOCAL count: the coefficients of dy then use the global
-                # means, and dgamma / dbeta receive global_sum / world - what the DDP gradient mean of the per-rank sums gives
-                bwd.append(("ALLREDUCE", (self.stats[bn.stat_off + 2 * S * bn.C:bn.stat_off + 4 * S * bn.C], "avg")))
-                return ("dfd_bn_bwd_finalize", (bn.bs1, bn.bs2, float(count), bn.gamma, bn.mean, bn.rstd, bn.dgamma, bn.dbeta,
-                                                bn.cA, bn.cB, bn.cC, bn.C))
-            if fused_fin:
-                return None         # done by the last CTA of the kernel that produced bs1 / bs2 (descriptor bn.bfin)
-            return ("dfd_bn_bwd_finalize", (bn.bs1, bn.bs2, float(count), bn.gamma, bn.mean, bn.rstd, bn.dgamma, bn.dbeta,
-                                            bn.cA, bn.cB, bn.cC, bn.C))
-
-        BF = (lambda bn: bn.bfin) if fused_fin else (lambda bn: None)
-        def FF(bn):         # forward producer other than the GEMM (depthwise conv): fused finalisation of its BatchNorm
-            bn.fused = fused_fin
-            return bn.fin if fused_fin else None
-
-        # ---- scratch for backward ----------------------------------------------------------------
-        mid_max = max([N * h * w * b.cmid for b, h, w, ho, wo in blocks if b.kind == "ir"] +
-                      [N * ho * wo * b.cmid for b, h, w, ho, wo in blocks] + [N * Hf * Wf * spec.num_features] +
-                      [N * Hs * Ws * spec.stem])
-        small_max = max([N * h * w * b.cin for b, h, w, ho, wo in blocks] +
-                        [N * ho * wo * b.cout for b, h, w, ho, wo in blocks])
-        self.mid = [self._alloc16(mid_max) for _ in range(2)]
-        self.small = [self._alloc16(small_max) for _ in range(3)]
-        mid_a, mid_b = _ptr(self.mid[0]), _ptr(self.mid[1])
-        sm = [_ptr(t) for t in self.small]
-        se_max_c = max([b.cmid for b in spec.blocks if b.cse] + [8])
-        se_max_r = max([b.cse for b in spec.blocks if b.cse] + [8])
-        self.se_tmp = torch.zeros(3 * N * se_max_c + 2 * N * se_max_r, dtype=torch.float32, device=dev)
-        se_draw = _ptr(self.se_tmp)
-        self.pool_partial = torch.zeros(POOL_CHUNKS * N * max(se_max_c, spec.num_features), dtype=torch.float32, device=dev)
-        se_de = _ptr(self.se_tmp, N * se_max_c)
-        se_dpool = _ptr(self.se_tmp, 2 * N * se_max_c)
-        se_r = _ptr(self.se_tmp, 3 * N * se_max_c)
-        se_drp = _ptr(self.se_tmp, 3 * N * se_max_c + N * se_max_r)
-
-        # ---- forward -----------------------------------------------------------------------------
-        self.x_in = torch.zeros(N, spec.in_chans, self.H, self.W, dtype=self.tdtype, device=dev)
-        y0 = self._alloc16(N, Hs, Ws, spec.stem)
-        stem_out = self._alloc16(N, Hs, Ws, spec.stem)
-        self.acts["conv_stem"] = y0
-        self.acts["stem.out"] = stem_out
-        bn = self.bns["bn1"]
-        if self.stem_impl == "gemm":
-            taps, Kp = self._stem_gemm_setup("conv_stem.weight", spec.stem, 3, N * Hs * Ws)
-            if asym("conv_stem", 3):
-                fwd.append(("dfd_stem_im2col_pad", (_ptr(self.x_in), _ptr(self.stem_cols), N, spec.in_chans, self.H, self.W, 3, 2)
-                            + pads["conv_stem"] + (Kp, dt)))
-            else:
-                fwd.append(("dfd_stem_im2col", (_ptr(self.x_in), _ptr(self.stem_cols), N, spec.in_chans, self.H, self.W, 3, 2, 1, Kp, dt)))
-            fwd.append(gemm(_ptr(self.stem_cols), _ptr(self.stem_wpad), _ptr(y0), N * Hs * Ws, spec.stem, Kp, bn))
-        else:
-            fwd.append(("dfd_stem_fwd", (_ptr(self.x_in), P32("conv_stem.weight"), _ptr(y0), N, spec.in_chans, self.H, self.W,
-                                         spec.stem, 3, 2, 1, dt, bn.fsum, bn.fsq)))
-        fwd.append(finalize(bn, N * Hs * Ws))
-        fwd.append(("dfd_bn_act", (_ptr(y0), bn.scale, bn.shift, None, None, _ptr(stem_out), N, Hs * Ws, spec.stem,
-                                   ACT_SWISH, 0, dt)))
-        x = stem_out
-        recs = []
-        # stochastic regularisation (train mode only): per-sample drop-path scale of every residual block
-        # (rate = drop_path_rate * block_idx / n_blocks, efficientnet_builder.py:228-230,343) and the classifier dropout mask;
-        # the gates are [N, C] fp32 tensors (one draw per sample replicated over the channels) filled by ONE dfd_rng_masks
-        # launch at the head of the forward plan, consumed through the GATE operand of dfd_bn_act
-        masks = []               # (tensor, rows, width, keep_prob)
-        n_blocks = len(blocks)
-        ones_c = zeros_c = None
-        for bi, (b, h, w, ho, wo) in enumerate(blocks):
-            p = b.name
-            M1, M2 = N * h * w, N * ho * wo
-            rec = dict(b=b, h=h, w=w, ho=ho, wo=wo, x=x)
-            if b.kind == "ir":
-                bn1, bn2, bn3 = self.bns[p + ".bn1"], self.bns[p + ".bn2"], self.bns[p + ".bn3"]
-                y1 = self._alloc16(N, h, w, b.cmid)
-                self.acts[p + ".conv_pw"] = y1
-                fwd.append(gemm(_ptr(x), P16(p + ".conv_pw.weight"), _ptr(y1), M1, b.cmid, b.cin, bn1))
-                fwd.append(finalize(bn1, M1))
-                dw_in, dw_bn, bn_mid, bn_out, pw_name = y1, bn1, bn2, bn3, ".conv_pwl"
-                rec.update(y1=y1)
-            else:
-                dw_in, dw_bn, bn_mid, bn_out, pw_name = x, None, self.bns[p + ".bn1"], self.bns[p + ".bn2"], ".conv_pw"
-            y2 = self._alloc16(N, ho, wo, b.cmid)
-            self.acts[p + ".conv_dw"] = y2
-            dw_pad = pads[p + ".conv_dw"] if asym(p + ".conv_dw", b.k) else ()
-            fwd.append(("dfd_dwconv_fwd" + ("_pad" if dw_pad else ""),
-                        (_ptr(dw_in), dw_bn.scale if dw_bn else None, dw_bn.shift if dw_bn else None,
-                         P32(p + ".conv_dw.weight"), _ptr(y2), N, h, w, b.cmid, b.k, b.stride) + dw_pad +
-                        (ACT_SWISH if dw_bn else ACT_NONE, dt, bn_mid.fsum, bn_mid.fsq, FF(bn_mid))))
-            fwd.append(finalize(bn_mid, M2))
-            gate_ptr = None
-            if b.cse:
-                pooled = torch.zeros(N, b.cmid, dtype=torch.float32, device=dev)
-                gate = torch.zeros(N, b.cmid, dtype=torch.float32, device=dev)
-                self._keep += [pooled, gate]
-                rec.update(pooled=pooled, gate=gate)
-                if os.environ.get("DFD_SE_FUSED"):
-                    # squeeze + excite in ONE launch (the CTA that completes an image's pooled vector runs its FC chain):
-                    # slower than the two launches on the GPU this code was first tuned on (not re-measured on the H100):
-                    # a 256-thread CTA walks the latency-bound chain four times longer than the 1024-thread FC kernel and
-                    # the tail is not hidden; kept selectable
-                    fwd.append(("dfd_pool_se", (_ptr(y2), bn_mid.scale, bn_mid.shift, _ptr(pooled), P32(p + ".se.conv_reduce.weight"),
-                                                P32(p + ".se.conv_reduce.bias"), P32(p + ".se.conv_expand.weight"),
-                                                P32(p + ".se.conv_expand.bias"), _ptr(gate), N, ho * wo, b.cmid, b.cse, ACT_SWISH, dt,
-                                                POOL_CHUNKS)))
-                else:
-                    fwd.append(("dfd_pool", (_ptr(y2), bn_mid.scale, bn_mid.shift, _ptr(pooled), N, ho * wo, b.cmid, ACT_SWISH, dt,
-                                             None, POOL_CHUNKS)))
-                    fwd.append(("dfd_se_fc_fwd", (_ptr(pooled), P32(p + ".se.conv_reduce.weight"), P32(p + ".se.conv_reduce.bias"),
-                                                  P32(p + ".se.conv_expand.weight"), P32(p + ".se.conv_expand.bias"),
-                                                  _ptr(gate), N, b.cmid, b.cse)))
-                gate_ptr = _ptr(gate)
-            a2 = self._alloc16(N, ho, wo, b.cmid)
-            fwd.append(("dfd_bn_act", (_ptr(y2), bn_mid.scale, bn_mid.shift, gate_ptr, None, _ptr(a2), N, ho * wo, b.cmid,
-                                       ACT_SWISH, 0, dt)))
-            y3 = self._alloc16(N, ho, wo, b.cout)
-            self.acts[p + pw_name] = y3
-            fwd.append(gemm(_ptr(a2), P16(p + pw_name + ".weight"), _ptr(y3), M2, b.cout, b.cmid, bn_out))
-            fwd.append(finalize(bn_out, M2))
-            out = self._alloc16(N, ho, wo, b.cout)
-            self.acts[p + ".out"] = out
-            dp_rate = self.drop_path_rate * bi / n_blocks if b.has_residual else 0.0
-            dp_gate = None
-            if dp_rate > 0.0:
-                dp_gate = torch.ones(N, b.cout, dtype=torch.float32, device=dev)
-                self._keep.append(dp_gate)
-                masks.append((dp_gate, N, b.cout, 1.0 - dp_rate))
-            fwd.append(("dfd_bn_act", [_ptr(y3), bn_out.scale, bn_out.shift, ("TRAIN_ONLY", _ptr(dp_gate)) if dp_gate is not None else None,
-                                       _ptr(x) if b.has_residual else None,
-                                       _ptr(out), N, ho * wo, b.cout, ACT_NONE, 1 if b.has_residual else 0, dt]))
-            rec.update(y2=y2, a2=a2, y3=y3, out=out, dw_bn=dw_bn, bn_mid=bn_mid, bn_out=bn_out, pw_name=pw_name, dp_gate=dp_gate,
-                       dw_pad=dw_pad)
-            recs.append(rec)
-            x = out
-        # head
-        F = spec.num_features
-        Mf = N * Hf * Wf
-        bnh = self.bns["bn2"]
-        yh = self._alloc16(N, Hf, Wf, F)
-        self.acts["conv_head"] = yh
-        fwd.append(gemm(_ptr(x), P16("conv_head.weight"), _ptr(yh), Mf, F, spec.head_in, bnh))
-        fwd.append(finalize(bnh, Mf))
-        P, pool_t = spec.pooled_features, _lib.POOL_TYPES[spec.global_pool]
-        self.pooled = torch.zeros(N, P, dtype=torch.float32, device=dev)
-        if pool_t == _lib.POOL_TYPES["avg"]:
-            fwd.append(("dfd_pool", (_ptr(yh), bnh.scale, bnh.shift, _ptr(self.pooled), N, Hf * Wf, F, ACT_SWISH, dt,
-                                     None, POOL_CHUNKS)))
-        else:
-            # max / avgmax / catavgmax: one pass gives the mean (dfd_pool's order), the max and its argmax for the backward
-            self.pool_argmax = torch.zeros(N, F, dtype=torch.int32, device=dev)
-            fwd.append(("dfd_global_pool", (_ptr(yh), bnh.scale, bnh.shift, _ptr(self.pooled), _ptr(self.pool_argmax), N,
-                                            Hf * Wf, F, ACT_SWISH, pool_t, dt, POOL_CHUNKS)))
-        self.drop_masks = OrderedDict()
-        if self.drop_rate > 0.0:
-            self.dropout_mask = torch.ones(N, P, dtype=torch.float32, device=dev)
-            masks.append((self.dropout_mask, N * P, 1, 1.0 - self.drop_rate))
-            fwd.append(("dfd_mul_f32_train", (_ptr(self.pooled), _ptr(self.dropout_mask), N * P)))
-        for r_ in recs:
-            if r_["dp_gate"] is not None:
-                self.drop_masks[r_["b"].name] = r_["dp_gate"]
+    def _mask_head(self, masks, n_drop_block=0):
+        """the ops at the head of the training forward that draw the step's masks: the DropBlock sites of
+        self._drop_block_table, then the dropout / drop-path masks (tensor, rows, width, keep_prob); the generator's step then
+        advances on the device"""
+        head = []
+        if n_drop_block:
+            head.append(("dfd_memset_async_train", (_ptr(self.drop_block_kept), 0, 8 * n_drop_block)))
+            head.append(("dfd_drop_block_masks_train", (_ptr(self._drop_block_table), n_drop_block, _ptr(self.rng_state))))
         if masks:
-            import struct
             raw = b"".join(struct.pack("<Qqifii", _ptr(t), rows, width, keep, si, 0) for si, (t, rows, width, keep) in enumerate(masks))
-            self._mask_table = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(dev)
-            fwd.insert(0, ("dfd_rng_masks_train", (_ptr(self._mask_table), len(masks), _ptr(self.rng_state))))
-            fwd.insert(1, ("dfd_rng_tick_train", (_ptr(self.rng_state),)))
-            cmax = max(t.shape[-1] for t, _, _, _ in masks)
-            self._unit_affine = torch.cat([torch.ones(cmax, device=dev), torch.zeros(cmax, device=dev)]).float()
-            self._keep.append(self._unit_affine)
-        K = spec.num_classes
-        self.logits = torch.zeros(N, K, dtype=torch.float32, device=dev)
-        self.dlogits = torch.zeros(N, K, dtype=torch.float32, device=dev)
-        self.dpooled = torch.zeros(N, P, dtype=torch.float32, device=dev)
-        self.target_i = torch.zeros(N, dtype=torch.int64, device=dev)
-        self.target_f = torch.zeros(N, K, dtype=torch.float32, device=dev)
-        self._head_in = x
+            self._mask_table = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(self.device)
+            head.append(("dfd_rng_masks_train", (_ptr(self._mask_table), len(masks), _ptr(self.rng_state))))
+        if head:
+            head.append(("dfd_rng_tick_train", (_ptr(self.rng_state),)))
+        return head
 
-        # ---- backward ----------------------------------------------------------------------------
-        bwd.append(("dfd_head_bwd", (_ptr(self.dlogits), _ptr(self.pooled), P32("classifier.weight"),
-                                     G32("classifier.weight"), G32("classifier.bias"), _ptr(self.dpooled), N, P, K)))
-        if self.drop_rate > 0.0:
-            bwd.append(("dfd_mul_f32", (_ptr(self.dpooled), _ptr(self.dropout_mask), N * P)))
-        if pool_t == _lib.POOL_TYPES["avg"]:
-            bwd.append(("dfd_act_bwd", (None, _ptr(yh), bnh.scale, bnh.shift, bnh.mean, bnh.rstd, None, _ptr(self.dpooled),
-                                        mid_a, N, Hf * Wf, F, ACT_SWISH, dt, bnh.bs1, bnh.bs2, BF(bnh))))
-        else:
-            bwd.append(("dfd_act_bwd_gpool", (_ptr(yh), bnh.scale, bnh.shift, bnh.mean, bnh.rstd, _ptr(self.dpooled),
-                                              _ptr(self.pool_argmax), mid_a, N, Hf * Wf, F, ACT_SWISH, pool_t, dt, bnh.bs1,
-                                              bnh.bs2, BF(bnh))))
-        bwd.append(bwd_finalize(bnh, Mf))
-        bwd.append(("dfd_bn_bwd_apply", (mid_a, _ptr(yh), None, bnh.cA, bnh.cB, bnh.cC, mid_b, N, Hf * Wf, F, dt)))
-        cur = 0
-        bwd.append(gemm(mid_b, T16("conv_head.weight"), sm[cur], Mf, spec.head_in, F))
-        bwd.append(self._wgrad(mid_b, _ptr(self._head_in), G32("conv_head.weight"), Mf, F, spec.head_in))
-        self._flush_reduce(bwd)
-        for rec in reversed(recs):
-            b, h, w, ho, wo, xin = rec["b"], rec["h"], rec["w"], rec["ho"], rec["wo"], rec["x"]
-            p = b.name
-            M1, M2 = N * h * w, N * ho * wo
-            bn_out, bn_mid, dw_bn, pw_name = rec["bn_out"], rec["bn_mid"], rec["dw_bn"], rec["pw_name"]
-            y2, a2, y3 = rec["y2"], rec["a2"], rec["y3"]
-            dout = sm[cur]
-            t1, t2 = sm[(cur + 1) % 3], sm[(cur + 2) % 3]
-            gbn = dout
-            if rec["dp_gate"] is not None:
-                # drop path: the gradient reaching bn3 is dout * mask / keep (the identity branch keeps dout itself); one extra
-                # pass through the gated streaming kernel with a unit affine, only in this regularised configuration
-                cm = self._unit_affine.numel() // 2
-                bwd.append(("dfd_bn_act", (dout, _ptr(self._unit_affine), _ptr(self._unit_affine, cm), _ptr(rec["dp_gate"]), None, t2,
-                                           N, ho * wo, b.cout, ACT_NONE, 0, dt)))
-                gbn = t2
-            bwd.append(("dfd_bn_bwd_reduce", (gbn, _ptr(y3), None, bn_out.mean, bn_out.rstd, N, ho * wo, b.cout, dt,
-                                              bn_out.bs1, bn_out.bs2, BF(bn_out))))
-            bwd.append(bwd_finalize(bn_out, M2))
-            bwd.append(("dfd_bn_bwd_apply", (gbn, _ptr(y3), None, bn_out.cA, bn_out.cB, bn_out.cC, t1, N, ho * wo, b.cout, dt)))
-            bwd.append(gemm(t1, T16(p + pw_name + ".weight"), mid_a, M2, b.cmid, b.cout))
-            bwd.append(self._wgrad(t1, _ptr(a2), G32(p + pw_name + ".weight"), M2, b.cout, b.cmid))
-            gate_ptr = dpool_ptr = None
-            if b.cse:
-                gate_ptr, dpool_ptr = _ptr(rec["gate"]), se_dpool
-                if os.environ.get("DFD_SE_FUSED"):
-                    bwd.append(("dfd_se_bwd_chain", (mid_a, _ptr(y2), bn_mid.scale, bn_mid.shift, se_draw, _ptr(rec["pooled"]),
-                                                     P32(p + ".se.conv_reduce.weight"), P32(p + ".se.conv_reduce.bias"),
-                                                     P32(p + ".se.conv_expand.weight"), P32(p + ".se.conv_expand.bias"),
-                                                     se_de, se_r, se_drp, se_dpool, N, ho * wo, b.cmid, b.cse, dt)))
-                    bwd.append(("dfd_se_fc_wgrad", (se_de, se_r, se_drp, _ptr(rec["pooled"]),
-                                                    G32(p + ".se.conv_reduce.weight"), G32(p + ".se.conv_reduce.bias"),
-                                                    G32(p + ".se.conv_expand.weight"), G32(p + ".se.conv_expand.bias"),
-                                                    N, b.cmid, b.cse)))
-                else:
-                    bwd.append(("dfd_se_bwd_reduce", (mid_a, _ptr(y2), bn_mid.scale, bn_mid.shift, se_draw, N, ho * wo, b.cmid, dt)))
-                    bwd.append(("dfd_se_fc_bwd", (se_draw, _ptr(rec["pooled"]), P32(p + ".se.conv_reduce.weight"),
-                                                  P32(p + ".se.conv_reduce.bias"), P32(p + ".se.conv_expand.weight"),
-                                                  P32(p + ".se.conv_expand.bias"), se_de, se_r, se_drp, se_dpool,
-                                                  G32(p + ".se.conv_reduce.weight"), G32(p + ".se.conv_reduce.bias"),
-                                                  G32(p + ".se.conv_expand.weight"), G32(p + ".se.conv_expand.bias"),
-                                                  N, b.cmid, b.cse)))
-            bwd.append(("dfd_act_bwd", (mid_a, _ptr(y2), bn_mid.scale, bn_mid.shift, bn_mid.mean, bn_mid.rstd, gate_ptr,
-                                        dpool_ptr, mid_b, N, ho * wo, b.cmid, ACT_SWISH, dt, bn_mid.bs1, bn_mid.bs2, BF(bn_mid))))
-            bwd.append(bwd_finalize(bn_mid, M2))
-            if b.kind == "ir":
-                y1 = rec["y1"]
-                if os.environ.get("DFD_DW_SPLIT_BWD"):      # diagnostics: the two-pass form (same results)
-                    bwd.append(("dfd_dwconv_dgrad", (mid_b, _ptr(y2), bn_mid.cA, bn_mid.cB, bn_mid.cC, P32(p + ".conv_dw.weight"),
-                                                     _ptr(y1), dw_bn.scale, dw_bn.shift, dw_bn.mean, dw_bn.rstd, None, mid_a,
-                                                     N, h, w, b.cmid, b.k, b.stride, 1, dt, dw_bn.bs1, dw_bn.bs2)))
-                    bwd.append(("dfd_dwconv_wgrad", (_ptr(y1), dw_bn.scale, dw_bn.shift, mid_b, _ptr(y2), bn_mid.cA, bn_mid.cB,
-                                                     bn_mid.cC, G32(p + ".conv_dw.weight"), N, h, w, b.cmid, b.k, b.stride, dt)))
-                else:
-                    # input gradient (through bn1 + Swish) and weight gradient in one pass over the dy tile
-                    dw_pad = rec["dw_pad"]
-                    bwd.append(self._dw_bwd((mid_b, _ptr(y2), bn_mid.cA, bn_mid.cB, bn_mid.cC, P32(p + ".conv_dw.weight"),
-                                             _ptr(y1), dw_bn.scale, dw_bn.shift, dw_bn.mean, dw_bn.rstd, None, mid_a,
-                                             G32(p + ".conv_dw.weight"), N, h, w, b.cmid, b.k, b.stride) + dw_pad +
-                                            (dt, dw_bn.bs1, dw_bn.bs2), N, h, w, b.cmid, b.k, b.stride, BF(dw_bn),
-                                            name="dfd_dwconv_bwd" + ("_pad" if dw_pad else "")))
-                bwd.append(bwd_finalize(dw_bn, M1))
-                bwd.append(("dfd_bn_bwd_apply", (mid_a, _ptr(y1), None, dw_bn.cA, dw_bn.cB, dw_bn.cC, mid_b, N, h * w, b.cmid, dt)))
-                bwd.append(gemm(mid_b, T16(p + ".conv_pw.weight"), t2, M1, b.cin, b.cmid))
-                if b.has_residual:
-                    bwd.append(("dfd_add_inplace", (t2, dout, M1 * b.cin, dt)))
-                bwd.append(self._wgrad(mid_b, _ptr(xin), G32(p + ".conv_pw.weight"), M1, b.cmid, b.cin))
-            elif os.environ.get("DFD_DW_SPLIT_BWD"):
-                bwd.append(("dfd_dwconv_dgrad", (mid_b, _ptr(y2), bn_mid.cA, bn_mid.cB, bn_mid.cC, P32(p + ".conv_dw.weight"),
-                                                 None, None, None, None, None, dout if b.has_residual else None, t2,
-                                                 N, h, w, b.cmid, b.k, b.stride, 0, dt, None, None)))
-                bwd.append(("dfd_dwconv_wgrad", (_ptr(xin), None, None, mid_b, _ptr(y2), bn_mid.cA, bn_mid.cB, bn_mid.cC,
-                                                 G32(p + ".conv_dw.weight"), N, h, w, b.cmid, b.k, b.stride, dt)))
-            else:
-                # DS block: the depthwise conv reads the block input as is (mode 0 of the fused pass); stride 1 in every
-                # EfficientNet, so its padding is symmetric under TF "SAME" too
-                assert not rec["dw_pad"], p
-                bwd.append(self._dw_bwd((mid_b, _ptr(y2), bn_mid.cA, bn_mid.cB, bn_mid.cC, P32(p + ".conv_dw.weight"),
-                                         _ptr(xin), None, None, None, None, dout if b.has_residual else None, t2,
-                                         G32(p + ".conv_dw.weight"), N, h, w, b.cmid, b.k, b.stride, dt, None, None),
-                                        N, h, w, b.cmid, b.k, b.stride))
-            self._flush_reduce(bwd)
-            cur = (cur + 2) % 3
-        # stem
-        bn = self.bns["bn1"]
-        bwd.append(("dfd_act_bwd", (sm[cur], _ptr(y0), bn.scale, bn.shift, bn.mean, bn.rstd, None, None, mid_a, N, Hs * Ws,
-                                    spec.stem, ACT_SWISH, dt, bn.bs1, bn.bs2, BF(bn))))
-        bwd.append(bwd_finalize(bn, N * Hs * Ws))
-        if self.stem_impl == "gemm":
-            bwd.append(("dfd_bn_bwd_apply", (mid_a, _ptr(y0), None, bn.cA, bn.cB, bn.cC, mid_b, N, Hs * Ws, spec.stem, dt)))
-            bwd.append(("dfd_memset_async", (_ptr(self.stem_gpad), 0, spec.stem * Kp * 4)))
-            bwd.append(self._wgrad(mid_b, _ptr(self.stem_cols), _ptr(self.stem_gpad), N * Hs * Ws, spec.stem, Kp))
-            self._flush_reduce(bwd)          # the padded gradient must be complete before it is un-padded into the arena
-            bwd.append(("dfd_unpad_grad", (_ptr(self.stem_gpad), G32("conv_stem.weight"), spec.stem, taps, Kp)))
-        else:
-            bwd.append(("dfd_stem_wgrad", (_ptr(self.x_in), mid_a, _ptr(y0), bn.cA, bn.cB, bn.cC, G32("conv_stem.weight"), N,
-                                           spec.in_chans, self.H, self.W, spec.stem, 3, 2, 1, dt)))
-        bwd = self._patch_workspace([op for op in bwd if op is not None])
+    def _finish_plan(self, fwd, bwd):
+        """resolve the workspace, upload the finalisation descriptors, check every op against the ABI table and publish the
+        plan as fwd_ops / bwd_ops: (function, name, args)"""
+        bwd = self._patch_workspace(bwd)
         self._upload_fin_descs()
-
-        def base_name(n):
-            for suf in ("_train", "_evalonly", "_sync"):
-                if n.endswith(suf):
-                    return n[:-len(suf)]
-            return n
-
-        for n, a in fwd + bwd:      # arity / type check of the plan against the ABI table
+        for n, a in fwd + bwd:
             if n.startswith("ALLREDUCE"):
                 continue
             codes = _lib.SIGNATURES[base_name(n)]
@@ -823,15 +536,13 @@ class Engine:
                 if isinstance(v, tuple) and v[0] == "TRAIN_ONLY":
                     v = v[1]
                 ok = (v is None or isinstance(v, int)) if c == "p" else (
-                    isinstance(v, int) if c in "il" else (isinstance(v, (int, float)) or v == "TRAINING"))
+                    isinstance(v, int) if c in "il" else isinstance(v, (int, float)))
                 if not (ok or v == "TRAINING"):
                     raise AssertionError("%s: argument %r does not fit code %r" % (n, v, c))
-        # `<name>_train` ops run in training mode only (mask generation, dropout); ("TRAIN_ONLY", ptr) operands are NULL in eval
-        fwd = [(n, a) for n, a in fwd]
-        self.fwd_ops = [(None if n.startswith("ALLREDUCE") else getattr(L, base_name(n)), n, a) for n, a in fwd]
-        self.bwd_ops = [(None if n.startswith("ALLREDUCE") else getattr(L, n), n, tuple(a)) for n, a in bwd]
-        self.n_launch["fwd"] = len(fwd)
-        self.n_launch["bwd"] = len(bwd)
+        fn = lambda n: None if n.startswith("ALLREDUCE") else getattr(self.L, base_name(n))
+        self.fwd_ops = [(fn(n), n, a) for n, a in fwd]
+        self.bwd_ops = [(fn(n), n, tuple(a)) for n, a in bwd]
+        self.n_launch["fwd"], self.n_launch["bwd"] = len(fwd), len(bwd)
 
     # ------------------------------------------------------------------------------------------
     # execution
@@ -855,12 +566,8 @@ class Engine:
         elif name.endswith("_train"):
             if not training:
                 return None
-        elif name in ("dfd_bn_act", "dfd_bn_act_drop") and any(isinstance(a, tuple) for a in args):
+        elif any(isinstance(a, tuple) for a in args):
             args = tuple((a[1] if training else None) if isinstance(a, tuple) else a for a in args)
-        elif not training and name in ("dfd_gemm_tn", "dfd_gemm_tn_rowpack", "dfd_dwconv_fwd", "dfd_dwconv_fwd_pad"):
-            args = tuple(args[:-3]) + (None, None, None)      # eval: no batch statistics, no finalisation
-        elif not training and name in ("dfd_gemm_tn_mma", "dfd_stem_fwd"):
-            args = tuple(args[:-2]) + (None, None)
         return args
 
     def _run(self, ops, stream, training=None, skip_finalize=False):

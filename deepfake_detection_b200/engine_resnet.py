@@ -17,6 +17,7 @@ strided 3x3 is four parity-class implicit GEMMs (`dfd_conv_dgrad_s2_tc`) storing
 import os
 import struct
 from collections import OrderedDict
+from functools import partial
 
 import torch
 
@@ -60,7 +61,6 @@ def build_resnet(e):
     e._keep = []
     e.acts = {}
     fwd, bwd = [], []
-    mom, eps = e.bn_momentum, e.bn_eps
 
     # ---- packed (kh, kw, ci) copies of the k x k weights -------------------------------------------------
     pk_off, off = {}, 0
@@ -117,15 +117,10 @@ def build_resnet(e):
     e._alloc_bn(bn_specs)
     bns = e.bns
 
-    fused_fin = os.environ.get("DFD_FUSED_FINALIZE", "") not in ("", "0", "gemm")   # off by default, see engine.py
-
-    def gemm(A, B, C, M, Nn, K, bn=None):
-        fs, fq = (bn.fsum, bn.fsq) if bn is not None else (None, None)
-        if e.gemm_impl == "tc":
-            if bn is not None:
-                bn.fused = fused_fin
-            return ("dfd_gemm_tn", (A, B, C, M, Nn, K, dt, fs, fq, bn.fin if (bn is not None and fused_fin) else None))
-        return ("dfd_gemm_tn_mma", (A, B, C, None, M, Nn, K, dt, fs, fq))
+    fused_fin = e._fused_fin
+    # no row-packed GEMMs: every ResNet K is >= 64 except the stem's Kp = 56 at in_chans = 1, which keeps the plain GEMM
+    gemm = partial(e._gemm, fuse=fused_fin, rowpack=False)
+    finalize, bwd_finalize, BF = e._finalize, e._bwd_finalize, e._bfin
 
     implicit = e.gemm_impl == "tc" and not os.environ.get("DFD_NO_IMPLICIT_CONV")
     implicit_wgrad = not os.environ.get("DFD_NO_IMPLICIT_WGRAD")
@@ -135,29 +130,11 @@ def build_resnet(e):
     def conv3x3(xin, name, y, h, w, cin, cout, stride, bn):
         """3x3 / padding 1 forward into y (+ BatchNorm statistics of y)"""
         if implicit and (stride == 1 or implicit_s2) and cin % 64 == 0 and cout % 64 == 0:
-            bn.fused = fused_fin
             e.n_implicit += 1
-            return [("dfd_conv_tc", (xin, PK(name), y, N, h, w, cin, cout, 3, stride, dt, bn.fsum, bn.fsq,
-                                     bn.fin if fused_fin else None))]
+            return [("dfd_conv_tc", (xin, PK(name), y, N, h, w, cin, cout, 3, stride, dt) + e._stats(bn, fused_fin))]
         ho, wo = conv_out(h, 3, stride, 1), conv_out(w, 3, stride, 1)
         return [("dfd_im2col", (xin, COLS, N, h, w, cin, 3, stride, 1, dt)),
                 gemm(COLS, PK(name), y, N * ho * wo, cout, 9 * cin, bn)]
-
-    def finalize(bn, count):
-        # training: finalised by the last CTA of the producing GEMM (bn.fin); this op runs in eval mode only (see Engine._run)
-        bn.count = count
-        return ("dfd_bn_finalize" + ("_evalonly" if bn.fused else ""),
-                [bn.fsum, bn.fsq, float(count), bn.gamma, bn.beta, bn.rm, bn.rv, bn.nbt, mom, eps,
-                 "TRAINING", bn.C, bn.scale, bn.shift, bn.mean, bn.rstd])
-
-    def bwd_finalize(bn, count):
-        bn.count = count
-        if fused_fin:
-            return None             # the last CTA of dfd_act_bwd / dfd_bn_bwd_reduce does it (bn.bfin)
-        return ("dfd_bn_bwd_finalize", (bn.bs1, bn.bs2, float(count), bn.gamma, bn.mean, bn.rstd, bn.dgamma, bn.dbeta,
-                                        bn.cA, bn.cB, bn.cC, bn.C))
-
-    BF = (lambda bn: bn.bfin) if fused_fin else (lambda bn: None)
 
     # ---- stochastic regularisation (training only): DropBlock sites, drop-path gates, classifier dropout ---------------
     relu_fuse = not (fused_fin or os.environ.get("DFD_NO_RELU_FUSE"))
@@ -230,9 +207,9 @@ def build_resnet(e):
         fwd.append(("dfd_stem_im2col", (_ptr(e.x_in), _ptr(e.stem_cols), N, spec.in_chans, e.H, e.W, 7, 2, 3, Kp, dt)))
         fwd.append(gemm(_ptr(e.stem_cols), _ptr(e.stem_wpad), _ptr(y0), N * H1 * W1, 64, Kp, bn0))
     else:
-        fwd.append(("dfd_stem_fwd", (_ptr(e.x_in), P32("conv1.weight"), _ptr(y0), N, spec.in_chans, e.H, e.W, 64, 7, 2, 3, dt,
-                                     bn0.fsum, bn0.fsq)))
-    fwd.append(finalize(bn0, N * H1 * W1))
+        fwd.append(("dfd_stem_fwd", (_ptr(e.x_in), P32("conv1.weight"), _ptr(y0), N, spec.in_chans, e.H, e.W, 64, 7, 2, 3, dt)
+                    + e._stats(bn0)[:2]))
+    fwd += finalize(bn0, N * H1 * W1)
     fwd.append(bn_relu(y0, bn0, a0, H1 * W1, 64))
     fwd.append(("dfd_maxpool_fwd", (_ptr(a0), _ptr(x0), _ptr(e.pool_idx), N, H1, W1, 64, dt)))
     e.acts["stem.out"] = x0
@@ -248,10 +225,10 @@ def build_resnet(e):
             a1 = e._alloc16(N, ho, wo, b.planes)
             y2 = e._alloc16(N, ho, wo, b.cout)
             fwd += conv3x3(_ptr(x), p + ".conv1.weight", _ptr(y1), h, w, b.cin, b.planes, b.stride, bn1)
-            fwd.append(finalize(bn1, M2))
+            fwd += finalize(bn1, M2)
             fwd.append(bn_relu(y1, bn1, a1, ho * wo, b.planes, p + ".bn1"))
             fwd += conv3x3(_ptr(a1), p + ".conv2.weight", _ptr(y2), ho, wo, b.planes, b.cout, 1, bn2)
-            fwd.append(finalize(bn2, M2))
+            fwd += finalize(bn2, M2)
             rec.update(y1=y1, a1=a1, ylast=y2, bnlast=bn2, site_last=p + ".bn2")
         else:
             bn1, bn2, bn3 = bns[p + ".bn1"], bns[p + ".bn2"], bns[p + ".bn3"]
@@ -261,13 +238,13 @@ def build_resnet(e):
             a2 = e._alloc16(N, ho, wo, b.planes)
             y3 = e._alloc16(N, ho, wo, b.cout)
             fwd.append(gemm(_ptr(x), P16(p + ".conv1.weight"), _ptr(y1), M1, b.planes, b.cin, bn1))
-            fwd.append(finalize(bn1, M1))
+            fwd += finalize(bn1, M1)
             fwd.append(bn_relu(y1, bn1, a1, h * w, b.planes, p + ".bn1"))
             fwd += conv3x3(_ptr(a1), p + ".conv2.weight", _ptr(y2), h, w, b.planes, b.planes, b.stride, bn2)
-            fwd.append(finalize(bn2, M2))
+            fwd += finalize(bn2, M2)
             fwd.append(bn_relu(y2, bn2, a2, ho * wo, b.planes, p + ".bn2"))
             fwd.append(gemm(_ptr(a2), P16(p + ".conv3.weight"), _ptr(y3), M2, b.cout, b.planes, bn3))
-            fwd.append(finalize(bn3, M2))
+            fwd += finalize(bn3, M2)
             rec.update(y1=y1, a1=a1, y2=y2, a2=a2, ylast=y3, bnlast=bn3, site_last=p + ".bn3")
         res = x
         if b.downsample:
@@ -282,14 +259,13 @@ def build_resnet(e):
             elif ds_implicit:
                 # strided 1x1 convolution straight from the block input (k = 1, stride 2 implicit GEMM): no gathered copy
                 xs = None
-                bnd.fused = fused_fin
-                fwd.append(("dfd_conv_tc", (_ptr(x), P16(p + ".downsample.0.weight"), _ptr(yd), N, h, w, b.cin, b.cout, 1, b.stride, dt,
-                                            bnd.fsum, bnd.fsq, bnd.fin if fused_fin else None)))
+                fwd.append(("dfd_conv_tc", (_ptr(x), P16(p + ".downsample.0.weight"), _ptr(yd), N, h, w, b.cin, b.cout, 1, b.stride, dt)
+                            + e._stats(bnd, fused_fin)))
             else:
                 xs = e._alloc16(N, ho, wo, b.cin)
                 fwd.append(("dfd_im2col", (_ptr(x), _ptr(xs), N, h, w, b.cin, 1, b.stride, 0, dt)))
                 fwd.append(gemm(_ptr(xs), P16(p + ".downsample.0.weight"), _ptr(yd), M2, b.cout, b.cin, bnd))
-            fwd.append(finalize(bnd, M2))
+            fwd += finalize(bnd, M2)
             fwd.append(("dfd_bn_act", (_ptr(yd), bnd.scale, bnd.shift, None, None, _ptr(r), N, ho * wo, b.cout, ACT_NONE, 0, dt)))
             rec.update(yd=yd, xs=xs, bnd=bnd)
             res = r
@@ -327,18 +303,7 @@ def build_resnet(e):
         e.dropout_mask = torch.ones(N, P, dtype=torch.float32, device=dev)
         masks.append((e.dropout_mask, N * P, 1, 1.0 - e.drop_rate))
         fwd.append(("dfd_mul_f32_train", (_ptr(e.pooled), _ptr(e.dropout_mask), N * P)))
-    # the step's masks are drawn at the head of the training forward, then the generator's step advances on the device
-    head = []
-    if sites:
-        head.append(("dfd_memset_async_train", (_ptr(e.drop_block_kept), 0, 8 * len(sites))))
-        head.append(("dfd_drop_block_masks_train", (_ptr(e._drop_block_table), len(sites), _ptr(e.rng_state))))
-    if masks:
-        raw = b"".join(struct.pack("<Qqifii", _ptr(t), rows, width, keep, si, 0) for si, (t, rows, width, keep) in enumerate(masks))
-        e._mask_table = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(dev)
-        head.append(("dfd_rng_masks_train", (_ptr(e._mask_table), len(masks), _ptr(e.rng_state))))
-    if head:
-        head.append(("dfd_rng_tick_train", (_ptr(e.rng_state),)))
-    fwd = head + fwd
+    fwd = e._mask_head(masks, len(sites)) + fwd
     e.logits = torch.zeros(N, K, dtype=torch.float32, device=dev)
     e.dlogits = torch.zeros(N, K, dtype=torch.float32, device=dev)
     e.dpooled = torch.zeros(N, P, dtype=torch.float32, device=dev)
@@ -379,7 +344,7 @@ def build_resnet(e):
             ops += [("dfd_im2col", (_ptr(xin_t), COLS, N, n_h, n_w, Cin, 3, stride, 1, dt)),
                     zero_gperm(gp, Cout * 9 * Cin),
                     e._wgrad(dy, COLS, gp, M_out, Cout, 9 * Cin)]
-        if os.environ.get("DFD_NONDET"):
+        if e._nondet:
             ops.append(("dfd_unpack_grad", (gp, G32(name), Cout, Cin, 3)))       # atomics: complete when the kernel is
         else:
             pending_unpack.append((gp, name, Cout, Cin))     # complete after the block's ordered reduce (flush_block)
@@ -428,14 +393,14 @@ def build_resnet(e):
             bwd.append(("dfd_relu_bn_bwd_reduce", (dout, dout2, _ptr(rec["ylast"]), _ptr(rec["out"]), gm, bl.mean, bl.rstd, N, ho * wo,
                                                    b.cout, dt, bl.bs1, bl.bs2)))
         gd = t2 if (rec["site_last"] in sites or rec["gate"] is not None) else gm
-        bwd.append(bwd_finalize(bl, M2))
+        bwd += bwd_finalize(bl, M2)
         bwd.append(("dfd_bn_bwd_apply", (gd, _ptr(rec["ylast"]), None, bl.cA, bl.cB, bl.cC, t1, N, ho * wo, b.cout, dt)))
         if b.kind == "basic":
             bn1 = bns[p + ".bn1"]
             # conv2 (3x3 s1): dy2 = t1 -> da1 = t2
             bwd += conv3x3_bwd(p + ".conv2.weight", t1, M2, b.planes, b.cout, rec["a1"], ho, wo, 1, t2)
             bwd.append(relu_bwd(t2, rec["y1"], bn1, t1, ho * wo, b.planes, p + ".bn1"))
-            bwd.append(bwd_finalize(bn1, M2))
+            bwd += bwd_finalize(bn1, M2)
             bwd.append(("dfd_bn_bwd_apply", (t1, _ptr(rec["y1"]), None, bn1.cA, bn1.cB, bn1.cC, t2, N, ho * wo, b.planes, dt)))
             # conv1 (3x3 stride s): dy1 = t2 -> dx = t3 [M1, cin]
             bwd += conv3x3_bwd(p + ".conv1.weight", t2, M2, b.cin, b.planes, xin, h, w, b.stride, t3)
@@ -445,12 +410,12 @@ def build_resnet(e):
             bwd.append(gemm(t1, T16(p + ".conv3.weight"), t2, M2, b.planes, b.cout))
             bwd.append(e._wgrad(t1, _ptr(rec["a2"]), G32(p + ".conv3.weight"), M2, b.cout, b.planes))
             bwd.append(relu_bwd(t2, rec["y2"], bn2, t1, ho * wo, b.planes, p + ".bn2"))
-            bwd.append(bwd_finalize(bn2, M2))
+            bwd += bwd_finalize(bn2, M2)
             bwd.append(("dfd_bn_bwd_apply", (t1, _ptr(rec["y2"]), None, bn2.cA, bn2.cB, bn2.cC, t2, N, ho * wo, b.planes, dt)))
             # conv2 (3x3 stride s): dy2 = t2 -> da1 = t1 [M1, planes]
             bwd += conv3x3_bwd(p + ".conv2.weight", t2, M2, b.planes, b.planes, rec["a1"], h, w, b.stride, t1)
             bwd.append(relu_bwd(t1, rec["y1"], bn1, t2, h * w, b.planes, p + ".bn1"))
-            bwd.append(bwd_finalize(bn1, M1))
+            bwd += bwd_finalize(bn1, M1)
             bwd.append(("dfd_bn_bwd_apply", (t2, _ptr(rec["y1"]), None, bn1.cA, bn1.cB, bn1.cC, t1, N, h * w, b.planes, dt)))
             # conv1 (1x1): dy1 = t1 -> dx = t3 [M1, cin]
             bwd.append(gemm(t1, T16(p + ".conv1.weight"), t3, M1, b.cin, b.planes))
@@ -459,7 +424,7 @@ def build_resnet(e):
         if b.downsample:
             bnd = rec["bnd"]
             bwd.append(("dfd_bn_bwd_reduce", (gm, _ptr(rec["yd"]), None, bnd.mean, bnd.rstd, N, ho * wo, b.cout, dt, bnd.bs1, bnd.bs2, BF(bnd))))
-            bwd.append(bwd_finalize(bnd, M2))
+            bwd += bwd_finalize(bnd, M2)
             bwd.append(("dfd_bn_bwd_apply", (gm, _ptr(rec["yd"]), None, bnd.cA, bnd.cB, bnd.cC, t1, N, ho * wo, b.cout, dt)))
             ds_add = (implicit and implicit_s2 and b.cin % 64 == 0 and b.cout % 64 == 0 and
                       not os.environ.get("DFD_NO_DGRAD_ADD"))
@@ -497,7 +462,7 @@ def build_resnet(e):
     bwd.append(("dfd_maxpool_bwd", (dout, _ptr(e.pool_idx), t1, N, H1, W1, 64, dt)))
     bwd.append(("dfd_act_bwd", (t1, _ptr(y0), bn0.scale, bn0.shift, bn0.mean, bn0.rstd, None, None, t2, N, H1 * W1, 64,
                                 ACT_RELU, dt, bn0.bs1, bn0.bs2, BF(bn0))))
-    bwd.append(bwd_finalize(bn0, N * H1 * W1))
+    bwd += bwd_finalize(bn0, N * H1 * W1)
     if e.stem_impl == "gemm":
         bwd.append(("dfd_bn_bwd_apply", (t2, _ptr(y0), None, bn0.cA, bn0.cB, bn0.cC, t1, N, H1 * W1, 64, dt)))
         bwd.append(("dfd_memset_async", (_ptr(e.stem_gpad), 0, 64 * Kp * 4)))
@@ -507,21 +472,4 @@ def build_resnet(e):
     else:
         bwd.append(("dfd_stem_wgrad", (_ptr(e.x_in), t2, _ptr(y0), bn0.cA, bn0.cB, bn0.cC, G32("conv1.weight"), N, spec.in_chans,
                                        e.H, e.W, 64, 7, 2, 3, dt)))
-
-    bwd = e._patch_workspace([op for op in bwd if op is not None])
-    e._upload_fin_descs()
-
-    def base_name(n):
-        for suf in ("_evalonly", "_train"):
-            if n.endswith(suf):
-                return n[:-len(suf)]
-        return n
-
-    for n, a in fwd + bwd:
-        codes = _lib.SIGNATURES[base_name(n)]
-        if len(a) != len(codes) - 1:
-            raise AssertionError("%s: %d args for signature %r" % (n, len(a), codes))
-    L = e.L
-    e.fwd_ops = [(getattr(L, base_name(n)), n, a) for n, a in fwd]
-    e.bwd_ops = [(getattr(L, n), n, tuple(a)) for n, a in bwd]
-    e.n_launch["fwd"], e.n_launch["bwd"] = len(fwd), len(bwd)
+    e._finish_plan(fwd, bwd)

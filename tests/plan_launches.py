@@ -13,6 +13,7 @@ import functools
 from collections import OrderedDict, namedtuple
 
 from deepfake_detection_b200 import _lib
+from deepfake_detection_b200.engine import base_name
 
 # (tag, arch, batch, resolution, dtype, extra Engine kwargs): BASELINE configs 2/3 (B0; the per-GPU batch of the DDP config is
 # also 256), config 5 (B4 fp16), config 4 (ResNet-50), ResNet-18, and the production model of test_production_model_gpu.py
@@ -25,15 +26,6 @@ CONFIGS = [
 ]
 
 Launch = namedtuple("Launch", "kernel shape ptrs")
-
-_SUFFIXES = ("_train", "_evalonly", "_sync")
-
-
-def base_name(name):
-    for suf in _SUFFIXES:
-        if name.endswith(suf):
-            return name[:-len(suf)]
-    return name
 
 
 def _split(name, args):

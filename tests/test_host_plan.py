@@ -109,3 +109,52 @@ def test_plan_uses_the_fused_and_packed_kernels():
     assert ar.params_only and ar.fwd_ops == [] and not hasattr(ar, "acts") and ar.n_params == eng.n_params
     eng3 = Engine("efficientnet_b0", 2, 64, 64, device="plan-only", share_from=ar)
     assert eng3.arena is ar and eng3.grads32 is ar.grads32 and len(ar._bd_reg) > 0 and len(ar._stem_reg) == 1
+
+
+def test_resnet_plan_validation_checks_argument_types(monkeypatch):
+    """a ResNet plan is held to the ABI table's argument codes, not only to its argument counts"""
+    from deepfake_detection_b200.engine import Engine
+    _lib.lib()              # bind the library with the real table first: the patched one must only reach the plan check
+    codes = _lib.SIGNATURES["dfd_bn_finalize"]
+    monkeypatch.setitem(_lib.SIGNATURES, "dfd_bn_finalize", codes[:2] + "l" + codes[3:])   # the float count no longer fits
+    with pytest.raises(AssertionError, match="does not fit code 'l'"):
+        Engine("resnet18", 2, 64, 64, device="plan-only")
+
+
+@pytest.mark.parametrize("fused_finalize", ["", "1"])
+def test_resnet_eval_forward_passes_no_statistics_to_the_implicit_conv(monkeypatch, fused_finalize):
+    """dfd_conv_tc writes batch statistics (and, with DFD_FUSED_FINALIZE=1, finalises them) in training only: an eval forward
+    passes NULL for the statistics and the descriptor, so it neither accumulates them nor moves the running statistics"""
+    from deepfake_detection_b200.engine import Engine
+    monkeypatch.setenv("DFD_FUSED_FINALIZE", fused_finalize)
+    eng = Engine("resnet50", 2, 160, 160, device="plan-only")
+    convs = [a for _, n, a in eng.fwd_ops if n == "dfd_conv_tc"]
+    assert len(convs) == 16 + 3          # every 3x3 convolution and the three strided 1x1 downsamples
+    for a in convs:
+        train, ev = eng.launch_args("dfd_conv_tc", a, True), eng.launch_args("dfd_conv_tc", a, False)
+        assert ev[:-3] == train[:-3] and ev[-3:] == (None, None, None)
+        assert train[-3] and train[-2] and bool(train[-1]) == (fused_finalize == "1")
+
+
+def test_resnet_refuses_sync_bn_over_several_ranks(monkeypatch):
+    """the ResNet plan has no synchronised BatchNorm: over more than one rank it refuses, instead of running rank-local
+    statistics; on one rank sync_bn is plain BatchNorm, as in torch"""
+    import torch.distributed as dist
+    from deepfake_detection_b200.engine import Engine
+    Engine("resnet18", 2, 64, 64, device="plan-only", sync_bn=True)
+    monkeypatch.setattr(dist, "is_available", lambda: True)
+    monkeypatch.setattr(dist, "is_initialized", lambda: True)
+    monkeypatch.setattr(dist, "get_world_size", lambda *a, **k: 2)
+    for kw in (dict(), dict(params_only=True)):
+        with pytest.raises(_lib.NativeError, match="sync_bn over 2 ranks"):
+            Engine("resnet18", 2, 64, 64, device="plan-only", sync_bn=True, **kw)
+    eng = Engine("efficientnet_b0", 2, 64, 64, device="plan-only", sync_bn=True)
+    assert eng.sync_world == 2 and any(n == "dfd_bn_finalize_sync" for _, n, _ in eng.fwd_ops)
+
+
+def test_resnet_stem_gemm_is_never_row_packed():
+    """one input channel gives the ResNet stem GEMM K = 56; the ResNet plan keeps the plain GEMM there"""
+    from deepfake_detection_b200.engine import Engine
+    eng = Engine("resnet18", 2, 64, 64, device="plan-only", in_chans=1)
+    names = [n for _, n, _ in eng.fwd_ops + eng.bwd_ops]
+    assert "dfd_gemm_tn_rowpack" not in names and not getattr(eng, "_bd_reg", None)

@@ -171,7 +171,7 @@ def test_run_issues_what_launch_args_gives(monkeypatch, arch, kw):
     assert not any(isinstance(v, (tuple, str)) for _, a in ev for v in a)
     fin = [a for n, a in ev if n.startswith("dfd_bn_finalize")]
     assert fin and all(a[0] is None and a[1] is None and a[10] == 0 for a in fin)
-    assert all(a[-3:] == (None, None, None) for n, a in ev if n in ("dfd_gemm_tn", "dfd_gemm_tn_rowpack", "dfd_dwconv_fwd"))
+    assert all(a[-3:] == (None, None, None) for n, a in ev if n in ("dfd_gemm_tn", "dfd_gemm_tn_rowpack", "dfd_dwconv_fwd", "dfd_conv_tc"))
     del calls[:]
     eng.forward(training=False, stream=0)
     assert calls == [c for c in ev if not c[0].startswith("dfd_bn_finalize")]

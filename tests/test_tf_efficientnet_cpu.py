@@ -12,7 +12,7 @@ import tf_same_cases as TC
 import tf_same_oracle as TO
 from deepfake_detection_b200 import _lib
 from deepfake_detection_b200.arch import SUPPORTED_ARCHS, TF_ARCHS, conv_pads, get_spec, param_entries, state_entries
-from deepfake_detection_b200.engine import Engine
+from deepfake_detection_b200.engine import Engine, base_name
 from oracle import train as OT
 from oracle.weights import synth_batch, synth_state
 
@@ -168,11 +168,7 @@ def test_plan_only_engines_build_at_default_resolution(arch, in_chans):
 
 def _norm(name, args):
     """a planned launch with every pointer argument reduced to NULL / non-NULL (two engines own different buffers)"""
-    base = name
-    for suf in ("_train", "_evalonly", "_sync"):
-        if base.endswith(suf):
-            base = base[: -len(suf)]
-    codes = _lib.SIGNATURES[base]
+    codes = _lib.SIGNATURES[base_name(name)]
     out = []
     for v, c in zip(args, codes):
         if isinstance(v, tuple) and v[0] == "TRAIN_ONLY":
@@ -213,12 +209,17 @@ def test_tf_plan_at_all_odd_extents_issues_no_new_kernel():
     assert not names & set(TC.NEW_KERNELS)
 
 
-def test_eval_rewrite_drops_the_statistics_of_the_padded_forward():
+def test_padded_forward_marks_its_statistics_training_only():
+    """the padded depthwise forward's batch statistics are training-only operands: NULL in eval mode, their pointers in
+    training, every other argument as planned in both modes"""
     e = Engine("tf_efficientnet_b0", 2, 64, 96, device="plan-only")
     op = next((n, a) for _, n, a in e.fwd_ops if n == "dfd_dwconv_fwd_pad")
     ev = e.launch_args(op[0], op[1], False)
     assert ev[:-3] == tuple(op[1][:-3]) and ev[-3:] == (None, None, None)
-    assert e.launch_args(op[0], op[1], True) == op[1]
+    # training runs the op as planned: only the statistics are marked training-only, and they resolve to their pointers
+    bn = e.bns["blocks.1.0.bn2"]
+    assert op[1][-3:] == (("TRAIN_ONLY", bn.fsum), ("TRAIN_ONLY", bn.fsq), None)
+    assert e.launch_args(op[0], op[1], True) == tuple(op[1][:-3]) + (bn.fsum, bn.fsq, None)
 
 
 def test_gpu_cases_cover_every_new_launch_of_the_default_plans():
