@@ -14,8 +14,6 @@ gradients live in ONE flat fp32 arena laid out in forward execution order, so:
 `NativeDDP` is the object the runner sees: `.module` unwraps, calling it runs the model, and the wrapped model's
 backward (autograd bridge and fused step alike) goes through `GradReducer.backward_and_reduce`.
 """
-import os
-
 import torch
 import torch.distributed as dist
 import torch.nn as nn
@@ -89,7 +87,7 @@ class GradReducer:
         self.arena = engine.arena
         self.group = group
         self.world = dist.get_world_size(group)
-        self.bucket_mb = float(os.environ.get("DFD_DDP_BUCKET_MB", bucket_mb))      # env: diagnostic override
+        self.bucket_mb = float(bucket_mb)
         self.side = None if self.arena._plan_only else torch.cuda.Stream(device=self.arena.device)
         backend = dist.get_backend(group)
         self._avg = backend == "nccl"              # gloo has no AVG: SUM, then scale
@@ -207,10 +205,6 @@ class GradReducer:
         else:
             dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
             t.mul_(1.0 / self.world)
-
-    def reduce_all(self):
-        """one mean all-reduce over the whole gradient arena on the current stream (split-graph mode of the Trainer)"""
-        self._mean(self.arena.grads32)
 
     def backward_and_reduce(self, engine=None):
         """Runs `engine`'s backward plan (the one whose forward just ran) on the current stream, launching each bucket's

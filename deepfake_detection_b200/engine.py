@@ -12,14 +12,13 @@ and lists the ops; the conventions every plan shares (BatchNorm statistics and f
 deterministic weight-gradient reduce, validation against the ABI table) are the plan helpers of this class.
 
 A plan op is (name, args). `base_name(name)` is the C-ABI entry point it calls: `<entry>_train` runs in training mode
-only, `<entry>_evalonly` in eval mode only and `dfd_bn_finalize_sync` finalises the summed statistics of all ranks. In
-args, ("TRAIN_ONLY", ptr) is an operand that is NULL in eval mode, "TRAINING" is the mode flag (1 / 0) and ("WS", off)
-a slot of the deterministic-reduce workspace, resolved when the plan is finished.
+only and `dfd_bn_finalize_sync` finalises the summed statistics of all ranks. In args, ("TRAIN_ONLY", ptr) is an operand
+that is NULL in eval mode, "TRAINING" is the mode flag (1 / 0) and ("WS", off) a slot of the deterministic-reduce
+workspace, resolved when the plan is finished.
 
 PyTorch is used for device memory and streams only; there is no PyTorch compute on the hot path and no CPU
 fallback: constructing an Engine without a CUDA device or without libdfd_b200.so raises.
 """
-import os
 import struct
 from collections import OrderedDict
 
@@ -38,7 +37,7 @@ def _ptr(t, off_elems=0):
 
 def base_name(name):
     """the C-ABI entry point of the plan op `name`"""
-    for suf in ("_train", "_evalonly", "_sync"):
+    for suf in ("_train", "_sync"):
         if name.endswith(suf):
             return name[:-len(suf)]
     return name
@@ -47,7 +46,7 @@ def base_name(name):
 class _BN:
     """Pointers of one BatchNorm layer (parameters, running stats, per-step statistics, bwd coefficients)."""
     __slots__ = ("name", "C", "gamma", "beta", "dgamma", "dbeta", "rm", "rv", "nbt", "scale", "shift", "mean",
-                 "rstd", "cA", "cB", "cC", "fsum", "fsq", "bs1", "bs2", "fin", "bfin", "count", "idx", "fused", "stat_off")
+                 "rstd", "cA", "cB", "cC", "fsum", "fsq", "bs1", "bs2", "stat_off")
 
 
 class Engine:
@@ -90,22 +89,10 @@ class Engine:
         if self.sync_bn and spec.family == "resnet":
             raise _lib.NativeError("sync_bn over %d ranks: the ResNet plan has no synchronised BatchNorm (only the "
                                    "EfficientNet plan all-reduces its batch statistics)" % self.sync_world)
-        # DFD_NONDET=1: weight gradients flushed with atomics instead of the ordered reduce (see _wgrad)
-        self._nondet = bool(os.environ.get("DFD_NONDET"))
-        # BatchNorm finalisation by the last CTA of the statistics-producing kernel (descriptors, csrc/bn_finalize.cuh)
-        # instead of one-block launches: implemented and tested, but off by default: every CTA pays a __threadfence + a
-        # same-address ticket atomic before it may retire (the depthwise kernels run ~14k short CTAs), and the one finalising
-        # CTA walks C channels with a fraction of the threads of the standalone launch. DFD_FUSED_FINALIZE=1: every
-        # producer, forward and backward; =gemm: only the EfficientNet BatchNorms whose statistics come from the persistent
-        # tensor-core GEMM (one CTA per SM: the ticket is free there). Never with synchronised BatchNorm.
-        ff_mode = os.environ.get("DFD_FUSED_FINALIZE", "")
-        self._fused_fin = ff_mode not in ("", "0", "gemm") and not self.sync_bn
-        self._fused_gemm = (self._fused_fin or ff_mode == "gemm") and not self.sync_bn
         self.bn_momentum = float(bn_momentum)
         self.bn_eps = float(bn_eps)
+        # "tc": wgmma GEMMs and implicit convolutions; "mma": the mma.sync cross-check path (GEMMs over im2col columns)
         self.gemm_impl = gemm_impl
-        # 1x1 weight gradient: wgmma with MN-major operands, or the mma.sync cross-check path
-        self._wgrad_name = "dfd_gemm_wgrad" if gemm_impl == "tc" and not os.environ.get("DFD_WGRAD_MMA") else "dfd_gemm_wgrad_mma"
         self.stem_impl = stem_impl
         self.training = True
         self.n_launch = {"fwd": 0, "bwd": 0, "opt": 0}
@@ -264,12 +251,9 @@ class Engine:
     # block of the network, right behind that block's backward ops - adds the partials into the gradient arena in slot
     # order. Gradients (and with them every later step) therefore do not depend on the arrival order of CTAs; the reduce
     # launches are also the points at which a block's gradients become final for the DDP bucketing.
-    # DFD_NONDET=1 switches back to the atomic flushes (diagnostics / timing comparison).
     def _wgrad(self, G, X, dW, M, Nw, Kw):
-        if self._wgrad_name != "dfd_gemm_wgrad":
-            return (self._wgrad_name, (G, X, dW, M, Nw, Kw, self.dt))
-        if self._nondet:
-            return ("dfd_gemm_wgrad", (G, X, dW, M, Nw, Kw, self.dt, None, 0))
+        if self.gemm_impl != "tc":
+            return ("dfd_gemm_wgrad_mma", (G, X, dW, M, Nw, Kw, self.dt))
         splits = self.L.cdll.dfd_gemm_wgrad_splits(M, Nw, Kw)
         off, nbytes = self._ws_take(splits * Nw * Kw * 4)
         self._red_pending.append((off, dW, Nw * Kw, Nw * Kw, splits))
@@ -279,16 +263,12 @@ class Engine:
         """implicit-GEMM weight gradient of a dense k x k convolution (H, W = input extents) into the packed
         [Cout][kh][kw][Cin] fp32 buffer"""
         Kw = k * k * Cin
-        if self._nondet:
-            return ("dfd_conv_wgrad_tc", (dY, X, dW, N, H, W, Cin, Cout, k, stride, self.dt, None, 0))
         splits = self.L.cdll.dfd_conv_wgrad_splits(N, H, W, Cin, Cout, k, stride)
         off, nbytes = self._ws_take(splits * Cout * Kw * 4)
         self._red_pending.append((off, dW, Cout * Kw, Cout * Kw, splits))
         return ("dfd_conv_wgrad_tc", [dY, X, dW, N, H, W, Cin, Cout, k, stride, self.dt, ("WS", off), nbytes])
 
-    def _dw_bwd(self, args, N, H, W, C, k, stride, fin=None, name="dfd_dwconv_bwd"):
-        if self._nondet:
-            return (name, list(args) + [None, 0, fin])
+    def _dw_bwd(self, args, N, H, W, C, k, stride, name="dfd_dwconv_bwd"):
         parts = self.L.cdll.dfd_dwconv_bwd_parts(N, H, W, C, k, stride)
         cw = self.L.cdll.dfd_dwconv_block_channels(C)          # channels per CTA: 64, or 32 / 16 for C = 32, 96 / 144
         cbs = (C + cw - 1) // cw
@@ -297,7 +277,7 @@ class Engine:
         for cb in range(cbs):
             n = min(cw, C - cw * cb) * k * k
             self._red_pending.append((off + cb * parts * cw * k * k * 4, dW + cb * cw * k * k * 4, n, cw * k * k, parts))
-        return (name, list(args) + [("WS", off), nbytes, fin])
+        return (name, list(args) + [("WS", off), nbytes, None])
 
     def _ws_take(self, nbytes):
         off = getattr(self, "_ws_bytes", 0)
@@ -346,8 +326,6 @@ class Engine:
     @classmethod
     def _row_pack(cls, M, K):
         """rows of A read as one (dfd_gemm_tn_rowpack): keeps the TMA rows of small-K pointwise convs at >= 128 bytes"""
-        if os.environ.get("DFD_NO_ROWPACK"):
-            return 1
         pack = cls._ROW_PACK.get(K, 1)
         while pack > 1 and M % pack:
             pack //= 2
@@ -356,22 +334,6 @@ class Engine:
     # Derived 16-bit weight layouts (block-diagonal small-K copies, the padded stem weight, the packed k x k weights of
     # the ResNet path) are registered with, owned by and refreshed through the ARENA engine, whichever plan asked for them:
     # the optimizer refreshes them once per step for every plan that shares the weights.
-    def _upload_fin_descs(self):
-        """fill the BatchNorm finalisation descriptors once the plan knows every layer's element count"""
-        n = len(self.bns)
-        raw = bytearray(2 * n * 128)
-        for bn in self.bns.values():
-            if bn.count is None:
-                continue
-            cnt = float(bn.count)
-            unb = cnt / (cnt - 1.0) if cnt > 1 else 1.0
-            struct.pack_into("<12Qddffii", raw, bn.idx * 128, bn.fsum, bn.fsq, bn.gamma, bn.beta, bn.rm, bn.rv, bn.nbt, bn.scale,
-                             bn.shift, bn.mean, bn.rstd, _ptr(self._fin_tickets, bn.idx), 1.0 / cnt, unb, self.bn_momentum,
-                             self.bn_eps, bn.C, 0)
-            struct.pack_into("<11Qdii", raw, (n + bn.idx) * 128, bn.bs1, bn.bs2, bn.gamma, bn.mean, bn.rstd, bn.dgamma, bn.dbeta,
-                             bn.cA, bn.cB, bn.cC, _ptr(self._fin_tickets, n + bn.idx), 1.0 / cnt, bn.C, 0)
-        self._fin_buf.copy_(torch.frombuffer(raw, dtype=torch.int32).to(self._fin_buf.device))
-
     def _blockdiag(self, B, Nn, K, pack):
         """block-diagonal [pack*Nn, pack*K] copy of the weight at B"""
         o = self.arena
@@ -424,16 +386,9 @@ class Engine:
         self.stats = torch.zeros(4 * S * tot_c + 8, dtype=torch.float64, device=dev)  # fsum fsq bs1 bs2 (+ loss/correct)
         self.bns = {}
         co = 0
-        # finalisation descriptors (csrc/bn_finalize.cuh: BnFinDesc / BnBwdFinDesc, 128-byte stride) + one ticket each: the
-        # last CTA of the kernel that produced a layer's statistics finalises that BatchNorm (no one-block launches)
-        self._fin_buf = torch.zeros(2 * len(bn_specs) * 32, dtype=torch.int32, device=dev)
-        self._fin_tickets = torch.zeros(2 * len(bn_specs), dtype=torch.int32, device=dev)
-        for bi, (name, c) in enumerate(bn_specs):
+        for name, c in bn_specs:
             bn = _BN()
             bn.name, bn.C = name, c
-            bn.idx, bn.count, bn.fused = bi, None, False
-            bn.fin = _ptr(self._fin_buf, bi * 32)
-            bn.bfin = _ptr(self._fin_buf, (len(bn_specs) + bi) * 32)
             bn.gamma = _ptr(self.params32, self.p_off[name + ".weight"][0])
             bn.beta = _ptr(self.params32, self.p_off[name + ".bias"][0])
             bn.dgamma = _ptr(self.grads32, self.p_off[name + ".weight"][0])
@@ -459,51 +414,44 @@ class Engine:
         (build_resnet if self.spec.family == "resnet" else build_efficientnet)(self)
 
     # ---- plan helpers shared by the family builders ---------------------------------------------------------------------
-    def _stats(self, bn, fuse=False):
-        """a forward producer's (sum, sum of squares, finalisation descriptor) operands for `bn`, all training-only (NULL in
-        eval mode). With `fuse` the producer's last CTA finalises `bn` in training, and its finalise op runs in eval only."""
+    def _stats(self, bn):
+        """a forward producer's (sum, sum of squares) operands for `bn`, training-only (NULL in eval mode). Every producer
+        passes NULL for its finalisation-descriptor operand: a finalise op of its own follows it."""
         if bn is None:
-            return None, None, None
-        bn.fused = fuse
-        return ("TRAIN_ONLY", bn.fsum), ("TRAIN_ONLY", bn.fsq), ("TRAIN_ONLY", bn.fin) if fuse else None
+            return None, None
+        return ("TRAIN_ONLY", bn.fsum), ("TRAIN_ONLY", bn.fsq)
 
-    def _gemm(self, A, B, C, M, Nn, K, bn=None, fuse=False, rowpack=True):
-        """C [M, Nn] = A [M, K] . B [Nn, K]^T (+ the batch statistics of `bn` over C); `fuse`: see _stats"""
+    def _gemm(self, A, B, C, M, Nn, K, bn=None, rowpack=True):
+        """C [M, Nn] = A [M, K] . B [Nn, K]^T (+ the batch statistics of `bn` over C)"""
         if self.gemm_impl != "tc":
-            return ("dfd_gemm_tn_mma", (A, B, C, None, M, Nn, K, self.dt) + self._stats(bn)[:2])
-        fs, fq, fin = self._stats(bn, fuse)
+            return ("dfd_gemm_tn_mma", (A, B, C, None, M, Nn, K, self.dt) + self._stats(bn))
+        fs, fq = self._stats(bn)
         pack = self._row_pack(M, K) if rowpack else 1
         if pack > 1:
-            return ("dfd_gemm_tn_rowpack", (A, self._blockdiag(B, Nn, K, pack), C, M, Nn, K, pack, self.dt, fs, fq, fin))
-        return ("dfd_gemm_tn", (A, B, C, M, Nn, K, self.dt, fs, fq, fin))
+            return ("dfd_gemm_tn_rowpack", (A, self._blockdiag(B, Nn, K, pack), C, M, Nn, K, pack, self.dt, fs, fq, None))
+        return ("dfd_gemm_tn", (A, B, C, M, Nn, K, self.dt, fs, fq, None))
 
     def _finalize(self, bn, count):
         """ops that finalise `bn` over `count` elements per rank: batch statistics -> scale / shift and the running
         statistics in training, running statistics -> scale / shift in eval (once per weight state, see forward).
         Synchronised BatchNorm finalises the SUM of every rank's statistics against the global count (torch SyncBatchNorm)."""
-        bn.count = count
         args = [bn.fsum, bn.fsq, float(count), bn.gamma, bn.beta, bn.rm, bn.rv, bn.nbt, self.bn_momentum, self.bn_eps,
                 "TRAINING", bn.C, bn.scale, bn.shift, bn.mean, bn.rstd]
         if self.sync_bn:
             return [("ALLREDUCE_train", (self.stats[bn.stat_off:bn.stat_off + 2 * self.L.stat_slots * bn.C], "sum")),
                     ("dfd_bn_finalize_sync", args)]
-        return [("dfd_bn_finalize" + ("_evalonly" if bn.fused else ""), args)]
+        return [("dfd_bn_finalize", args)]
 
     def _bwd_finalize(self, bn, count):
-        """ops that turn the backward sums of `bn` into the coefficients of dy (none when the producer's last CTA does it).
+        """ops that turn the backward sums of `bn` into the coefficients of dy.
         Synchronised BatchNorm averages (sum g, sum g*xhat) over the ranks and keeps the LOCAL count: the coefficients then use
         the global means, and dgamma / dbeta receive global_sum / world - what the DDP gradient mean of the per-rank sums gives."""
-        bn.count = count
         op = ("dfd_bn_bwd_finalize", (bn.bs1, bn.bs2, float(count), bn.gamma, bn.mean, bn.rstd, bn.dgamma, bn.dbeta,
                                       bn.cA, bn.cB, bn.cC, bn.C))
         if self.sync_bn:
             S = self.L.stat_slots
             return [("ALLREDUCE", (self.stats[bn.stat_off + 2 * S * bn.C:bn.stat_off + 4 * S * bn.C], "avg")), op]
-        return [] if self._fused_fin else [op]
-
-    def _bfin(self, bn):
-        """the finalisation descriptor a backward producer of `bn`'s sums takes (NULL: a dfd_bn_bwd_finalize op follows)"""
-        return bn.bfin if self._fused_fin else None
+        return [op]
 
     def _mask_head(self, masks, n_drop_block=0):
         """the ops at the head of the training forward that draw the step's masks: the DropBlock sites of
@@ -522,10 +470,9 @@ class Engine:
         return head
 
     def _finish_plan(self, fwd, bwd):
-        """resolve the workspace, upload the finalisation descriptors, check every op against the ABI table and publish the
-        plan as fwd_ops / bwd_ops: (function, name, args)"""
+        """resolve the workspace, check every op against the ABI table and publish the plan as fwd_ops / bwd_ops:
+        (function, name, args)"""
         bwd = self._patch_workspace(bwd)
-        self._upload_fin_descs()
         for n, a in fwd + bwd:
             if n.startswith("ALLREDUCE"):
                 continue
@@ -550,16 +497,14 @@ class Engine:
     def launch_args(self, name, args, training):
         """the C-ABI arguments (stream excluded) that the planned op `name` runs with in training or eval mode, or None when
         the op does not run in that mode. Eval mode: BatchNorm finalises from the running statistics (training = 0, no batch
-        sums), producers write no batch statistics, `_train` ops and ("TRAIN_ONLY", ptr) operands drop out. Training: an
-        `_evalonly` finalisation is done by its producer's last CTA, and a synchronised BatchNorm counts every rank's elements."""
+        sums), producers write no batch statistics, `_train` ops and ("TRAIN_ONLY", ptr) operands drop out. Training: a
+        synchronised BatchNorm counts every rank's elements."""
         if name == "dfd_bn_finalize_sync":
             args = list(args)
             if training:
                 args[2] = args[2] * self.sync_world          # global element count behind the summed statistics
             name = "dfd_bn_finalize"
-        if name.startswith("dfd_bn_finalize"):
-            if training and name.endswith("_evalonly"):
-                return None
+        if name == "dfd_bn_finalize":
             args = tuple((1 if training else 0) if a == "TRAINING" else a for a in args)
             if not training:
                 args = (None, None) + args[2:]

@@ -6,9 +6,7 @@ Stem 3x3 s2 -> BN -> Swish -> MBConv blocks (depthwise-separable and inverted-re
 NHWC tensors, the depthwise convolutions and their fused backward are `dfd_dwconv_*`, and the BatchNorm + activation of
 each conv output is folded into the kernel that consumes it, except where `dfd_bn_act` materialises it.
 """
-import os
 from collections import OrderedDict
-from functools import partial
 
 import torch
 
@@ -43,8 +41,6 @@ def build_efficientnet(e):
     if asym("conv_stem", 3) and e.stem_impl != "gemm":
         raise ValueError("stem_impl=%r: TF 'SAME' padding of the stem is planned through dfd_stem_im2col_pad (stem_impl='gemm')"
                          % (e.stem_impl,))
-    if os.environ.get("DFD_DW_SPLIT_BWD") and any(asym(b.name + ".conv_dw", b.k) for b in spec.blocks):
-        raise ValueError("DFD_DW_SPLIT_BWD: the split depthwise backward has no TF 'SAME' padding variant")
 
     # ---- BN bookkeeping arenas ---------------------------------------------------------------
     bn_specs = [("bn1", spec.stem)]
@@ -60,8 +56,7 @@ def build_efficientnet(e):
     G32 = lambda n: _ptr(e.grads32, e.p_off[n][0])
     P16 = lambda n: _ptr(e.params16, e.p_off[n][0])
     T16 = lambda n: _ptr(e.paramsT16, e.t_off[n][0])
-    gemm = partial(e._gemm, fuse=e._fused_gemm)
-    finalize, bwd_finalize, BF = e._finalize, e._bwd_finalize, e._bfin
+    gemm, finalize, bwd_finalize = e._gemm, e._finalize, e._bwd_finalize
 
     # ---- scratch for backward ----------------------------------------------------------------
     mid_max = max([N * h * w * b.cmid for b, h, w, ho, wo in blocks if b.kind == "ir"] +
@@ -100,7 +95,7 @@ def build_efficientnet(e):
         fwd.append(gemm(_ptr(e.stem_cols), _ptr(e.stem_wpad), _ptr(y0), N * Hs * Ws, spec.stem, Kp, bn))
     else:
         fwd.append(("dfd_stem_fwd", (_ptr(e.x_in), P32("conv_stem.weight"), _ptr(y0), N, spec.in_chans, e.H, e.W,
-                                     spec.stem, 3, 2, 1, dt) + e._stats(bn)[:2]))
+                                     spec.stem, 3, 2, 1, dt) + e._stats(bn)))
     fwd += finalize(bn, N * Hs * Ws)
     fwd.append(("dfd_bn_act", (_ptr(y0), bn.scale, bn.shift, None, None, _ptr(stem_out), N, Hs * Ws, spec.stem,
                                ACT_SWISH, 0, dt)))
@@ -132,7 +127,7 @@ def build_efficientnet(e):
         fwd.append(("dfd_dwconv_fwd" + ("_pad" if dw_pad else ""),
                     (_ptr(dw_in), dw_bn.scale if dw_bn else None, dw_bn.shift if dw_bn else None,
                      P32(p + ".conv_dw.weight"), _ptr(y2), N, h, w, b.cmid, b.k, b.stride) + dw_pad +
-                    (ACT_SWISH if dw_bn else ACT_NONE, dt) + e._stats(bn_mid, e._fused_fin)))
+                    (ACT_SWISH if dw_bn else ACT_NONE, dt) + e._stats(bn_mid) + (None,)))
         fwd += finalize(bn_mid, M2)
         gate_ptr = None
         if b.cse:
@@ -140,21 +135,11 @@ def build_efficientnet(e):
             gate = torch.zeros(N, b.cmid, dtype=torch.float32, device=dev)
             e._keep += [pooled, gate]
             rec.update(pooled=pooled, gate=gate)
-            if os.environ.get("DFD_SE_FUSED"):
-                # squeeze + excite in ONE launch (the CTA that completes an image's pooled vector runs its FC chain):
-                # slower than the two launches on the GPU this code was first tuned on (not re-measured on the H100):
-                # a 256-thread CTA walks the latency-bound chain four times longer than the 1024-thread FC kernel and
-                # the tail is not hidden; kept selectable
-                fwd.append(("dfd_pool_se", (_ptr(y2), bn_mid.scale, bn_mid.shift, _ptr(pooled), P32(p + ".se.conv_reduce.weight"),
-                                            P32(p + ".se.conv_reduce.bias"), P32(p + ".se.conv_expand.weight"),
-                                            P32(p + ".se.conv_expand.bias"), _ptr(gate), N, ho * wo, b.cmid, b.cse, ACT_SWISH, dt,
-                                            POOL_CHUNKS)))
-            else:
-                fwd.append(("dfd_pool", (_ptr(y2), bn_mid.scale, bn_mid.shift, _ptr(pooled), N, ho * wo, b.cmid, ACT_SWISH, dt,
-                                         None, POOL_CHUNKS)))
-                fwd.append(("dfd_se_fc_fwd", (_ptr(pooled), P32(p + ".se.conv_reduce.weight"), P32(p + ".se.conv_reduce.bias"),
-                                              P32(p + ".se.conv_expand.weight"), P32(p + ".se.conv_expand.bias"),
-                                              _ptr(gate), N, b.cmid, b.cse)))
+            fwd.append(("dfd_pool", (_ptr(y2), bn_mid.scale, bn_mid.shift, _ptr(pooled), N, ho * wo, b.cmid, ACT_SWISH, dt,
+                                     None, POOL_CHUNKS)))
+            fwd.append(("dfd_se_fc_fwd", (_ptr(pooled), P32(p + ".se.conv_reduce.weight"), P32(p + ".se.conv_reduce.bias"),
+                                          P32(p + ".se.conv_expand.weight"), P32(p + ".se.conv_expand.bias"),
+                                          _ptr(gate), N, b.cmid, b.cse)))
             gate_ptr = _ptr(gate)
         a2 = e._alloc16(N, ho, wo, b.cmid)
         fwd.append(("dfd_bn_act", (_ptr(y2), bn_mid.scale, bn_mid.shift, gate_ptr, None, _ptr(a2), N, ho * wo, b.cmid,
@@ -224,11 +209,11 @@ def build_efficientnet(e):
         bwd.append(("dfd_mul_f32", (_ptr(e.dpooled), _ptr(e.dropout_mask), N * P)))
     if pool_t == _lib.POOL_TYPES["avg"]:
         bwd.append(("dfd_act_bwd", (None, _ptr(yh), bnh.scale, bnh.shift, bnh.mean, bnh.rstd, None, _ptr(e.dpooled),
-                                    mid_a, N, Hf * Wf, F, ACT_SWISH, dt, bnh.bs1, bnh.bs2, BF(bnh))))
+                                    mid_a, N, Hf * Wf, F, ACT_SWISH, dt, bnh.bs1, bnh.bs2, None)))
     else:
         bwd.append(("dfd_act_bwd_gpool", (_ptr(yh), bnh.scale, bnh.shift, bnh.mean, bnh.rstd, _ptr(e.dpooled),
                                           _ptr(e.pool_argmax), mid_a, N, Hf * Wf, F, ACT_SWISH, pool_t, dt, bnh.bs1,
-                                          bnh.bs2, BF(bnh))))
+                                          bnh.bs2, None)))
     bwd += bwd_finalize(bnh, Mf)
     bwd.append(("dfd_bn_bwd_apply", (mid_a, _ptr(yh), None, bnh.cA, bnh.cB, bnh.cC, mid_b, N, Hf * Wf, F, dt)))
     cur = 0
@@ -252,7 +237,7 @@ def build_efficientnet(e):
                                        N, ho * wo, b.cout, ACT_NONE, 0, dt)))
             gbn = t2
         bwd.append(("dfd_bn_bwd_reduce", (gbn, _ptr(y3), None, bn_out.mean, bn_out.rstd, N, ho * wo, b.cout, dt,
-                                          bn_out.bs1, bn_out.bs2, BF(bn_out))))
+                                          bn_out.bs1, bn_out.bs2, None)))
         bwd += bwd_finalize(bn_out, M2)
         bwd.append(("dfd_bn_bwd_apply", (gbn, _ptr(y3), None, bn_out.cA, bn_out.cB, bn_out.cC, t1, N, ho * wo, b.cout, dt)))
         bwd.append(gemm(t1, T16(p + pw_name + ".weight"), mid_a, M2, b.cmid, b.cout))
@@ -260,54 +245,31 @@ def build_efficientnet(e):
         gate_ptr = dpool_ptr = None
         if b.cse:
             gate_ptr, dpool_ptr = _ptr(rec["gate"]), se_dpool
-            if os.environ.get("DFD_SE_FUSED"):
-                bwd.append(("dfd_se_bwd_chain", (mid_a, _ptr(y2), bn_mid.scale, bn_mid.shift, se_draw, _ptr(rec["pooled"]),
-                                                 P32(p + ".se.conv_reduce.weight"), P32(p + ".se.conv_reduce.bias"),
-                                                 P32(p + ".se.conv_expand.weight"), P32(p + ".se.conv_expand.bias"),
-                                                 se_de, se_r, se_drp, se_dpool, N, ho * wo, b.cmid, b.cse, dt)))
-                bwd.append(("dfd_se_fc_wgrad", (se_de, se_r, se_drp, _ptr(rec["pooled"]),
-                                                G32(p + ".se.conv_reduce.weight"), G32(p + ".se.conv_reduce.bias"),
-                                                G32(p + ".se.conv_expand.weight"), G32(p + ".se.conv_expand.bias"),
-                                                N, b.cmid, b.cse)))
-            else:
-                bwd.append(("dfd_se_bwd_reduce", (mid_a, _ptr(y2), bn_mid.scale, bn_mid.shift, se_draw, N, ho * wo, b.cmid, dt)))
-                bwd.append(("dfd_se_fc_bwd", (se_draw, _ptr(rec["pooled"]), P32(p + ".se.conv_reduce.weight"),
-                                              P32(p + ".se.conv_reduce.bias"), P32(p + ".se.conv_expand.weight"),
-                                              P32(p + ".se.conv_expand.bias"), se_de, se_r, se_drp, se_dpool,
-                                              G32(p + ".se.conv_reduce.weight"), G32(p + ".se.conv_reduce.bias"),
-                                              G32(p + ".se.conv_expand.weight"), G32(p + ".se.conv_expand.bias"),
-                                              N, b.cmid, b.cse)))
+            bwd.append(("dfd_se_bwd_reduce", (mid_a, _ptr(y2), bn_mid.scale, bn_mid.shift, se_draw, N, ho * wo, b.cmid, dt)))
+            bwd.append(("dfd_se_fc_bwd", (se_draw, _ptr(rec["pooled"]), P32(p + ".se.conv_reduce.weight"),
+                                          P32(p + ".se.conv_reduce.bias"), P32(p + ".se.conv_expand.weight"),
+                                          P32(p + ".se.conv_expand.bias"), se_de, se_r, se_drp, se_dpool,
+                                          G32(p + ".se.conv_reduce.weight"), G32(p + ".se.conv_reduce.bias"),
+                                          G32(p + ".se.conv_expand.weight"), G32(p + ".se.conv_expand.bias"),
+                                          N, b.cmid, b.cse)))
         bwd.append(("dfd_act_bwd", (mid_a, _ptr(y2), bn_mid.scale, bn_mid.shift, bn_mid.mean, bn_mid.rstd, gate_ptr,
-                                    dpool_ptr, mid_b, N, ho * wo, b.cmid, ACT_SWISH, dt, bn_mid.bs1, bn_mid.bs2, BF(bn_mid))))
+                                    dpool_ptr, mid_b, N, ho * wo, b.cmid, ACT_SWISH, dt, bn_mid.bs1, bn_mid.bs2, None)))
         bwd += bwd_finalize(bn_mid, M2)
         if b.kind == "ir":
             y1 = rec["y1"]
-            if os.environ.get("DFD_DW_SPLIT_BWD"):      # diagnostics: the two-pass form (same results)
-                bwd.append(("dfd_dwconv_dgrad", (mid_b, _ptr(y2), bn_mid.cA, bn_mid.cB, bn_mid.cC, P32(p + ".conv_dw.weight"),
-                                                 _ptr(y1), dw_bn.scale, dw_bn.shift, dw_bn.mean, dw_bn.rstd, None, mid_a,
-                                                 N, h, w, b.cmid, b.k, b.stride, 1, dt, dw_bn.bs1, dw_bn.bs2)))
-                bwd.append(("dfd_dwconv_wgrad", (_ptr(y1), dw_bn.scale, dw_bn.shift, mid_b, _ptr(y2), bn_mid.cA, bn_mid.cB,
-                                                 bn_mid.cC, G32(p + ".conv_dw.weight"), N, h, w, b.cmid, b.k, b.stride, dt)))
-            else:
-                # input gradient (through bn1 + Swish) and weight gradient in one pass over the dy tile
-                dw_pad = rec["dw_pad"]
-                bwd.append(e._dw_bwd((mid_b, _ptr(y2), bn_mid.cA, bn_mid.cB, bn_mid.cC, P32(p + ".conv_dw.weight"),
-                                      _ptr(y1), dw_bn.scale, dw_bn.shift, dw_bn.mean, dw_bn.rstd, None, mid_a,
-                                      G32(p + ".conv_dw.weight"), N, h, w, b.cmid, b.k, b.stride) + dw_pad +
-                                     (dt, dw_bn.bs1, dw_bn.bs2), N, h, w, b.cmid, b.k, b.stride, BF(dw_bn),
-                                     name="dfd_dwconv_bwd" + ("_pad" if dw_pad else "")))
+            # input gradient (through bn1 + Swish) and weight gradient in one pass over the dy tile
+            dw_pad = rec["dw_pad"]
+            bwd.append(e._dw_bwd((mid_b, _ptr(y2), bn_mid.cA, bn_mid.cB, bn_mid.cC, P32(p + ".conv_dw.weight"),
+                                  _ptr(y1), dw_bn.scale, dw_bn.shift, dw_bn.mean, dw_bn.rstd, None, mid_a,
+                                  G32(p + ".conv_dw.weight"), N, h, w, b.cmid, b.k, b.stride) + dw_pad +
+                                 (dt, dw_bn.bs1, dw_bn.bs2), N, h, w, b.cmid, b.k, b.stride,
+                                 name="dfd_dwconv_bwd" + ("_pad" if dw_pad else "")))
             bwd += bwd_finalize(dw_bn, M1)
             bwd.append(("dfd_bn_bwd_apply", (mid_a, _ptr(y1), None, dw_bn.cA, dw_bn.cB, dw_bn.cC, mid_b, N, h * w, b.cmid, dt)))
             bwd.append(gemm(mid_b, T16(p + ".conv_pw.weight"), t2, M1, b.cin, b.cmid))
             if b.has_residual:
                 bwd.append(("dfd_add_inplace", (t2, dout, M1 * b.cin, dt)))
             bwd.append(e._wgrad(mid_b, _ptr(xin), G32(p + ".conv_pw.weight"), M1, b.cmid, b.cin))
-        elif os.environ.get("DFD_DW_SPLIT_BWD"):
-            bwd.append(("dfd_dwconv_dgrad", (mid_b, _ptr(y2), bn_mid.cA, bn_mid.cB, bn_mid.cC, P32(p + ".conv_dw.weight"),
-                                             None, None, None, None, None, dout if b.has_residual else None, t2,
-                                             N, h, w, b.cmid, b.k, b.stride, 0, dt, None, None)))
-            bwd.append(("dfd_dwconv_wgrad", (_ptr(xin), None, None, mid_b, _ptr(y2), bn_mid.cA, bn_mid.cB, bn_mid.cC,
-                                             G32(p + ".conv_dw.weight"), N, h, w, b.cmid, b.k, b.stride, dt)))
         else:
             # DS block: the depthwise conv reads the block input as is (mode 0 of the fused pass); stride 1 in every
             # EfficientNet, so its padding is symmetric under TF "SAME" too
@@ -321,7 +283,7 @@ def build_efficientnet(e):
     # stem
     bn = e.bns["bn1"]
     bwd.append(("dfd_act_bwd", (sm[cur], _ptr(y0), bn.scale, bn.shift, bn.mean, bn.rstd, None, None, mid_a, N, Hs * Ws,
-                                spec.stem, ACT_SWISH, dt, bn.bs1, bn.bs2, BF(bn))))
+                                spec.stem, ACT_SWISH, dt, bn.bs1, bn.bs2, None)))
     bwd += bwd_finalize(bn, N * Hs * Ws)
     if e.stem_impl == "gemm":
         bwd.append(("dfd_bn_bwd_apply", (mid_a, _ptr(y0), None, bn.cA, bn.cB, bn.cC, mid_b, N, Hs * Ws, spec.stem, dt)))

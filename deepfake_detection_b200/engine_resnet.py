@@ -3,18 +3,22 @@
 Reference graph: dfd/timm/models/resnet.py:450-468 (stem 7x7 s2 -> BN -> ReLU -> maxpool 3x3 s2 -> 4 stages -> GAP
 -> fc), BasicBlock :150-175, Bottleneck :215-246 (stride on the 3x3, :195-197), downsample 1x1 conv + BN :249-260.
 
-Dense 3x3 convolutions with stride 1 (13 of the 16 in resnet50, all but 3 in resnet18) run as IMPLICIT GEMMs on wgmma
-(`dfd_conv_tc`, csrc/gemm_tc.cu conv mode: the TMA producer fetches the input box shifted by the tap through a 4-D tensor
-map, no im2col matrix in memory) in the forward pass and for the input gradient (same kernel on dY with the tap-flipped
-[Cin][kh'][kw'][Cout] weights). The strided 3x3 convolutions keep the round-1 formulation (csrc/conv_dense.cu):
-materialised im2col -> tensor-core GEMM (forward), GEMM -> col2im (input gradient). The weight gradient of every 3x3 is the
-MN-major wgmma wgrad GEMM, implicit too (`dfd_conv_wgrad_tc`: one pipeline stage = one patch of <= 64 output pixels of dY
-and the input box shifted by the tap). Stride-2 convolutions (the three strided 3x3 and the strided 1x1 downsample inputs) use
-the same kernels with TMA element strides {1, 2, 2, 1} in the forward pass and the weight gradient; the input gradient of a
-strided 3x3 is four parity-class implicit GEMMs (`dfd_conv_dgrad_s2_tc`) storing through strided views of dx. Only the strided
-1x1 downsample input gradient keeps GEMM + col2im (a scatter fused with the main-path add). 1x1 convolutions are plain GEMMs on the NHWC tensors. BN + ReLU outputs are materialised (`dfd_bn_act`) because three consumers read them.
+With gemm_impl="tc" every 3x3 convolution runs as an IMPLICIT GEMM on wgmma (`dfd_conv_tc`, csrc/gemm_tc.cu conv mode: the
+TMA producer fetches the input box shifted by the tap through a 4-D tensor map, no im2col matrix in memory), and so does the
+strided 1x1 downsample. Stride-2 convolutions use the same kernels with TMA element strides {1, 2, 2, 1}. The input gradient of
+a stride-1 3x3 is the same kernel on dY with the tap-flipped [Cin][kh'][kw'][Cout] weights; that of a strided 3x3 is four
+parity-class implicit GEMMs (`dfd_conv_dgrad_s2_tc`) storing through strided views of dx. The weight gradient of every 3x3 and
+of the strided downsample is the MN-major wgmma wgrad GEMM, implicit too (`dfd_conv_wgrad_tc`: one pipeline stage = one patch of
+<= 64 output pixels of dY and the input box shifted by the tap). The downsample's input gradient is added into the main-path
+gradient by the GEMM's own epilogue (`dfd_conv1x1_dgrad_add`).
+
+With gemm_impl="mma" (the mma.sync cross-check path) the convolutions keep the explicit formulation (csrc/conv_dense.cu):
+materialised im2col -> GEMM (forward and weight gradient), GEMM -> col2im (input gradient), and the strided downsample reads
+a gathered copy of its input.
+
+1x1 convolutions are plain GEMMs on the NHWC tensors. BN + ReLU outputs are materialised (`dfd_bn_act`) because three
+consumers read them.
 """
-import os
 import struct
 from collections import OrderedDict
 from functools import partial
@@ -117,31 +121,22 @@ def build_resnet(e):
     e._alloc_bn(bn_specs)
     bns = e.bns
 
-    fused_fin = e._fused_fin
     # no row-packed GEMMs: every ResNet K is >= 64 except the stem's Kp = 56 at in_chans = 1, which keeps the plain GEMM
-    gemm = partial(e._gemm, fuse=fused_fin, rowpack=False)
-    finalize, bwd_finalize, BF = e._finalize, e._bwd_finalize, e._bfin
+    gemm = partial(e._gemm, rowpack=False)
+    finalize, bwd_finalize = e._finalize, e._bwd_finalize
 
-    implicit = e.gemm_impl == "tc" and not os.environ.get("DFD_NO_IMPLICIT_CONV")
-    implicit_wgrad = not os.environ.get("DFD_NO_IMPLICIT_WGRAD")
-    implicit_s2 = not os.environ.get("DFD_NO_IMPLICIT_S2")          # stride-2 convolutions through TMA element strides
-    e.n_implicit = 0
+    implicit = e.gemm_impl == "tc"
 
     def conv3x3(xin, name, y, h, w, cin, cout, stride, bn):
         """3x3 / padding 1 forward into y (+ BatchNorm statistics of y)"""
-        if implicit and (stride == 1 or implicit_s2) and cin % 64 == 0 and cout % 64 == 0:
-            e.n_implicit += 1
-            return [("dfd_conv_tc", (xin, PK(name), y, N, h, w, cin, cout, 3, stride, dt) + e._stats(bn, fused_fin))]
+        if implicit and cin % 64 == 0 and cout % 64 == 0:
+            return [("dfd_conv_tc", (xin, PK(name), y, N, h, w, cin, cout, 3, stride, dt) + e._stats(bn) + (None,))]
         ho, wo = conv_out(h, 3, stride, 1), conv_out(w, 3, stride, 1)
         return [("dfd_im2col", (xin, COLS, N, h, w, cin, 3, stride, 1, dt)),
                 gemm(COLS, PK(name), y, N * ho * wo, cout, 9 * cin, bn)]
 
     # ---- stochastic regularisation (training only): DropBlock sites, drop-path gates, classifier dropout ---------------
-    relu_fuse = not (fused_fin or os.environ.get("DFD_NO_RELU_FUSE"))
     dp_rate, db_rate = e.drop_path_rate, e.drop_block_rate
-    if (e.drop_rate > 0.0 or dp_rate > 0.0 or db_rate > 0.0) and not relu_fuse:
-        raise _lib.NativeError("ResNet drop_rate / drop_path_rate / drop_block_rate need the default plan "
-                               "(not DFD_FUSED_FINALIZE or DFD_NO_RELU_FUSE)")
     sites = OrderedDict()           # "<block>.bn<i>" -> (H, W, C, gamma, cb)
     if db_rate > 0.0:
         for b, h, w, ho, wo in shapes:
@@ -208,7 +203,7 @@ def build_resnet(e):
         fwd.append(gemm(_ptr(e.stem_cols), _ptr(e.stem_wpad), _ptr(y0), N * H1 * W1, 64, Kp, bn0))
     else:
         fwd.append(("dfd_stem_fwd", (_ptr(e.x_in), P32("conv1.weight"), _ptr(y0), N, spec.in_chans, e.H, e.W, 64, 7, 2, 3, dt)
-                    + e._stats(bn0)[:2]))
+                    + e._stats(bn0)))
     fwd += finalize(bn0, N * H1 * W1)
     fwd.append(bn_relu(y0, bn0, a0, H1 * W1, 64))
     fwd.append(("dfd_maxpool_fwd", (_ptr(a0), _ptr(x0), _ptr(e.pool_idx), N, H1, W1, 64, dt)))
@@ -251,16 +246,14 @@ def build_resnet(e):
             bnd = bns[p + ".downsample.1"]
             yd = e._alloc16(N, ho, wo, b.cout)
             r = e._alloc16(N, ho, wo, b.cout)
-            ds_implicit = (implicit and implicit_s2 and implicit_wgrad and b.stride == 2 and b.cin % 64 == 0 and b.cout % 64 == 0 and
-                           e._wgrad_name == "dfd_gemm_wgrad")
             if b.stride == 1:
                 xs = x
                 fwd.append(gemm(_ptr(xs), P16(p + ".downsample.0.weight"), _ptr(yd), M2, b.cout, b.cin, bnd))
-            elif ds_implicit:
+            elif implicit and b.cin % 64 == 0 and b.cout % 64 == 0:
                 # strided 1x1 convolution straight from the block input (k = 1, stride 2 implicit GEMM): no gathered copy
                 xs = None
                 fwd.append(("dfd_conv_tc", (_ptr(x), P16(p + ".downsample.0.weight"), _ptr(yd), N, h, w, b.cin, b.cout, 1, b.stride, dt)
-                            + e._stats(bnd, fused_fin)))
+                            + e._stats(bnd) + (None,)))
             else:
                 xs = e._alloc16(N, ho, wo, b.cin)
                 fwd.append(("dfd_im2col", (_ptr(x), _ptr(xs), N, h, w, b.cin, 1, b.stride, 0, dt)))
@@ -328,8 +321,7 @@ def build_resnet(e):
         if implicit and stride == 1 and dx_add is None and Cin % 64 == 0 and Cout % 64 == 0:
             # input gradient = the same implicit GEMM on dY with the tap-flipped [Cin][kh'][kw'][Cout] weights
             ops = [("dfd_conv_tc", (dy, PKD(name), dx_out, N, n_h, n_w, Cout, Cin, 3, 1, dt, None, None, None))]
-        elif implicit and implicit_s2 and stride == 2 and dx_add is None and Cin % 64 == 0 and Cout % 64 == 0 and \
-                not os.environ.get("DFD_NO_IMPLICIT_S2_DGRAD"):
+        elif implicit and stride == 2 and dx_add is None and Cin % 64 == 0 and Cout % 64 == 0:
             # strided input gradient: four parity-class implicit GEMMs storing through strided views of dx
             ops = [("dfd_conv_dgrad_s2_tc", (dy, PKD(name), dx_out, N, n_h, n_w, Cin, Cout, dt))]
         else:
@@ -337,17 +329,14 @@ def build_resnet(e):
                    ("dfd_col2im", (COLS, dx_add, dx_out, N, n_h, n_w, Cin, 3, stride, 1, dt))]
         gp = _ptr(e.gperm, len(pending_unpack) * gperm_max)         # this block's next free region
         assert len(pending_unpack) < 2
-        if implicit and implicit_wgrad and (stride == 1 or implicit_s2) and Cin % 64 == 0 and e._wgrad_name == "dfd_gemm_wgrad":
+        if implicit and Cin % 64 == 0:
             ops += [zero_gperm(gp, Cout * 9 * Cin),
                     e._wgrad_conv(dy, _ptr(xin_t), gp, N, n_h, n_w, Cin, Cout, 3, stride)]
         else:
             ops += [("dfd_im2col", (_ptr(xin_t), COLS, N, n_h, n_w, Cin, 3, stride, 1, dt)),
                     zero_gperm(gp, Cout * 9 * Cin),
                     e._wgrad(dy, COLS, gp, M_out, Cout, 9 * Cin)]
-        if e._nondet:
-            ops.append(("dfd_unpack_grad", (gp, G32(name), Cout, Cin, 3)))       # atomics: complete when the kernel is
-        else:
-            pending_unpack.append((gp, name, Cout, Cin))     # complete after the block's ordered reduce (flush_block)
+        pending_unpack.append((gp, name, Cout, Cin))     # complete after the block's ordered reduce (flush_block)
         return ops
 
     bwd.append(("dfd_head_bwd", (_ptr(e.dlogits), _ptr(e.pooled), P32("fc.weight"), G32("fc.weight"), G32("fc.bias"),
@@ -360,7 +349,7 @@ def build_resnet(e):
         bwd.append(("dfd_gpool_bwd", (_ptr(e.dpooled), _ptr(e.pool_argmax), gA, N, Hf * Wf, F, pool_t, dt)))
     # The gradient entering a block is kept as up to TWO tensors (main-path dx + identity-path gm of the block above): the
     # fused ReLU / BN-backward reduction adds them on the fly (dfd_relu_bn_bwd_reduce), which removes the materialised
-    # residual add of every block without a downsample branch. DFD_NO_RELU_FUSE=1 restores the three separate passes.
+    # residual add of every block without a downsample branch.
     def relu_bwd(da, y, bn, gu, hw, C, site):
         """gradient through BN output -> (DropBlock) -> ReLU, plus the BN backward sums"""
         if site in sites:
@@ -368,7 +357,7 @@ def build_resnet(e):
             return ("dfd_act_bwd_drop", (da, _ptr(y), bn.scale, bn.shift, bn.mean, bn.rstd, m, k, numel, gu, N, hw, C, dt,
                                          bn.bs1, bn.bs2))
         return ("dfd_act_bwd", (da, _ptr(y), bn.scale, bn.shift, bn.mean, bn.rstd, None, None, gu, N, hw, C, ACT_RELU, dt,
-                                bn.bs1, bn.bs2, BF(bn)))
+                                bn.bs1, bn.bs2, None))
 
     bufs = [gA, gB, gC, gD, gE, gF]
     dout, dout2 = gA, None
@@ -378,10 +367,7 @@ def build_resnet(e):
         M1, M2 = N * h * w, N * ho * wo
         gm, t1, t2, t3 = [g for g in bufs if g not in (dout, dout2)][:4]
         bl = rec["bnlast"]
-        if not relu_fuse:
-            bwd.append(("dfd_relu_bwd", (dout, _ptr(rec["out"]), gm, M2 * b.cout, dt)))
-            bwd.append(("dfd_bn_bwd_reduce", (gm, _ptr(rec["ylast"]), None, bl.mean, bl.rstd, N, ho * wo, b.cout, dt, bl.bs1, bl.bs2, BF(bl))))
-        elif rec["site_last"] in sites or rec["gate"] is not None:
+        if rec["site_last"] in sites or rec["gate"] is not None:
             # gm goes unmasked to the identity / downsample path; the last BN sees gd = gm * (DropBlock) * (drop path) in t2
             m, k, numel = site_args(rec["site_last"]) if rec["site_last"] in sites else (None, None, 0)
             gate = _ptr(rec["gate"]) if rec["gate"] is not None else None
@@ -423,11 +409,10 @@ def build_resnet(e):
         # identity / downsample path: gradient gm flows to the block input too
         if b.downsample:
             bnd = rec["bnd"]
-            bwd.append(("dfd_bn_bwd_reduce", (gm, _ptr(rec["yd"]), None, bnd.mean, bnd.rstd, N, ho * wo, b.cout, dt, bnd.bs1, bnd.bs2, BF(bnd))))
+            bwd.append(("dfd_bn_bwd_reduce", (gm, _ptr(rec["yd"]), None, bnd.mean, bnd.rstd, N, ho * wo, b.cout, dt, bnd.bs1, bnd.bs2, None)))
             bwd += bwd_finalize(bnd, M2)
             bwd.append(("dfd_bn_bwd_apply", (gm, _ptr(rec["yd"]), None, bnd.cA, bnd.cB, bnd.cC, t1, N, ho * wo, b.cout, dt)))
-            ds_add = (implicit and implicit_s2 and b.cin % 64 == 0 and b.cout % 64 == 0 and
-                      not os.environ.get("DFD_NO_DGRAD_ADD"))
+            ds_add = implicit and b.cin % 64 == 0 and b.cout % 64 == 0
             if ds_add:
                 # the downsample input gradient is ADDED into t3 (main-path gradient) by the GEMM's own epilogue: a TMA reduction
                 # store through the stride-s pixel view of t3 - no scratch tensor, no col2im scatter / add pass
@@ -448,11 +433,8 @@ def build_resnet(e):
                 # has been consumed by the reduction above: reused as the destination)
                 bwd.append(("dfd_col2im", (t2, t3, dout, N, h, w, b.cin, 1, b.stride, 0, dt)))
                 new_dout = (dout, None)
-        elif relu_fuse:
-            new_dout = (t3, gm)             # the block below adds them while it masks and reduces
         else:
-            bwd.append(("dfd_add_inplace", (t3, gm, M1 * b.cin, dt)))
-            new_dout = (t3, None)
+            new_dout = (t3, gm)             # the block below adds them while it masks and reduces
         flush_block(bwd)
         dout, dout2 = new_dout
     # stem: maxpool -> relu/bn1 -> conv1 wgrad
@@ -461,7 +443,7 @@ def build_resnet(e):
     t1, t2 = [g for g in bufs if g != dout][:2]
     bwd.append(("dfd_maxpool_bwd", (dout, _ptr(e.pool_idx), t1, N, H1, W1, 64, dt)))
     bwd.append(("dfd_act_bwd", (t1, _ptr(y0), bn0.scale, bn0.shift, bn0.mean, bn0.rstd, None, None, t2, N, H1 * W1, 64,
-                                ACT_RELU, dt, bn0.bs1, bn0.bs2, BF(bn0))))
+                                ACT_RELU, dt, bn0.bs1, bn0.bs2, None)))
     bwd += bwd_finalize(bn0, N * H1 * W1)
     if e.stem_impl == "gemm":
         bwd.append(("dfd_bn_bwd_apply", (t2, _ptr(y0), None, bn0.cA, bn0.cB, bn0.cC, t1, N, H1 * W1, 64, dt)))

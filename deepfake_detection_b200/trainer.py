@@ -41,8 +41,6 @@ class Trainer:
             self.optimizer.skip_flag = _ptr(e0.flags, 0)
         # every optimizer is graph-captured: learning rates and Adam's step count are device-resident (optim.py)
         self.use_graph = bool(use_graph)
-        import os
-        self.split_graph = bool(os.environ.get("DFD_DDP_SPLIT_GRAPH"))      # diagnostic, see step_resident
         self._graph = None
         self._graph_key = None
         self.n_captures = 0
@@ -66,8 +64,7 @@ class Trainer:
 
     # ---- the step ---------------------------------------------------------------------------------
     def _launch_step(self, soft, part=None):
-        """part: None = the whole step; "front" = up to and including backward (no gradient collective), "back" = everything
-        after the gradient mean (split-graph data-parallel mode, see step_resident)"""
+        """part: None = the whole step; "back" = only the update phase that follows backward and the gradient mean"""
         e = self.engine
         st = torch.cuda.current_stream().cuda_stream
         if part != "back":
@@ -75,12 +72,10 @@ class Trainer:
             e.forward(training=True, stream=st)
             e.head(True, smoothing=self.smoothing, soft=soft, stream=st,
                    loss_scale_dev=_ptr(e.loss_scale_state, 0) if self.dynamic_scale else None)
-            if self.reducer is not None and part is None:
+            if self.reducer is not None:
                 self.reducer.backward_and_reduce(e)
             else:
                 e.backward(stream=st)
-            if part == "front":
-                return
         if self.dynamic_scale:
             _lib.call("dfd_check_finite", _ptr(e.grads32), e.n_params, _ptr(e.flags, 0), st)
         self.optimizer.step(stream=st, push=False)      # learning rates were pushed to the device before the launch / replay
@@ -102,27 +97,6 @@ class Trainer:
             self._launch_step(soft)
             return
         key = self._graph_signature(soft)
-        if self.reducer is not None and self.split_graph:
-            # data-parallel, split mode: [forward + backward] graph -> ONE eager NCCL mean over the whole gradient arena ->
-            # [update] graph. No collective inside a captured graph, no overlap with backward.
-            if self._graph is None or key != self._graph_key:
-                self._launch_step(soft, "front")
-                self.reducer.reduce_all()
-                self._launch_step(soft, "back")
-                torch.cuda.synchronize()
-                ga, gb = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
-                with torch.cuda.graph(ga):
-                    self._launch_step(soft, "front")
-                self.reducer.reduce_all()
-                with torch.cuda.graph(gb):
-                    self._launch_step(soft, "back")
-                self._graph, self._graph_key = (ga, gb), key
-                self.n_captures += 1
-                return
-            self._graph[0].replay()
-            self.reducer.reduce_all()
-            self._graph[1].replay()
-            return
         if self._graph is None or key != self._graph_key:
             # warm-up launch outside capture (module loading, cudaFuncSetAttribute, tensor-map encoding paths)
             self._launch_step(soft)

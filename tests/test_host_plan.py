@@ -121,19 +121,59 @@ def test_resnet_plan_validation_checks_argument_types(monkeypatch):
         Engine("resnet18", 2, 64, 64, device="plan-only")
 
 
-@pytest.mark.parametrize("fused_finalize", ["", "1"])
-def test_resnet_eval_forward_passes_no_statistics_to_the_implicit_conv(monkeypatch, fused_finalize):
-    """dfd_conv_tc writes batch statistics (and, with DFD_FUSED_FINALIZE=1, finalises them) in training only: an eval forward
-    passes NULL for the statistics and the descriptor, so it neither accumulates them nor moves the running statistics"""
+def test_resnet_eval_forward_passes_no_statistics_to_the_implicit_conv():
+    """dfd_conv_tc writes batch statistics in training only: an eval forward passes NULL for them, so it does not accumulate
+    them. No producer is planned with a finalisation descriptor: a dfd_bn_finalize launch of its own follows it"""
     from deepfake_detection_b200.engine import Engine
-    monkeypatch.setenv("DFD_FUSED_FINALIZE", fused_finalize)
     eng = Engine("resnet50", 2, 160, 160, device="plan-only")
     convs = [a for _, n, a in eng.fwd_ops if n == "dfd_conv_tc"]
     assert len(convs) == 16 + 3          # every 3x3 convolution and the three strided 1x1 downsamples
     for a in convs:
         train, ev = eng.launch_args("dfd_conv_tc", a, True), eng.launch_args("dfd_conv_tc", a, False)
         assert ev[:-3] == train[:-3] and ev[-3:] == (None, None, None)
-        assert train[-3] and train[-2] and bool(train[-1]) == (fused_finalize == "1")
+        assert train[-3] and train[-2] and train[-1] is None
+
+
+def test_package_reads_no_environment():
+    """what a plan launches follows from the Engine / Trainer arguments alone: no module of the package reads the
+    environment (the kernels' own launch-geometry overrides under csrc/ are C code)"""
+    pkg = os.path.join(ROOT, "deepfake_detection_b200")
+    for dp, _, files in os.walk(pkg):
+        for f in files:
+            if f.endswith(".py"):
+                src = open(os.path.join(dp, f)).read()
+                assert not re.search(r"\b(environ|getenv)\b", src), f
+
+
+# environment variables that earlier versions of the plan builders, the Trainer and the DDP reducer read, each at a
+# non-default value
+RETIRED_VARIABLES = dict(DFD_NONDET="1", DFD_WGRAD_MMA="1", DFD_NO_ROWPACK="1", DFD_SE_FUSED="1", DFD_DW_SPLIT_BWD="1",
+                         DFD_NO_IMPLICIT_CONV="1", DFD_NO_IMPLICIT_WGRAD="1", DFD_NO_IMPLICIT_S2="1",
+                         DFD_NO_IMPLICIT_S2_DGRAD="1", DFD_NO_DGRAD_ADD="1", DFD_NO_RELU_FUSE="1", DFD_DDP_SPLIT_GRAPH="1",
+                         DFD_DDP_BUCKET_MB="1")
+
+
+@pytest.mark.parametrize("fused_finalize", ["1", "gemm"])
+def test_retired_environment_variables_leave_the_plan_alone(monkeypatch, fused_finalize):
+    """plan-only engines built with every retired variable set issue the same launches as without them"""
+    from plan_launches import _split
+    from deepfake_detection_b200.engine import Engine, base_name
+
+    def launches(arch, H, W, kw):
+        eng = Engine(arch, 2, H, W, device="plan-only", **kw)
+        return [(n, _split(base_name(n), a)) for _, n, a in eng.fwd_ops + eng.bwd_ops]
+
+    configs = [("efficientnet_b0", 64, 64, dict(drop_rate=0.2, drop_path_rate=0.2)),
+               ("tf_efficientnet_b0", 66, 96, {}),
+               ("resnet50", 160, 160, dict(drop_rate=0.2, drop_path_rate=0.1, drop_block_rate=0.1)),
+               ("resnet18", 64, 64, dict(gemm_impl="mma"))]
+    for name in list(RETIRED_VARIABLES) + ["DFD_FUSED_FINALIZE"]:
+        monkeypatch.delenv(name, raising=False)
+    plain = [launches(*c) for c in configs]
+    for name, value in dict(RETIRED_VARIABLES, DFD_FUSED_FINALIZE=fused_finalize).items():
+        monkeypatch.setenv(name, value)
+    for c, ref in zip(configs, plain):
+        assert launches(*c) == ref, c[0]
 
 
 def test_resnet_refuses_sync_bn_over_several_ranks(monkeypatch):

@@ -57,7 +57,7 @@ def make_trainer(eng, opt, use_graph=False, lrs=LRS):
         a.loss_scale_state.copy_(torch.tensor([65536.0, 1.0 / 65536.0]))
         tr.optimizer.gscale_dev = _ptr(a.loss_scale_state, 1)
         tr.optimizer.skip_flag = _ptr(a.flags, 0)
-    tr.use_graph, tr.split_graph = use_graph, False
+    tr.use_graph = use_graph
     tr._graph = tr._graph_key = None
     tr.n_captures = 0
     tr.reducer = None

@@ -1,13 +1,13 @@
 """Canonical digest of the engine's call plans, for checking that a host-side change leaves the plans alone (CPU only).
 
-For every configuration below and every environment switch of the plan builders, a plan-only engine is built and written
-out as text: the training forward and backward and the eval forward, each op as `Engine.launch_args` gives it (a skipped
-op is listed as such), then the descriptor tables the engine uploads (ordered reduce, BatchNorm finalisation, dropout /
-drop-path masks, DropBlock sites) and the derived weight layouts its arena registers (block-diagonal copies, packed k x k
-weights, transposed 1x1 weights, padded stem weight). Every device pointer, in the arguments and in the tables, is replaced
-by the index of its first appearance, so two builds of the same plan give the same text.
+For every configuration below a plan-only engine is built and written out as text: the training forward and backward and
+the eval forward, each op as `Engine.launch_args` gives it (a skipped op is listed as such), then the descriptor tables the
+engine uploads (ordered reduce, dropout / drop-path masks, DropBlock sites) and the derived weight layouts its arena
+registers (block-diagonal copies, packed k x k weights, transposed 1x1 weights, padded stem weight). Every device pointer,
+in the arguments and in the tables, is replaced by the index of its first appearance, so two builds of the same plan give
+the same text.
 
-    python tools/plan_digest.py OUT.txt              # every configuration, every switch
+    python tools/plan_digest.py OUT.txt              # every configuration
     python tools/plan_digest.py OUT.txt --quick      # the small configurations only
 
 Run it on two commits and diff the outputs.
@@ -28,7 +28,7 @@ import torch  # noqa: E402
 from deepfake_detection_b200 import _lib  # noqa: E402
 from deepfake_detection_b200.engine import Engine  # noqa: E402
 
-SUFFIXES = ("_train", "_evalonly", "_sync")
+SUFFIXES = ("_train", "_sync")
 
 # (arch, batch, H, W, Engine kwargs)
 SMALL = [
@@ -53,11 +53,6 @@ SMALL = [
     ("resnet50", 3, 96, 96, {}),
 ] + [(a, 2, 64, 64, dict(global_pool=g)) for a in ("efficientnet_b0", "resnet18") for g in ("max", "avgmax", "catavgmax")]
 
-SWITCHES = [{}, {"DFD_FUSED_FINALIZE": "1"}, {"DFD_FUSED_FINALIZE": "gemm"}, {"DFD_SE_FUSED": "1"},
-            {"DFD_DW_SPLIT_BWD": "1"}, {"DFD_NONDET": "1"}, {"DFD_NO_ROWPACK": "1"}, {"DFD_WGRAD_MMA": "1"},
-            {"DFD_NO_IMPLICIT_CONV": "1"}, {"DFD_NO_IMPLICIT_WGRAD": "1"}, {"DFD_NO_IMPLICIT_S2": "1"},
-            {"DFD_NO_IMPLICIT_S2_DGRAD": "1"}, {"DFD_NO_RELU_FUSE": "1"}, {"DFD_NO_DGRAD_ADD": "1"}]
-
 
 def shipped_configs():
     from plan_launches import CONFIGS
@@ -65,21 +60,15 @@ def shipped_configs():
 
 
 @contextmanager
-def environment(switch, world):
-    old = {k: os.environ.pop(k) for k in list(os.environ) if k.startswith("DFD_")}
-    os.environ.update(switch)
-    try:
-        if world > 1:       # a process group of `world` ranks, as a synchronised BatchNorm plan sees it
-            with mock.patch("torch.distributed.is_available", return_value=True), \
-                    mock.patch("torch.distributed.is_initialized", return_value=True), \
-                    mock.patch("torch.distributed.get_world_size", return_value=world):
-                yield
-        else:
-            yield
-    finally:
-        for k in [k for k in os.environ if k.startswith("DFD_")]:
-            del os.environ[k]
-        os.environ.update(old)
+def world_size(world):
+    """a process group of `world` ranks, as a synchronised BatchNorm plan sees it"""
+    if world == 1:
+        yield
+        return
+    with mock.patch("torch.distributed.is_available", return_value=True), \
+            mock.patch("torch.distributed.is_initialized", return_value=True), \
+            mock.patch("torch.distributed.get_world_size", return_value=world):
+        yield
 
 
 class Pointers:
@@ -151,12 +140,6 @@ def digest(e):
     lines.append("n_launch %r" % sorted(e.n_launch.items()))
     if getattr(e, "_red_table", None) is not None:
         lines += ["reduce " + r for r in table(ptr, as_bytes(e._red_table), "<QQqqii", 2)]
-    raw = as_bytes(e._fin_buf)
-    nb = len(e.bns)
-    for bn in sorted(e.bns.values(), key=lambda b: b.idx):
-        lines += ["fin %s %s" % (bn.name, r) for r in table(ptr, raw[bn.idx * 128:bn.idx * 128 + 96], "<12Qddffii", 12)]
-        lines += ["bfin %s %s" % (bn.name, r) for r in
-                  table(ptr, raw[(nb + bn.idx) * 128:(nb + bn.idx) * 128 + 112], "<11Qdii", 11)]
     if getattr(e, "_mask_table", None) is not None:
         lines += ["mask " + r for r in table(ptr, as_bytes(e._mask_table), "<Qqifii", 1)]
     if getattr(e, "_drop_block_table", None) is not None:
@@ -181,17 +164,15 @@ def main():
     with open(args.out, "w") as f:
         for arch, batch, H, W, kw in configs:
             kw = dict(kw)
-            world = 2 if kw.get("sync_bn") else 1
-            for switch in SWITCHES:
-                head = "=== %s n=%d %dx%d %r %r" % (arch, batch, H, W, sorted(kw.items()), sorted(switch.items()))
-                with environment(switch, world):
-                    try:
-                        e = Engine(arch, batch, H, W, device="plan-only", **kw)
-                    except (ValueError, _lib.NativeError) as err:
-                        f.write("%s\nREFUSED %s: %s\n" % (head, type(err).__name__, err))
-                        continue
-                    f.write("\n".join([head] + digest(e)) + "\n")
-                    e = None
+            head = "=== %s n=%d %dx%d %r" % (arch, batch, H, W, sorted(kw.items()))
+            with world_size(2 if kw.get("sync_bn") else 1):
+                try:
+                    e = Engine(arch, batch, H, W, device="plan-only", **kw)
+                except (ValueError, _lib.NativeError) as err:
+                    f.write("%s\nREFUSED %s: %s\n" % (head, type(err).__name__, err))
+                    continue
+                f.write("\n".join([head] + digest(e)) + "\n")
+                e = None
             print(arch, batch, H, W, kw, flush=True)
 
 
