@@ -52,6 +52,8 @@ SIGNATURES = {
     "dfd_act_bwd": "ppppppppp" "ili" "ii" "ppp" "p",
     "dfd_act_bwd_gpool": "pppppppp" "ili" "iii" "ppp" "p",
     "dfd_add_inplace": "pp" "li" "p",
+    "dfd_avgpool2_fwd": "pp" "iiii" "i" "p",
+    "dfd_avgpool2_bwd_add": "ppp" "iiii" "i" "p",
     "dfd_se_fc_fwd": "pppppp" "iii" "p",
     "dfd_se_fc_bwd": "pppppp" "pppppppp" "iii" "p",
     "dfd_se_fc_wgrad": "pppp" "pppp" "iii" "p",

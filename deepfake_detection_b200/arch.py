@@ -15,6 +15,8 @@ BASELINE.json names; it builds no modules and owns no tensors.
   * tf_efficientnet_b0..b7 (+ _ap, _ns): the B0 generator with pad_type='same', efficientnet.py:1265-1530; TF "SAME"
     padding of the stride-2 convolutions, layers/padding.py `pad_same` / layers/conv2d_same.py
   * ResNet-18/50 layout: dfd/timm/models/resnet.py:115-260,280-468,472,523
+  * ResNet-26/34/101/152, tv_*, wide_* (base_width 128) and ResNet-D (deep stem, downsample_avg): resnet.py:187,263-277,
+    349-439,483-625
 """
 import math
 import re
@@ -157,6 +159,8 @@ class ResBlock:
     cout: int
     stride: int
     downsample: bool     # 1x1 conv (stride) + BN on the identity path
+    width: int           # bottleneck width int(planes * base_width / 64), resnet.py:187 (== planes for a BasicBlock)
+    avg_down: bool = False   # ResNet-D shortcut: AvgPool2d(2, stride, ceil_mode, count_include_pad=False) -> 1x1 conv -> BN
 
 
 @dataclass
@@ -170,13 +174,15 @@ class ResNetSpec:
     input_size: Tuple[int, int, int]
     family: str = "resnet"
     global_pool: str = "avg"
+    stem_type: str = ""          # '' (7x7 conv) or 'deep' (3x3 s2 -> 3x3 -> 3x3 of stem_width, stem_width, 64), resnet.py:365-379
+    stem_width: int = 32
 
     @property
     def pooled_features(self):
         return self.num_features * pool_feat_mult(self.global_pool)
 
 
-def _resnet_spec(arch, kind, layers, in_chans, num_classes, input_size):
+def _resnet_spec(arch, kind, layers, in_chans, num_classes, input_size, base_width=64, stem_type="", avg_down=False):
     exp = 4 if kind == "bottleneck" else 1
     blocks = []
     cin = 64
@@ -186,10 +192,11 @@ def _resnet_spec(arch, kind, layers, in_chans, num_classes, input_size):
             cout = planes * exp
             blocks.append(ResBlock(name="layer%d.%d" % (li + 1, bi), kind=kind, cin=cin, planes=planes,
                                    cout=cout, stride=stride,
-                                   downsample=(bi == 0 and (stride != 1 or cin != cout))))
+                                   downsample=(bi == 0 and (stride != 1 or cin != cout)),
+                                   width=int(math.floor(planes * (base_width / 64))), avg_down=avg_down))
             cin = cout
     return ResNetSpec(arch=arch, in_chans=in_chans, stem=64, blocks=blocks, num_features=cin,
-                      num_classes=num_classes, input_size=input_size)
+                      num_classes=num_classes, input_size=input_size, stem_type=stem_type)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -232,10 +239,31 @@ def _base_spec(arch, num_classes, in_chans):
         return _resnet_spec(arch, "basic", (2, 2, 2, 2), in_chans, num_classes, (3, 224, 224))
     if arch == "resnet50":
         return _resnet_spec(arch, "bottleneck", (3, 4, 6, 3), in_chans, num_classes, (3, 224, 224))
+    if arch in RESNET_ARCHS:
+        kind, layers, base_width, deep = _RESNET_DEFS[arch]
+        return _resnet_spec(arch, kind, layers, in_chans, num_classes, (3, 224, 224), base_width=base_width,
+                            stem_type="deep" if deep else "", avg_down=deep)
     raise ValueError("arch %r is not on the native hot path (see SURVEY.md section 8)" % (arch,))
 
 
 SUPPORTED_ARCHS = ("efficientnet_b0", "efficientnet_b4", "efficientnet_deepfake_v4", "resnet18", "resnet50")
+
+# The rest of the dense ResNet registry (resnet.py:483-625): arch -> (block, layers, base_width, ResNet-D). ResNet-D is
+# stem_type='deep', stem_width=32, avg_down=True (resnet26d, resnet50d); base_width=128 doubles the bottleneck width
+# (wide_*). tv_* differ from resnet34 / resnet50 only in their default_cfg.
+_RESNET_DEFS = {
+    "resnet26": ("bottleneck", (2, 2, 2, 2), 64, False),
+    "resnet34": ("basic", (3, 4, 6, 3), 64, False),
+    "resnet101": ("bottleneck", (3, 4, 23, 3), 64, False),
+    "resnet152": ("bottleneck", (3, 8, 36, 3), 64, False),
+    "tv_resnet34": ("basic", (3, 4, 6, 3), 64, False),
+    "tv_resnet50": ("bottleneck", (3, 4, 6, 3), 64, False),
+    "wide_resnet50_2": ("bottleneck", (3, 4, 6, 3), 128, False),
+    "wide_resnet101_2": ("bottleneck", (3, 4, 23, 3), 128, False),
+    "resnet26d": ("bottleneck", (2, 2, 2, 2), 64, True),
+    "resnet50d": ("bottleneck", (3, 4, 6, 3), 64, True),
+}
+RESNET_ARCHS = tuple(_RESNET_DEFS)
 
 # TensorFlow-ported EfficientNets (efficientnet.py:1265-1530): the B0 generator with TF "SAME" padding and BatchNorm eps 1e-3.
 # _ap (AdvProp) and _ns (Noisy Student) share the plain variant's layers; only their default_cfg differs (models.py).
@@ -315,7 +343,16 @@ def state_entries(spec):
         out.append(("classifier.weight", (spec.num_classes, spec.pooled_features), "fc_w"))
         out.append(("classifier.bias", (spec.num_classes,), "fc_b"))
     else:
-        out.append(("conv1.weight", (64, spec.in_chans, 7, 7), "conv_w"))
+        if spec.stem_type == "deep":
+            # conv1 = Sequential(conv, bn, relu, conv, bn, relu, conv), resnet.py:370-377
+            sw = spec.stem_width
+            out.append(("conv1.0.weight", (sw, spec.in_chans, 3, 3), "conv_w"))
+            out += _bn_entries("conv1.1", sw)
+            out.append(("conv1.3.weight", (sw, sw, 3, 3), "conv_w"))
+            out += _bn_entries("conv1.4", sw)
+            out.append(("conv1.6.weight", (64, sw, 3, 3), "conv_w"))
+        else:
+            out.append(("conv1.weight", (64, spec.in_chans, 7, 7), "conv_w"))
         out += _bn_entries("bn1", 64)
         for b in spec.blocks:
             p = b.name
@@ -325,15 +362,17 @@ def state_entries(spec):
                 out.append((p + ".conv2.weight", (b.cout, b.planes, 3, 3), "conv_w"))
                 out += _bn_entries(p + ".bn2", b.cout)
             else:
-                out.append((p + ".conv1.weight", (b.planes, b.cin, 1, 1), "conv_w"))
-                out += _bn_entries(p + ".bn1", b.planes)
-                out.append((p + ".conv2.weight", (b.planes, b.planes, 3, 3), "conv_w"))
-                out += _bn_entries(p + ".bn2", b.planes)
-                out.append((p + ".conv3.weight", (b.cout, b.planes, 1, 1), "conv_w"))
+                out.append((p + ".conv1.weight", (b.width, b.cin, 1, 1), "conv_w"))
+                out += _bn_entries(p + ".bn1", b.width)
+                out.append((p + ".conv2.weight", (b.width, b.width, 3, 3), "conv_w"))
+                out += _bn_entries(p + ".bn2", b.width)
+                out.append((p + ".conv3.weight", (b.cout, b.width, 1, 1), "conv_w"))
                 out += _bn_entries(p + ".bn3", b.cout)
             if b.downsample:
-                out.append((p + ".downsample.0.weight", (b.cout, b.cin, 1, 1), "conv_w"))
-                out += _bn_entries(p + ".downsample.1", b.cout)
+                # downsample_avg puts the pool (nn.Identity at stride 1: no keys) at index 0, resnet.py:263-277
+                i = 1 if b.avg_down else 0
+                out.append((p + ".downsample.%d.weight" % i, (b.cout, b.cin, 1, 1), "conv_w"))
+                out += _bn_entries(p + ".downsample.%d" % (i + 1), b.cout)
         out.append(("fc.weight", (spec.num_classes, spec.pooled_features), "fc_w"))
         out.append(("fc.bias", (spec.num_classes,), "fc_b"))
     return out

@@ -1030,6 +1030,93 @@ __global__ void relu_bn_bwd_reduce_drop_kernel(const T* __restrict__ g, const T*
 
 static size_t reduce_smem(const RowGeom& g) { return (size_t)g.block.x * 8 * g.block.y * sizeof(float); }
 
+// ---------------------------------------------------------------------------------------------
+// 2x2 / stride-2 average pool of the ResNet-D shortcut: nn.AvgPool2d(2, 2, ceil_mode=True, count_include_pad=False)
+// (resnet.py:263-277). Ho = ceil(H/2), Wo = ceil(W/2); a window clipped by an odd extent averages its 2 or 1 in-image
+// values. The count is 4, 2 or 1, so dividing by it is exact in fp32 and each output is rounded once.
+// Row geometry: a row is one output pixel (forward) or one input pixel (backward).
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ float avgpool2_inv_count(int oy, int ox, int H, int W) {
+    const int ch = 2 * oy + 1 < H ? 2 : 1, cw = 2 * ox + 1 < W ? 2 : 1;
+    return 1.0f / (float)(ch * cw);
+}
+
+// y = round16(((x00 + x01) + x10) + x11) * (1 / count)), the terms in row-major order, out-of-image ones left out
+template <typename T>
+__global__ void avgpool2_fwd_kernel(const T* __restrict__ x, T* __restrict__ y, int H, int W, int Wo, long long hwo,
+                                   int rows_per_block) {
+    const int V = blockDim.x, C = V * 8;
+    const int c0 = threadIdx.x * 8;
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    long long r1 = r0 + rows_per_block;
+    if (r1 > hwo) r1 = hwo;
+    const T* img = x + (size_t)blockIdx.y * H * W * C + c0;
+    T* out = y + (size_t)blockIdx.y * hwo * C + c0;
+    for (long long r = r0 + threadIdx.y; r < r1; r += blockDim.y) {
+        const int oy = (int)(r / Wo), ox = (int)(r - (long long)oy * Wo);
+        const int iy = 2 * oy, ix = 2 * ox;
+        const bool right = ix + 1 < W, below = iy + 1 < H;
+        uint4 raw[4];
+        raw[0] = ldg16(img + ((size_t)iy * W + ix) * C);
+        if (right) raw[1] = ldg16(img + ((size_t)iy * W + ix + 1) * C);
+        if (below) raw[2] = ldg16(img + ((size_t)(iy + 1) * W + ix) * C);
+        if (right && below) raw[3] = ldg16(img + ((size_t)(iy + 1) * W + ix + 1) * C);
+        float s[8], f[8];
+        unpack8<T>(raw[0], s);
+        if (right) {
+            unpack8<T>(raw[1], f);
+#pragma unroll
+            for (int i = 0; i < 8; i++) s[i] += f[i];
+        }
+        if (below) {
+            unpack8<T>(raw[2], f);
+#pragma unroll
+            for (int i = 0; i < 8; i++) s[i] += f[i];
+        }
+        if (right && below) {
+            unpack8<T>(raw[3], f);
+#pragma unroll
+            for (int i = 0; i < 8; i++) s[i] += f[i];
+        }
+        const float inv = avgpool2_inv_count(oy, ox, H, W);
+#pragma unroll
+        for (int i = 0; i < 8; i++) s[i] *= inv;
+        stg16(out + (size_t)r * C, pack8<T>(s));
+    }
+}
+
+// dx = round16(add + dy[y/2, x/2] * (1 / count)); add == NULL reads as zero. Every dx element is written by one thread
+// that reads add at the same address first, so add may be dx itself.
+template <typename T>
+__global__ void avgpool2_bwd_add_kernel(const T* __restrict__ dy, const T* add, T* dx, int H, int W, int Ho, int Wo,
+                                        int rows_per_block) {
+    const int V = blockDim.x, C = V * 8;
+    const int c0 = threadIdx.x * 8;
+    const long long hw = (long long)H * W;
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    long long r1 = r0 + rows_per_block;
+    if (r1 > hw) r1 = hw;
+    const T* g = dy + (size_t)blockIdx.y * Ho * Wo * C + c0;
+    const size_t img = (size_t)blockIdx.y * hw * C + c0;
+    for (long long r = r0 + threadIdx.y; r < r1; r += blockDim.y) {
+        const int iy = (int)(r / W), ix = (int)(r - (long long)iy * W);
+        const int oy = iy >> 1, ox = ix >> 1;
+        float f[8];
+        unpack8<T>(ldg16(g + ((size_t)oy * Wo + ox) * C), f);
+        const float inv = avgpool2_inv_count(oy, ox, H, W);
+        if (add) {
+            float a[8];
+            unpack8<T>(*reinterpret_cast<const uint4*>(add + img + (size_t)r * C), a);
+#pragma unroll
+            for (int i = 0; i < 8; i++) f[i] = fmaf(f[i], inv, a[i]);
+        } else {
+#pragma unroll
+            for (int i = 0; i < 8; i++) f[i] *= inv;
+        }
+        stg16(dx + img + (size_t)r * C, pack8<T>(f));
+    }
+}
+
 }  // namespace
 
 // =============================================================================================
@@ -1405,6 +1492,28 @@ int dfd_add_inplace(void* a, const void* b, long long numel, int dt, void* strea
     if (blocks > DFD_SMS * 16) blocks = DFD_SMS * 16;
     cudaStream_t st = (cudaStream_t)stream;
     DISPATCH_T(dt, (add_inplace_kernel<T><<<blocks, 256, 0, st>>>((T*)a, (const T*)b, nvec)));
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+int dfd_avgpool2_fwd(const void* x, void* y, int N, int H, int W, int C, int dt, void* stream) {
+    if (C % 8 || C <= 0 || C > 8192 || N <= 0 || H <= 0 || W <= 0)
+        return dfd_set_error(DFD_ERR_ARG, "dfd_avgpool2_fwd: C%8, C <= 8192, sizes");
+    const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;
+    RowGeom g = make_geom(C, (long long)Ho * Wo, N);
+    DISPATCH_T(dt, (avgpool2_fwd_kernel<T><<<g.grid, g.block, 0, (cudaStream_t)stream>>>((const T*)x, (T*)y, H, W, Wo,
+                                                                                        (long long)Ho * Wo, g.rows_per_block)));
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+int dfd_avgpool2_bwd_add(const void* dy, const void* add, void* dx, int N, int H, int W, int C, int dt, void* stream) {
+    if (C % 8 || C <= 0 || C > 8192 || N <= 0 || H <= 0 || W <= 0)
+        return dfd_set_error(DFD_ERR_ARG, "dfd_avgpool2_bwd_add: C%8, C <= 8192, sizes");
+    const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;
+    RowGeom g = make_geom(C, (long long)H * W, N);
+    DISPATCH_T(dt, (avgpool2_bwd_add_kernel<T><<<g.grid, g.block, 0, (cudaStream_t)stream>>>((const T*)dy, (const T*)add, (T*)dx,
+                                                                                            H, W, Ho, Wo, g.rows_per_block)));
     DFD_LAUNCH_CHECK();
     return DFD_OK;
 }

@@ -1,7 +1,14 @@
-"""Kernel plan of the ResNet family (resnet18 / resnet50) for `Engine` — host side only.
+"""Kernel plan of the dense ResNet family (resnet18/26/34/50/101/152, tv_*, wide_*, resnet26d / resnet50d) for `Engine` — host
+side only.
 
 Reference graph: dfd/timm/models/resnet.py:450-468 (stem 7x7 s2 -> BN -> ReLU -> maxpool 3x3 s2 -> 4 stages -> GAP
--> fc), BasicBlock :150-175, Bottleneck :215-246 (stride on the 3x3, :195-197), downsample 1x1 conv + BN :249-260.
+-> fc), BasicBlock :150-175, Bottleneck :215-246 (stride on the 3x3, :195-197; width = planes * base_width / 64, :187),
+downsample 1x1 conv + BN :249-260.
+
+ResNet-D (resnet26d, resnet50d): the deep stem (3x3 s2 -> BN -> ReLU -> 3x3 -> BN -> ReLU -> 3x3, :365-377) runs its first
+convolution through the stem im2col + GEMM and the two 32-channel 3x3 convolutions through the explicit im2col route below;
+the average-pool shortcut (downsample_avg, :263-277) pools with `dfd_avgpool2_fwd` in front of a stride-1 1x1 GEMM, and its
+backward adds the pooled gradient into the main-path gradient in one pass (`dfd_avgpool2_bwd_add`).
 
 With gemm_impl="tc" every 3x3 convolution runs as an IMPLICIT GEMM on wgmma (`dfd_conv_tc`, csrc/gemm_tc.cu conv mode: the
 TMA producer fetches the input box shifted by the tap through a 4-D tensor map, no im2col matrix in memory), and so does the
@@ -60,6 +67,12 @@ def drop_block_desc(mask, noise, kept, gamma, N, H, W, C, cb, stream):
     return struct.pack("<QQQdiiiiiiii", mask, noise or 0, kept, gamma, N, H, W, C, cb, stream, 0, 0)
 
 
+def ds_names(b):
+    """(conv weight, BN prefix) of a block's downsample branch, relative to the block: downsample_conv is [conv, BN]; downsample_avg
+    is [pool, conv, BN] (resnet.py:249-277)"""
+    return (".downsample.1.weight", ".downsample.2") if b.avg_down else (".downsample.0.weight", ".downsample.1")
+
+
 def build_resnet(e):
     spec, N, dev, dt = e.spec, e.N, e.device, e.dt
     e._keep = []
@@ -70,7 +83,7 @@ def build_resnet(e):
     pk_off, off = {}, 0
     for n in e.param_names:
         o, s, k = e.p_off[n]
-        if len(s) == 4 and s[2] > 1 and not n.startswith("conv1."):
+        if len(s) == 4 and s[2] > 1 and n not in ("conv1.weight", "conv1.0.weight"):    # not the stem-GEMM weights
             pk_off[n] = (off, s[0], s[1], s[2])
             off += (k + 7) // 8 * 8
     ar = e.arena        # the packed layouts depend on the parameter shapes only: owned and refreshed by the arena engine
@@ -98,8 +111,17 @@ def build_resnet(e):
     PKT = lambda n: _ptr(e.wpackT16, pk_off[n][0])
     PKD = lambda n: _ptr(e.wpackD16, pk_off[n][0])
 
+    deep = spec.stem_type == "deep"
+    if deep and e.stem_impl != "gemm":
+        raise ValueError("stem_impl=%r: the deep stem's first convolution is planned through dfd_stem_im2col (stem_impl='gemm')"
+                         % (e.stem_impl,))
+    sw = spec.stem_width
+
     # ---- shapes ------------------------------------------------------------------------------------------
-    H1, W1 = conv_out(e.H, 7, 2, 3), conv_out(e.W, 7, 2, 3)
+    if deep:
+        H1, W1 = conv_out(e.H, 3, 2, 1), conv_out(e.W, 3, 2, 1)
+    else:
+        H1, W1 = conv_out(e.H, 7, 2, 3), conv_out(e.W, 7, 2, 3)
     H2, W2 = conv_out(H1, 3, 2, 1), conv_out(W1, 3, 2, 1)
     shapes = []
     h, w = H2, W2
@@ -110,14 +132,14 @@ def build_resnet(e):
     Hf, Wf = h, w
 
     # ---- BN arenas ---------------------------------------------------------------------------------------
-    bn_specs = [("bn1", 64)]
+    bn_specs = ([("conv1.1", sw), ("conv1.4", sw)] if deep else []) + [("bn1", 64)]
     for b in spec.blocks:
         if b.kind == "basic":
             bn_specs += [(b.name + ".bn1", b.planes), (b.name + ".bn2", b.cout)]
         else:
-            bn_specs += [(b.name + ".bn1", b.planes), (b.name + ".bn2", b.planes), (b.name + ".bn3", b.cout)]
+            bn_specs += [(b.name + ".bn1", b.width), (b.name + ".bn2", b.width), (b.name + ".bn3", b.cout)]
         if b.downsample:
-            bn_specs.append((b.name + ".downsample.1", b.cout))
+            bn_specs.append((b.name + ds_names(b)[1], b.cout))
     e._alloc_bn(bn_specs)
     bns = e.bns
 
@@ -146,7 +168,7 @@ def build_resnet(e):
             if b.kind == "basic":
                 dims = [("bn1", ho, wo, b.planes), ("bn2", ho, wo, b.cout)]
             else:       # the stride is on conv2: bn1 runs at the block's input resolution
-                dims = [("bn1", h, w, b.planes), ("bn2", ho, wo, b.planes), ("bn3", ho, wo, b.cout)]
+                dims = [("bn1", h, w, b.width), ("bn2", ho, wo, b.width), ("bn3", ho, wo, b.cout)]
             for bn_name, hh, ww, C in dims:
                 name = b.name + "." + bn_name
                 sites[name] = (hh, ww, C) + drop_block_geometry(name, hh, ww, db_rate, gs)
@@ -181,10 +203,10 @@ def build_resnet(e):
         return ("dfd_bn_act", (_ptr(y), bn.scale, bn.shift, None, None, _ptr(out), N, hw, C, ACT_RELU, 0, dt))
 
     # ---- scratch -----------------------------------------------------------------------------------------
-    max_act = max([N * H1 * W1 * 64] + [N * hh * ww * max(b.cin, b.planes) for b, hh, ww, ho, wo in shapes] +
+    max_act = max([N * H1 * W1 * 64] + [N * hh * ww * max(b.cin, b.width) for b, hh, ww, ho, wo in shapes] +
                   [N * ho * wo * b.cout for b, hh, ww, ho, wo in shapes])
-    max_cols = max([N * ho * wo * 9 * (b.cin if b.kind == "basic" else b.planes) for b, hh, ww, ho, wo in shapes] +
-                   [N * ho * wo * 9 * b.planes for b, hh, ww, ho, wo in shapes])
+    max_cols = max([N * ho * wo * 9 * (b.cin if b.kind == "basic" else b.width) for b, hh, ww, ho, wo in shapes] +
+                   [N * ho * wo * 9 * b.width for b, hh, ww, ho, wo in shapes] + ([N * H1 * W1 * 9 * sw] if deep else []))
     e.gbuf = [e._alloc16(max_act) for _ in range(6)]
     e.cols = e._alloc16(max_cols)
     COLS = _ptr(e.cols)
@@ -197,7 +219,21 @@ def build_resnet(e):
     x0 = e._alloc16(N, H2, W2, 64)
     e.pool_idx = torch.zeros(N * H2 * W2 * 64, dtype=torch.uint8, device=dev)
     bn0 = bns["bn1"]
-    if e.stem_impl == "gemm":
+    if deep:
+        # conv1.0 (3x3 s2, in_chans -> sw) as im2col + GEMM, conv1.3 / conv1.6 (Cin = sw) through conv3x3's im2col route
+        bs0, bs1 = bns["conv1.1"], bns["conv1.4"]
+        ys0, as0 = e._alloc16(N, H1, W1, sw), e._alloc16(N, H1, W1, sw)
+        ys1, as1 = e._alloc16(N, H1, W1, sw), e._alloc16(N, H1, W1, sw)
+        taps, Kp = e._stem_gemm_setup("conv1.0.weight", sw, 3, N * H1 * W1)
+        fwd.append(("dfd_stem_im2col", (_ptr(e.x_in), _ptr(e.stem_cols), N, spec.in_chans, e.H, e.W, 3, 2, 1, Kp, dt)))
+        fwd.append(gemm(_ptr(e.stem_cols), _ptr(e.stem_wpad), _ptr(ys0), N * H1 * W1, sw, Kp, bs0))
+        fwd += finalize(bs0, N * H1 * W1)
+        fwd.append(bn_relu(ys0, bs0, as0, H1 * W1, sw))
+        fwd += conv3x3(_ptr(as0), "conv1.3.weight", _ptr(ys1), H1, W1, sw, sw, 1, bs1)
+        fwd += finalize(bs1, N * H1 * W1)
+        fwd.append(bn_relu(ys1, bs1, as1, H1 * W1, sw))
+        fwd += conv3x3(_ptr(as1), "conv1.6.weight", _ptr(y0), H1, W1, sw, 64, 1, bn0)
+    elif e.stem_impl == "gemm":
         taps, Kp = e._stem_gemm_setup("conv1.weight", 64, 7, N * H1 * W1)
         fwd.append(("dfd_stem_im2col", (_ptr(e.x_in), _ptr(e.stem_cols), N, spec.in_chans, e.H, e.W, 7, 2, 3, Kp, dt)))
         fwd.append(gemm(_ptr(e.stem_cols), _ptr(e.stem_wpad), _ptr(y0), N * H1 * W1, 64, Kp, bn0))
@@ -227,40 +263,47 @@ def build_resnet(e):
             rec.update(y1=y1, a1=a1, ylast=y2, bnlast=bn2, site_last=p + ".bn2")
         else:
             bn1, bn2, bn3 = bns[p + ".bn1"], bns[p + ".bn2"], bns[p + ".bn3"]
-            y1 = e._alloc16(N, h, w, b.planes)
-            a1 = e._alloc16(N, h, w, b.planes)
-            y2 = e._alloc16(N, ho, wo, b.planes)
-            a2 = e._alloc16(N, ho, wo, b.planes)
+            y1 = e._alloc16(N, h, w, b.width)
+            a1 = e._alloc16(N, h, w, b.width)
+            y2 = e._alloc16(N, ho, wo, b.width)
+            a2 = e._alloc16(N, ho, wo, b.width)
             y3 = e._alloc16(N, ho, wo, b.cout)
-            fwd.append(gemm(_ptr(x), P16(p + ".conv1.weight"), _ptr(y1), M1, b.planes, b.cin, bn1))
+            fwd.append(gemm(_ptr(x), P16(p + ".conv1.weight"), _ptr(y1), M1, b.width, b.cin, bn1))
             fwd += finalize(bn1, M1)
-            fwd.append(bn_relu(y1, bn1, a1, h * w, b.planes, p + ".bn1"))
-            fwd += conv3x3(_ptr(a1), p + ".conv2.weight", _ptr(y2), h, w, b.planes, b.planes, b.stride, bn2)
+            fwd.append(bn_relu(y1, bn1, a1, h * w, b.width, p + ".bn1"))
+            fwd += conv3x3(_ptr(a1), p + ".conv2.weight", _ptr(y2), h, w, b.width, b.width, b.stride, bn2)
             fwd += finalize(bn2, M2)
-            fwd.append(bn_relu(y2, bn2, a2, ho * wo, b.planes, p + ".bn2"))
-            fwd.append(gemm(_ptr(a2), P16(p + ".conv3.weight"), _ptr(y3), M2, b.cout, b.planes, bn3))
+            fwd.append(bn_relu(y2, bn2, a2, ho * wo, b.width, p + ".bn2"))
+            fwd.append(gemm(_ptr(a2), P16(p + ".conv3.weight"), _ptr(y3), M2, b.cout, b.width, bn3))
             fwd += finalize(bn3, M2)
             rec.update(y1=y1, a1=a1, y2=y2, a2=a2, ylast=y3, bnlast=bn3, site_last=p + ".bn3")
         res = x
         if b.downsample:
-            bnd = bns[p + ".downsample.1"]
+            dsw, dsbn = [p + n for n in ds_names(b)]
+            bnd = bns[dsbn]
             yd = e._alloc16(N, ho, wo, b.cout)
             r = e._alloc16(N, ho, wo, b.cout)
             if b.stride == 1:
                 xs = x
-                fwd.append(gemm(_ptr(xs), P16(p + ".downsample.0.weight"), _ptr(yd), M2, b.cout, b.cin, bnd))
+                fwd.append(gemm(_ptr(xs), P16(dsw), _ptr(yd), M2, b.cout, b.cin, bnd))
+            elif b.avg_down:
+                # ResNet-D: 2x2 average pool (ceil_mode, count_include_pad=False), then the stride-1 1x1 convolution; the pooled
+                # input is kept for the weight gradient
+                xs = e._alloc16(N, ho, wo, b.cin)
+                fwd.append(("dfd_avgpool2_fwd", (_ptr(x), _ptr(xs), N, h, w, b.cin, dt)))
+                fwd.append(gemm(_ptr(xs), P16(dsw), _ptr(yd), M2, b.cout, b.cin, bnd))
             elif implicit and b.cin % 64 == 0 and b.cout % 64 == 0:
                 # strided 1x1 convolution straight from the block input (k = 1, stride 2 implicit GEMM): no gathered copy
                 xs = None
-                fwd.append(("dfd_conv_tc", (_ptr(x), P16(p + ".downsample.0.weight"), _ptr(yd), N, h, w, b.cin, b.cout, 1, b.stride, dt)
+                fwd.append(("dfd_conv_tc", (_ptr(x), P16(dsw), _ptr(yd), N, h, w, b.cin, b.cout, 1, b.stride, dt)
                             + e._stats(bnd) + (None,)))
             else:
                 xs = e._alloc16(N, ho, wo, b.cin)
                 fwd.append(("dfd_im2col", (_ptr(x), _ptr(xs), N, h, w, b.cin, 1, b.stride, 0, dt)))
-                fwd.append(gemm(_ptr(xs), P16(p + ".downsample.0.weight"), _ptr(yd), M2, b.cout, b.cin, bnd))
+                fwd.append(gemm(_ptr(xs), P16(dsw), _ptr(yd), M2, b.cout, b.cin, bnd))
             fwd += finalize(bnd, M2)
             fwd.append(("dfd_bn_act", (_ptr(yd), bnd.scale, bnd.shift, None, None, _ptr(r), N, ho * wo, b.cout, ACT_NONE, 0, dt)))
-            rec.update(yd=yd, xs=xs, bnd=bnd)
+            rec.update(yd=yd, xs=xs, bnd=bnd, dsw=dsw)
             res = r
         out = e._alloc16(N, ho, wo, b.cout)
         bl = rec["bnlast"]
@@ -393,41 +436,48 @@ def build_resnet(e):
         else:
             bn1, bn2 = bns[p + ".bn1"], bns[p + ".bn2"]
             # conv3 (1x1): dy3 = t1 -> da2 = t2
-            bwd.append(gemm(t1, T16(p + ".conv3.weight"), t2, M2, b.planes, b.cout))
-            bwd.append(e._wgrad(t1, _ptr(rec["a2"]), G32(p + ".conv3.weight"), M2, b.cout, b.planes))
-            bwd.append(relu_bwd(t2, rec["y2"], bn2, t1, ho * wo, b.planes, p + ".bn2"))
+            bwd.append(gemm(t1, T16(p + ".conv3.weight"), t2, M2, b.width, b.cout))
+            bwd.append(e._wgrad(t1, _ptr(rec["a2"]), G32(p + ".conv3.weight"), M2, b.cout, b.width))
+            bwd.append(relu_bwd(t2, rec["y2"], bn2, t1, ho * wo, b.width, p + ".bn2"))
             bwd += bwd_finalize(bn2, M2)
-            bwd.append(("dfd_bn_bwd_apply", (t1, _ptr(rec["y2"]), None, bn2.cA, bn2.cB, bn2.cC, t2, N, ho * wo, b.planes, dt)))
-            # conv2 (3x3 stride s): dy2 = t2 -> da1 = t1 [M1, planes]
-            bwd += conv3x3_bwd(p + ".conv2.weight", t2, M2, b.planes, b.planes, rec["a1"], h, w, b.stride, t1)
-            bwd.append(relu_bwd(t1, rec["y1"], bn1, t2, h * w, b.planes, p + ".bn1"))
+            bwd.append(("dfd_bn_bwd_apply", (t1, _ptr(rec["y2"]), None, bn2.cA, bn2.cB, bn2.cC, t2, N, ho * wo, b.width, dt)))
+            # conv2 (3x3 stride s): dy2 = t2 -> da1 = t1 [M1, width]
+            bwd += conv3x3_bwd(p + ".conv2.weight", t2, M2, b.width, b.width, rec["a1"], h, w, b.stride, t1)
+            bwd.append(relu_bwd(t1, rec["y1"], bn1, t2, h * w, b.width, p + ".bn1"))
             bwd += bwd_finalize(bn1, M1)
-            bwd.append(("dfd_bn_bwd_apply", (t2, _ptr(rec["y1"]), None, bn1.cA, bn1.cB, bn1.cC, t1, N, h * w, b.planes, dt)))
+            bwd.append(("dfd_bn_bwd_apply", (t2, _ptr(rec["y1"]), None, bn1.cA, bn1.cB, bn1.cC, t1, N, h * w, b.width, dt)))
             # conv1 (1x1): dy1 = t1 -> dx = t3 [M1, cin]
-            bwd.append(gemm(t1, T16(p + ".conv1.weight"), t3, M1, b.cin, b.planes))
-            bwd.append(e._wgrad(t1, _ptr(xin), G32(p + ".conv1.weight"), M1, b.planes, b.cin))
+            bwd.append(gemm(t1, T16(p + ".conv1.weight"), t3, M1, b.cin, b.width))
+            bwd.append(e._wgrad(t1, _ptr(xin), G32(p + ".conv1.weight"), M1, b.width, b.cin))
         # identity / downsample path: gradient gm flows to the block input too
         if b.downsample:
             bnd = rec["bnd"]
             bwd.append(("dfd_bn_bwd_reduce", (gm, _ptr(rec["yd"]), None, bnd.mean, bnd.rstd, N, ho * wo, b.cout, dt, bnd.bs1, bnd.bs2, None)))
             bwd += bwd_finalize(bnd, M2)
             bwd.append(("dfd_bn_bwd_apply", (gm, _ptr(rec["yd"]), None, bnd.cA, bnd.cB, bnd.cC, t1, N, ho * wo, b.cout, dt)))
-            ds_add = implicit and b.cin % 64 == 0 and b.cout % 64 == 0
+            pooled = b.avg_down and b.stride != 1
+            ds_add = implicit and b.cin % 64 == 0 and b.cout % 64 == 0 and not pooled
+            dsw = rec["dsw"]
             if ds_add:
                 # the downsample input gradient is ADDED into t3 (main-path gradient) by the GEMM's own epilogue: a TMA reduction
                 # store through the stride-s pixel view of t3 - no scratch tensor, no col2im scatter / add pass
-                bwd.append(("dfd_conv1x1_dgrad_add", (t1, T16(p + ".downsample.0.weight"), t3, N, h, w, b.cin, b.cout, b.stride, dt)))
+                bwd.append(("dfd_conv1x1_dgrad_add", (t1, T16(dsw), t3, N, h, w, b.cin, b.cout, b.stride, dt)))
             else:
-                bwd.append(gemm(t1, T16(p + ".downsample.0.weight"), t2, M2, b.cin, b.cout))
+                bwd.append(gemm(t1, T16(dsw), t2, M2, b.cin, b.cout))
             if rec["xs"] is None:      # strided 1x1: implicit weight gradient on the block input itself
-                bwd.append(e._wgrad_conv(t1, _ptr(xin), G32(p + ".downsample.0.weight"), N, h, w, b.cin, b.cout, 1, b.stride))
+                bwd.append(e._wgrad_conv(t1, _ptr(xin), G32(dsw), N, h, w, b.cin, b.cout, 1, b.stride))
             else:
-                bwd.append(e._wgrad(t1, _ptr(rec["xs"]), G32(p + ".downsample.0.weight"), M2, b.cout, b.cin))
+                bwd.append(e._wgrad(t1, _ptr(rec["xs"]), G32(dsw), M2, b.cout, b.cin))
             if ds_add:
                 new_dout = (t3, None)
             elif b.stride == 1:
                 bwd.append(("dfd_add_inplace", (t3, t2, M1 * b.cin, dt)))
                 new_dout = (t3, None)
+            elif pooled:
+                # spread the pooled gradient over each 2x2 window (/ its in-image count) and add the main-path gradient, into the
+                # old dout buffer (consumed by the reduction above)
+                bwd.append(("dfd_avgpool2_bwd_add", (t2, t3, dout, N, h, w, b.cin, dt)))
+                new_dout = (dout, None)
             else:
                 # scatter the strided gradient back onto the input grid and add the main-path gradient (the old dout buffer
                 # has been consumed by the reduction above: reused as the destination)
@@ -445,7 +495,24 @@ def build_resnet(e):
     bwd.append(("dfd_act_bwd", (t1, _ptr(y0), bn0.scale, bn0.shift, bn0.mean, bn0.rstd, None, None, t2, N, H1 * W1, 64,
                                 ACT_RELU, dt, bn0.bs1, bn0.bs2, None)))
     bwd += bwd_finalize(bn0, N * H1 * W1)
-    if e.stem_impl == "gemm":
+    if deep:
+        M0 = N * H1 * W1
+        bwd.append(("dfd_bn_bwd_apply", (t2, _ptr(y0), None, bn0.cA, bn0.cB, bn0.cC, t1, N, H1 * W1, 64, dt)))
+        # conv1.6 and conv1.3 take the two packed-gradient regions; conv1.0's gradient goes through the padded stem buffer.
+        # One ordered reduce for the three, then the unpack / unpad passes.
+        bwd += conv3x3_bwd("conv1.6.weight", t1, M0, sw, 64, as1, H1, W1, 1, t2)
+        bwd.append(relu_bwd(t2, ys1, bs1, t1, H1 * W1, sw, None))
+        bwd += bwd_finalize(bs1, M0)
+        bwd.append(("dfd_bn_bwd_apply", (t1, _ptr(ys1), None, bs1.cA, bs1.cB, bs1.cC, t2, N, H1 * W1, sw, dt)))
+        bwd += conv3x3_bwd("conv1.3.weight", t2, M0, sw, sw, as0, H1, W1, 1, t1)
+        bwd.append(relu_bwd(t1, ys0, bs0, t2, H1 * W1, sw, None))
+        bwd += bwd_finalize(bs0, M0)
+        bwd.append(("dfd_bn_bwd_apply", (t2, _ptr(ys0), None, bs0.cA, bs0.cB, bs0.cC, t1, N, H1 * W1, sw, dt)))
+        bwd.append(("dfd_memset_async", (_ptr(e.stem_gpad), 0, sw * Kp * 4)))
+        bwd.append(e._wgrad(t1, _ptr(e.stem_cols), _ptr(e.stem_gpad), M0, sw, Kp))
+        flush_block(bwd)
+        bwd.append(("dfd_unpad_grad", (_ptr(e.stem_gpad), G32("conv1.0.weight"), sw, taps, Kp)))
+    elif e.stem_impl == "gemm":
         bwd.append(("dfd_bn_bwd_apply", (t2, _ptr(y0), None, bn0.cA, bn0.cB, bn0.cC, t1, N, H1 * W1, 64, dt)))
         bwd.append(("dfd_memset_async", (_ptr(e.stem_gpad), 0, 64 * Kp * 4)))
         bwd.append(e._wgrad(t1, _ptr(e.stem_cols), _ptr(e.stem_gpad), N * H1 * W1, 64, Kp))

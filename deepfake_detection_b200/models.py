@@ -18,12 +18,14 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .arch import SUPPORTED_ARCHS, TF_ARCHS, TF_POOL_CROP, get_spec, state_entries
+from .arch import RESNET_ARCHS, SUPPORTED_ARCHS, TF_ARCHS, TF_POOL_CROP, get_spec, state_entries
 from .engine import Engine
 
 _DEFAULT_CFG = dict(num_classes=1000, pool_size=(7, 7), crop_pct=0.875, interpolation="bicubic",
                     mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225))
 _INCEPTION_MEAN_STD = dict(mean=(0.5, 0.5, 0.5), std=(0.5, 0.5, 0.5))      # the AdvProp (_ap) checkpoints' normalisation
+# resnet.py:22-58: bilinear unless the entry says bicubic
+_RESNET_BICUBIC = ("resnet26", "resnet26d", "resnet50d")
 
 
 class _NativeForward(torch.autograd.Function):
@@ -133,6 +135,8 @@ class NativeModel(nn.Module):
             self.default_cfg.update(pool_size=pool_size, crop_pct=crop_pct)
             if arch.endswith("_ap"):
                 self.default_cfg.update(_INCEPTION_MEAN_STD)
+        if arch in RESNET_ARCHS:
+            self.default_cfg.update(interpolation="bicubic" if arch in _RESNET_BICUBIC else "bilinear")
         self._engines = OrderedDict()
         self._primary = None
         self._pending_state = None
@@ -266,7 +270,7 @@ def create_model(model_name, pretrained=False, num_classes=1000, in_chans=3, che
     """dfd/timm/models/factory.py:8-64 for the architectures on the native hot path."""
     if pretrained:
         raise _lib.NativeError("pretrained weights need network access; load a checkpoint instead")
-    if model_name not in SUPPORTED_ARCHS and model_name not in TF_ARCHS:
+    if model_name not in SUPPORTED_ARCHS and model_name not in TF_ARCHS and model_name not in RESNET_ARCHS:
         raise RuntimeError("Unknown model (%s)" % model_name)       # factory.py:56
     model = NativeModel(model_name, num_classes=num_classes, in_chans=in_chans, **kwargs)
     if checkpoint_path:

@@ -241,6 +241,14 @@ int dfd_act_bwd_gpool(const void* y, const float* scale, const float* shift, con
                       const float* dpooled, const int* argmax, void* gu, int n, long long hw, int C, int act, int pool_type,
                       int dt, double* s1, double* s2, const void* fin, void* stream);
 int dfd_add_inplace(void* a, const void* b, long long numel, int dt, void* stream);
+/* 2x2 / stride-2 average pool of the ResNet-D shortcut, nn.AvgPool2d(2, 2, ceil_mode=True, count_include_pad=False)
+ * (resnet.py:263-277), NHWC 16-bit: x [N,H,W,C] -> y [N,ceil(H/2),ceil(W/2),C]. Each output is the fp32 sum of the in-image
+ * values of its window, in row-major order, times 1 / count (count 4, 2 or 1: a window clipped by an odd extent averages
+ * the values it holds), rounded once. C % 8 == 0, C <= 8192. */
+int dfd_avgpool2_fwd(const void* x, void* y, int N, int H, int W, int C, int dt, void* stream);
+/* its input gradient, added to a second source: dx[n,y,x,c] = round16(add[n,y,x,c] + dy[n,y/2,x/2,c] / count(y/2, x/2)).
+ * add may be NULL (zero) or dx itself. Elementwise, no atomics. H, W = INPUT extents. */
+int dfd_avgpool2_bwd_add(const void* dy, const void* add, void* dx, int N, int H, int W, int C, int dt, void* stream);
 
 /* ---- squeeze-excite FCs: SqueezeExcite.forward, efficientnet_blocks.py:104-110 ------------------------ */
 int dfd_se_fc_fwd(const float* pooled, const float* Wr, const float* br, const float* We, const float* be,
