@@ -37,6 +37,7 @@ SIGNATURES = {
     "dfd_dwconv_block_channels": "i",
     "dfd_dwconv_fwd_pad": "ppppp" "iiiiiiii" "ii" "ppp" "p",
     "dfd_dwconv_bwd_pad": "ppppp" "pppppp" "ppp" "iiiiiiii" "i" "pp" "pl" "p" "p",
+    "dfd_dwconv_bwd_relu": "ppppp" "pppppp" "ppp" "iiiiii" "i" "pp" "pl" "p" "p",
     "dfd_stem_fwd": "ppp" "iiiiiiii" "i" "ppp",
     "dfd_stem_wgrad": "ppppppp" "iiiiiiii" "i" "p",
     "dfd_colstats": "p" "ili" "i" "ppp",
@@ -54,6 +55,8 @@ SIGNATURES = {
     "dfd_add_inplace": "pp" "li" "p",
     "dfd_avgpool2_fwd": "pp" "iiii" "i" "p",
     "dfd_avgpool2_bwd_add": "ppp" "iiii" "i" "p",
+    "dfd_bn_maxpool_add": "pppppp" "pp" "iiii" "i" "p",
+    "dfd_maxpool_bn_bwd_reduce": "pppppp" "iiii" "i" "pp" "p",
     "dfd_se_fc_fwd": "pppppp" "iii" "p",
     "dfd_se_fc_bwd": "pppppp" "pppppppp" "iii" "p",
     "dfd_se_fc_wgrad": "pppp" "pppp" "iii" "p",

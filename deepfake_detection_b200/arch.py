@@ -17,6 +17,7 @@ BASELINE.json names; it builds no modules and owns no tensors.
   * ResNet-18/50 layout: dfd/timm/models/resnet.py:115-260,280-468,472,523
   * ResNet-26/34/101/152, tv_*, wide_* (base_width 128) and ResNet-D (deep stem, downsample_avg): resnet.py:187,263-277,
     349-439,483-625
+  * Xception: dfd/timm/models/xception.py (SeparableConv2d :58-69, Block :72-124, Xception :127-226)
 """
 import math
 import re
@@ -200,6 +201,73 @@ def _resnet_spec(arch, kind, layers, in_chans, num_classes, input_size, base_wid
 
 
 # ----------------------------------------------------------------------------------------------
+# Xception
+# ----------------------------------------------------------------------------------------------
+
+@dataclass
+class XBlock:
+    """One Xception `Block` (xception.py:72-124): separable convolutions, each followed by a BatchNorm, a max-pool 3x3 s2 p1
+    at the end of a strided block and a 1x1 convolution + BN shortcut where the shape changes."""
+    name: str            # 'block<i>'
+    cin: int
+    cout: int
+    stride: int
+    start_with_relu: bool
+    seps: List[Tuple[int, int, int]]     # (rep index of the SeparableConv2d, cin, cout); its BN is at rep index + 1
+
+    @property
+    def skip(self):
+        return self.cout != self.cin or self.stride != 1
+
+
+@dataclass
+class XceptionSpec:
+    arch: str
+    in_chans: int
+    blocks: List[XBlock]
+    num_features: int
+    num_classes: int
+    input_size: Tuple[int, int, int]
+    family: str = "xception"
+    global_pool: str = "avg"
+
+    @property
+    def pooled_features(self):
+        return self.num_features * pool_feat_mult(self.global_pool)
+
+
+def _xblock(i, cin, cout, reps, stride, start_with_relu=True, grow_first=True):
+    """rep indices count the ReLU modules (xception.py:89-110): every separable convolution follows a ReLU, except the
+    first one of a block that does not start with a ReLU (block1)"""
+    chans = [(cin, cout)] + [(cout, cout)] * (reps - 1) if grow_first else [(cin, cin)] * (reps - 1) + [(cin, cout)]
+    first = 1 if start_with_relu else 0
+    seps = [(first + 3 * j, ci, co) for j, (ci, co) in enumerate(chans)]
+    return XBlock("block%d" % i, cin, cout, stride, start_with_relu, seps)
+
+
+def _xception_spec(arch, in_chans, num_classes):
+    blocks = [_xblock(1, 64, 128, 2, 2, start_with_relu=False), _xblock(2, 128, 256, 2, 2), _xblock(3, 256, 728, 2, 2)]
+    blocks += [_xblock(i, 728, 728, 3, 1) for i in range(4, 12)]
+    blocks.append(_xblock(12, 728, 1024, 2, 2, grow_first=False))
+    return XceptionSpec(arch=arch, in_chans=in_chans, blocks=blocks, num_features=2048, num_classes=num_classes,
+                        input_size=(3, 299, 299))
+
+
+def xception_extents(H, W):
+    """feature-map extents of Xception at input H x W: [(h, w)] after conv1, conv2 and every block (xception.py:183-200):
+    3x3 s2 p0, 3x3 p0, then (h - 1) // 2 + 1 per strided block (max-pool 3x3 s2 p1 and the 1x1 s2 shortcut agree)"""
+    h, w = conv_out(H, 3, 2, 0), conv_out(W, 3, 2, 0)
+    out = [(h, w)]
+    h, w = conv_out(h, 3, 1, 0), conv_out(w, 3, 1, 0)
+    out.append((h, w))
+    for b in _xception_spec("xception", 3, 2).blocks:
+        if b.stride != 1:
+            h, w = conv_out(h, 3, 2, 1), conv_out(w, 3, 2, 1)
+        out.append((h, w))
+    return out
+
+
+# ----------------------------------------------------------------------------------------------
 # registry of the variants on the hot path
 # ----------------------------------------------------------------------------------------------
 
@@ -243,6 +311,8 @@ def _base_spec(arch, num_classes, in_chans):
         kind, layers, base_width, deep = _RESNET_DEFS[arch]
         return _resnet_spec(arch, kind, layers, in_chans, num_classes, (3, 224, 224), base_width=base_width,
                             stem_type="deep" if deep else "", avg_down=deep)
+    if arch in XCEPTION_ARCHS:
+        return _xception_spec(arch, in_chans, num_classes)
     raise ValueError("arch %r is not on the native hot path (see SURVEY.md section 8)" % (arch,))
 
 
@@ -264,6 +334,8 @@ _RESNET_DEFS = {
     "resnet50d": ("bottleneck", (3, 4, 6, 3), 64, True),
 }
 RESNET_ARCHS = tuple(_RESNET_DEFS)
+
+XCEPTION_ARCHS = ("xception",)      # xception.py:229-237
 
 # TensorFlow-ported EfficientNets (efficientnet.py:1265-1530): the B0 generator with TF "SAME" padding and BatchNorm eps 1e-3.
 # _ap (AdvProp) and _ns (Noisy Student) share the plain variant's layers; only their default_cfg differs (models.py).
@@ -308,6 +380,11 @@ def _bn_entries(prefix, c):
             (prefix + ".num_batches_tracked", (), "bn_nbt")]
 
 
+def _sep_entries(prefix, cin, cout):
+    """SeparableConv2d (xception.py:58-69): depthwise 3x3 `conv1`, then 1x1 `pointwise`, neither with a bias"""
+    return [(prefix + ".conv1.weight", (cin, 1, 3, 3), "dw_w"), (prefix + ".pointwise.weight", (cout, cin, 1, 1), "conv_w")]
+
+
 def state_entries(spec):
     """[(name, shape, role)] in the reference's `state_dict()` order (params and buffers interleaved).
 
@@ -342,6 +419,25 @@ def state_entries(spec):
         out += _bn_entries("bn2", spec.num_features)
         out.append(("classifier.weight", (spec.num_classes, spec.pooled_features), "fc_w"))
         out.append(("classifier.bias", (spec.num_classes,), "fc_b"))
+    elif spec.family == "xception":
+        out.append(("conv1.weight", (32, spec.in_chans, 3, 3), "conv_w"))
+        out += _bn_entries("bn1", 32)
+        out.append(("conv2.weight", (64, 32, 3, 3), "conv_w"))
+        out += _bn_entries("bn2", 64)
+        for b in spec.blocks:
+            p = b.name
+            if b.skip:      # registered before `rep` (xception.py:75-80)
+                out.append((p + ".skip.weight", (b.cout, b.cin, 1, 1), "conv_w"))
+                out += _bn_entries(p + ".skipbn", b.cout)
+            for r, ci, co in b.seps:
+                out += _sep_entries("%s.rep.%d" % (p, r), ci, co)
+                out += _bn_entries("%s.rep.%d" % (p, r + 1), co)
+        out += _sep_entries("conv3", 1024, 1536)
+        out += _bn_entries("bn3", 1536)
+        out += _sep_entries("conv4", 1536, spec.num_features)
+        out += _bn_entries("bn4", spec.num_features)
+        out.append(("fc.weight", (spec.num_classes, spec.pooled_features), "fc_w"))
+        out.append(("fc.bias", (spec.num_classes,), "fc_b"))
     else:
         if spec.stem_type == "deep":
             # conv1 = Sequential(conv, bn, relu, conv, bn, relu, conv), resnet.py:370-377

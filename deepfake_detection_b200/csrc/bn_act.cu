@@ -1117,6 +1117,120 @@ __global__ void avgpool2_bwd_add_kernel(const T* __restrict__ dy, const T* add, 
     }
 }
 
+// Tail of a strided Xception block (xception.py:110-124): out = maxpool3x3s2p1(scale*y + shift) + (scale_s*ys + shift_s), the
+// pooled BatchNorm output never stored and the sum rounded to 16 bit once. Windows are padded with -inf (the BN output can be
+// negative); the arg-max is the first maximum in row-major window order (as dfd_maxpool_fwd and ATen), one byte per output,
+// and is not written when idx == NULL (eval mode). Rows are output pixels.
+template <typename T>
+__global__ void bn_maxpool_add_kernel(const T* __restrict__ y, const float* __restrict__ scale, const float* __restrict__ shift,
+                                      const T* __restrict__ ys, const float* __restrict__ scale_s,
+                                      const float* __restrict__ shift_s, T* __restrict__ out, unsigned char* __restrict__ idx,
+                                      int H, int W, int Wo, long long hwo, int rows_per_block) {
+    const int V = blockDim.x, C = V * 8;
+    const int c0 = threadIdx.x * 8;
+    float sc[8], sh[8], ss[8], hs[8];
+    ldg_f8(scale + c0, sc);
+    ldg_f8(shift + c0, sh);
+    ldg_f8(scale_s + c0, ss);
+    ldg_f8(shift_s + c0, hs);
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    long long r1 = r0 + rows_per_block;
+    if (r1 > hwo) r1 = hwo;
+    const T* x = y + (size_t)blockIdx.y * H * W * C + c0;
+    const size_t img = (size_t)blockIdx.y * hwo * C + c0;
+    for (long long r = r0 + threadIdx.y; r < r1; r += blockDim.y) {
+        const int oy = (int)(r / Wo), ox = (int)(r - (long long)oy * Wo);
+        float best[8], f[8];
+        unsigned char bi[8];
+#pragma unroll
+        for (int j = 0; j < 8; j++) { best[j] = -INFINITY; bi[j] = 0; }
+        for (int kh = 0; kh < 3; kh++) {
+            const int iy = oy * 2 - 1 + kh;
+            if (iy < 0 || iy >= H) continue;
+            for (int kw = 0; kw < 3; kw++) {
+                const int ix = ox * 2 - 1 + kw;
+                if (ix < 0 || ix >= W) continue;
+                unpack8<T>(ldg16(x + ((size_t)iy * W + ix) * C), f);
+#pragma unroll
+                for (int j = 0; j < 8; j++) {
+                    const float u = fmaf(f[j], sc[j], sh[j]);
+                    if (u > best[j]) { best[j] = u; bi[j] = (unsigned char)(kh * 3 + kw); }
+                }
+            }
+        }
+        unpack8<T>(ldg16(ys + img + (size_t)r * C), f);
+#pragma unroll
+        for (int j = 0; j < 8; j++) best[j] += fmaf(f[j], ss[j], hs[j]);
+        stg16(out + img + (size_t)r * C, pack8<T>(best));
+        if (idx) {
+            uint2 pk;
+            pk.x = bi[0] | (bi[1] << 8) | (bi[2] << 16) | (bi[3] << 24);
+            pk.y = bi[4] | (bi[5] << 8) | (bi[6] << 16) | (bi[7] << 24);
+            *reinterpret_cast<uint2*>(idx + img + (size_t)r * C) = pk;
+        }
+    }
+}
+
+// Backward of the pooled BatchNorm of bn_maxpool_add_kernel: gx[iy, ix] = round16(sum of gy over the (at most 2 x 2) windows
+// whose arg-max is (iy, ix)) - a gather, no atomics - and in the same pass the BN-backward sums s1 += gx, s2 += gx * xhat,
+// xhat = (y - mean) * rstd, of the rounded gx. Rows are input pixels.
+template <typename T>
+__global__ void maxpool_bn_bwd_reduce_kernel(const T* __restrict__ gy, const unsigned char* __restrict__ idx,
+                                             const T* __restrict__ y, const float* __restrict__ mean,
+                                             const float* __restrict__ rstd, T* __restrict__ gx, int H, int W, int Ho,
+                                             int Wo, int rows_per_block, double* __restrict__ s1, double* __restrict__ s2) {
+    extern __shared__ float sm[];
+    const int V = blockDim.x, C = V * 8;
+    const int c0 = threadIdx.x * 8;
+    float mu[8], rs[8], a1[8], a2[8];
+#pragma unroll
+    for (int i = 0; i < 8; i++) { a1[i] = 0.f; a2[i] = 0.f; }
+    ldg_f8(mean + c0, mu);
+    ldg_f8(rstd + c0, rs);
+    const long long hw = (long long)H * W;
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    long long r1 = r0 + rows_per_block;
+    if (r1 > hw) r1 = hw;
+    const size_t oimg = (size_t)blockIdx.y * Ho * Wo * C + c0;
+    const size_t img = (size_t)blockIdx.y * hw * C + c0;
+    for (long long r = r0 + threadIdx.y; r < r1; r += blockDim.y) {
+        const int iy = (int)(r / W), ix = (int)(r - (long long)iy * W);
+        float acc[8], f[8];
+#pragma unroll
+        for (int j = 0; j < 8; j++) acc[j] = 0.f;
+        for (int kh = 0; kh < 3; kh++) {        // window (oy, ox) holds the pixel at tap (iy + 1 - 2*oy, ix + 1 - 2*ox)
+            const int ay = iy + 1 - kh;
+            if (ay < 0 || (ay & 1) || (ay >> 1) >= Ho) continue;
+            for (int kw = 0; kw < 3; kw++) {
+                const int ax = ix + 1 - kw;
+                if (ax < 0 || (ax & 1) || (ax >> 1) >= Wo) continue;
+                const size_t o = oimg + ((size_t)(ay >> 1) * Wo + (ax >> 1)) * C;
+                const uint2 pk = *reinterpret_cast<const uint2*>(idx + o);
+                unpack8<T>(ldg16(gy + o), f);
+                const unsigned char want = (unsigned char)(kh * 3 + kw);
+#pragma unroll
+                for (int j = 0; j < 8; j++) {
+                    const unsigned char b = (unsigned char)(((j < 4 ? pk.x : pk.y) >> (8 * (j & 3))) & 0xff);
+                    if (b == want) acc[j] += f[j];
+                }
+            }
+        }
+        const uint4 pk = pack8<T>(acc);
+        stg16(gx + img + (size_t)r * C, pk);
+        unpack8<T>(pk, acc);
+        unpack8<T>(ldg16(y + img + (size_t)r * C), f);
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+            a1[i] += acc[i];
+            a2[i] = fmaf(acc[i], (f[i] - mu[i]) * rs[i], a2[i]);
+        }
+    }
+    double* p1 = stat_slot(s1, C);
+    double* p2 = stat_slot(s2, C);
+    reduce_rows_and_emit(sm, a1, [&](int c, float v) { atomicAdd(p1 + c, (double)v); });
+    reduce_rows_and_emit(sm, a2, [&](int c, float v) { atomicAdd(p2 + c, (double)v); });
+}
+
 }  // namespace
 
 // =============================================================================================
@@ -1401,26 +1515,33 @@ int dfd_act_bwd_gpool(const void* y, const float* scale, const float* shift, con
     if (!dpooled || !argmax) return dfd_set_error(DFD_ERR_ARG, "dfd_act_bwd_gpool: operands");
     if (pool_type != DFD_POOL_MAX && pool_type != DFD_POOL_AVGMAX && pool_type != DFD_POOL_CATAVGMAX)
         return dfd_set_error(DFD_ERR_ARG, "dfd_act_bwd_gpool: pool_type (avg: dfd_act_bwd)");
-    if (act != DFD_ACT_SWISH) return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_act_bwd_gpool: activation (Swish only)");
+    if (act != DFD_ACT_SWISH && act != DFD_ACT_RELU)
+        return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_act_bwd_gpool: activation (Swish or ReLU)");
     RowGeom g = make_geom(C, hw, n);
     cudaStream_t st = (cudaStream_t)stream;
     const float inv_hw = 1.f / (float)hw;
     const size_t smem_ab = reduce_smem(g) + (size_t)14 * g.block.x * sizeof(float4);     // + g_max, g_avg / hw, argmax
     if (smem_ab > 200 * 1024) return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_act_bwd_gpool: channel count exceeds shared memory");
-    static bool smem_attr[2][2] = {};
+    static bool smem_attr[2][2][2] = {};
     const int var = g.block.x * g.block.y > 256 ? 1 : 0;      // 1: more than 2048 channels (one row of C / 8 threads)
+    const int relu = act == DFD_ACT_RELU;
 #define GARGS nullptr, (const T*)y, scale, shift, mean, rstd, nullptr, dpooled, inv_hw, (T*)gu, hw, g.rows_per_block, s1, s2, \
               (const BnBwdFinDesc*)fin, argmax, pool_type
+#define GLAUNCH(ACT_) do {                                                                                                      \
+        if (smem_ab > 48 * 1024 && !smem_attr[dt == DFD_DT_FP16][relu][var]) {                                               \
+            cudaError_t e_ = var ? cudaFuncSetAttribute(act_bwd_kernel<T, ACT_, false, 512, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) \
+                                 : cudaFuncSetAttribute(act_bwd_kernel<T, ACT_, false, 256, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); \
+            if (e_ != cudaSuccess) return dfd_set_cuda_error(e_, __FILE__, __LINE__);                                         \
+            smem_attr[dt == DFD_DT_FP16][relu][var] = true;                                                                   \
+        }                                                                                                                     \
+        if (var) act_bwd_kernel<T, ACT_, false, 512, 1, true><<<g.grid, g.block, smem_ab, st>>>(GARGS);                       \
+        else act_bwd_kernel<T, ACT_, false, 256, 2, true><<<g.grid, g.block, smem_ab, st>>>(GARGS);                           \
+    } while (0)
     DISPATCH_T(dt, {
-        if (smem_ab > 48 * 1024 && !smem_attr[dt == DFD_DT_FP16][var]) {
-            cudaError_t e_ = var ? cudaFuncSetAttribute(act_bwd_kernel<T, 1, false, 512, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)
-                                 : cudaFuncSetAttribute(act_bwd_kernel<T, 1, false, 256, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-            if (e_ != cudaSuccess) return dfd_set_cuda_error(e_, __FILE__, __LINE__);
-            smem_attr[dt == DFD_DT_FP16][var] = true;
-        }
-        if (var) act_bwd_kernel<T, 1, false, 512, 1, true><<<g.grid, g.block, smem_ab, st>>>(GARGS);
-        else act_bwd_kernel<T, 1, false, 256, 2, true><<<g.grid, g.block, smem_ab, st>>>(GARGS);
+        if (relu) GLAUNCH(DFD_ACT_RELU);
+        else GLAUNCH(DFD_ACT_SWISH);
     });
+#undef GLAUNCH
 #undef GARGS
     DFD_LAUNCH_CHECK();
     return DFD_OK;
@@ -1514,6 +1635,36 @@ int dfd_avgpool2_bwd_add(const void* dy, const void* add, void* dx, int N, int H
     RowGeom g = make_geom(C, (long long)H * W, N);
     DISPATCH_T(dt, (avgpool2_bwd_add_kernel<T><<<g.grid, g.block, 0, (cudaStream_t)stream>>>((const T*)dy, (const T*)add, (T*)dx,
                                                                                             H, W, Ho, Wo, g.rows_per_block)));
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+// out [N, Ho, Wo, C] = maxpool3x3s2p1(scale*y + shift) + scale_s*ys + shift_s, Ho = (H - 1) / 2 + 1 (Xception's strided block
+// tail); idx (optional): the arg-max byte per output that dfd_maxpool_bn_bwd_reduce routes the gradient by
+int dfd_bn_maxpool_add(const void* y, const float* scale, const float* shift, const void* ys, const float* scale_s,
+                       const float* shift_s, void* out, void* idx, int N, int H, int W, int C, int dt, void* stream) {
+    if (C % 8 || C <= 0 || C > 8192 || N <= 0 || H <= 0 || W <= 0)
+        return dfd_set_error(DFD_ERR_ARG, "dfd_bn_maxpool_add: C%8, C <= 8192, sizes");
+    if (!scale || !shift || !ys || !scale_s || !shift_s) return dfd_set_error(DFD_ERR_ARG, "dfd_bn_maxpool_add: operands");
+    const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
+    RowGeom g = make_geom(C, (long long)Ho * Wo, N);
+    DISPATCH_T(dt, (bn_maxpool_add_kernel<T><<<g.grid, g.block, 0, (cudaStream_t)stream>>>((const T*)y, scale, shift, (const T*)ys,
+        scale_s, shift_s, (T*)out, (unsigned char*)idx, H, W, Wo, (long long)Ho * Wo, g.rows_per_block)));
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+// gx [N, H, W, C]: the gradient of dfd_bn_maxpool_add's pooled BatchNorm output (gy routed by idx), and the BN-backward sums
+// s1 += gx, s2 += gx * (y - mean) * rstd for dfd_bn_bwd_finalize
+int dfd_maxpool_bn_bwd_reduce(const void* gy, const void* idx, const void* y, const float* mean, const float* rstd, void* gx,
+                              int N, int H, int W, int C, int dt, double* s1, double* s2, void* stream) {
+    if (C % 8 || C <= 0 || C > 8192 || N <= 0 || H <= 0 || W <= 0)
+        return dfd_set_error(DFD_ERR_ARG, "dfd_maxpool_bn_bwd_reduce: C%8, C <= 8192, sizes");
+    if (!gy || !idx || !y || !mean || !rstd || !gx || !s1 || !s2) return dfd_set_error(DFD_ERR_ARG, "dfd_maxpool_bn_bwd_reduce: operands");
+    const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
+    RowGeom g = make_geom(C, (long long)H * W, N);
+    DISPATCH_T(dt, (maxpool_bn_bwd_reduce_kernel<T><<<g.grid, g.block, reduce_smem(g), (cudaStream_t)stream>>>((const T*)gy,
+        (const unsigned char*)idx, (const T*)y, mean, rstd, (T*)gx, H, W, Ho, Wo, g.rows_per_block, s1, s2)));
     DFD_LAUNCH_CHECK();
     return DFD_OK;
 }

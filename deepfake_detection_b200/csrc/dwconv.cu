@@ -569,7 +569,10 @@ __device__ __forceinline__ void strip_bwd_s1(const uint32_t* __restrict__ tile, 
 }
 
 // MODE 1: xin is the pre-BN expand output (a = swish(scale*xin + shift), gx = ga * swish', BN-backward sums);
-// MODE 0: xin is the block input itself (DS block): a = xin, gx = ga (+ add).
+// MODE 0: xin is the block input itself (DS block): a = xin, gx = ga (+ add);
+// MODE 2: a = relu(scale*xin + shift) (Xception, inside a block): gx = ga * 1[a > 0], BN-backward sums as MODE 1;
+// MODE 3: a = relu(xin) (Xception, a block's first separable convolution): gx = ga * 1[xin > 0] (+ add).
+// The ReLU masks test the 16-bit value the forward staged, so that torch's (out > 0) rule holds after rounding too.
 // DT / DL (stride 2 only): the top / left pad is (K-1)/2 - DT / (K-1)/2 - DL (see strip_bwd_s2).
 template <typename T, int K, int S, bool AFFINE, int MODE, int NT, int P, int CPW = 32, int DT = 0, int DL = 0>
 #ifndef DW_BWD_OCC3
@@ -605,7 +608,7 @@ dwconv_bwd_kernel(const T* __restrict__ gy, const T* __restrict__ yout, const fl
         wacc[i][0] = 0.f; wacc[i][1] = 0.f;
     }
     float sc0 = 1.f, sc1 = 1.f, sh0 = 0.f, sh1 = 0.f, mu0 = 0.f, mu1 = 0.f, rs0 = 0.f, rs1 = 0.f;
-    if (MODE == 1 && chv) {
+    if ((MODE == 1 || MODE == 2) && chv) {
         sc0 = scale[ch]; sc1 = scale[ch + 1]; sh0 = shift[ch]; sh1 = shift[ch + 1];
         mu0 = mean[ch]; mu1 = mean[ch + 1]; rs0 = rstd[ch]; rs1 = rstd[ch + 1];
     }
@@ -672,6 +675,20 @@ dwconv_bwd_kernel(const T* __restrict__ gy, const T* __restrict__ yout, const fl
                     da[p][1] = fmaf(g1, fmaf(-u1, g1, u1), g1);
                     xh[p][0] = fmaf(xi.x, rs0, nm0);                  // (x - mean) * rstd
                     xh[p][1] = fmaf(xi.y, rs1, nm1);
+                } else if (MODE == 2) {
+                    const float2 ar = unpack2<T>(pack2<T>(fmaxf(fmaf(xi.x, sc0, sh0), 0.f), fmaxf(fmaf(xi.y, sc1, sh1), 0.f)));
+                    av[p][0] = ar.x;
+                    av[p][1] = ar.y;
+                    da[p][0] = ar.x > 0.f ? 1.f : 0.f;
+                    da[p][1] = ar.y > 0.f ? 1.f : 0.f;
+                    xh[p][0] = fmaf(xi.x, rs0, nm0);
+                    xh[p][1] = fmaf(xi.y, rs1, nm1);
+                } else if (MODE == 3) {
+                    av[p][0] = fmaxf(xi.x, 0.f);     // zero outside the image and beyond C already
+                    av[p][1] = fmaxf(xi.y, 0.f);
+                    da[p][0] = xi.x > 0.f ? 1.f : 0.f;
+                    da[p][1] = xi.y > 0.f ? 1.f : 0.f;
+                    xh[p][0] = xh[p][1] = 0.f;
                 } else {
                     av[p][0] = xi.x;                 // pre[] is zero outside the image and beyond C already
                     av[p][1] = xi.y;
@@ -679,7 +696,7 @@ dwconv_bwd_kernel(const T* __restrict__ gy, const T* __restrict__ yout, const fl
                     xh[p][0] = xh[p][1] = 0.f;
                 }
             }
-            if (MODE == 1 && !interior) {
+            if ((MODE == 1 || MODE == 2) && !interior) {
 #pragma unroll
                 for (int p = 0; p < P; p++) {
                     const bool ok = sy < g.TH && iy < g.H && ix + p < g.W;
@@ -699,7 +716,7 @@ dwconv_bwd_kernel(const T* __restrict__ gy, const T* __restrict__ yout, const fl
 #pragma unroll
                 for (int p = 0; p < P; p++) {
                     if (ix + p < g.W) {
-                        if (MODE == 1) {
+                        if (MODE == 1 || MODE == 2) {
                             const uint32_t pk = pack2<T>(acc[p][0] * da[p][0], acc[p][1] * da[p][1]);
                             *reinterpret_cast<uint32_t*>(gx_n + off0 + (uint32_t)(p * g.C)) = pk;
                             const float2 r = unpack2<T>(pk);
@@ -708,6 +725,7 @@ dwconv_bwd_kernel(const T* __restrict__ gy, const T* __restrict__ yout, const fl
                             b1 = fmaf(r.y, xh[p][1], b1);
                         } else {
                             float v0 = acc[p][0], v1 = acc[p][1];
+                            if (MODE == 3) { v0 *= da[p][0]; v1 *= da[p][1]; }
                             if (add) {
                                 const float2 ad = unpack2<T>(__ldg(reinterpret_cast<const uint32_t*>(add + ioff + off0 + (uint32_t)(p * g.C))));
                                 v0 += ad.x; v1 += ad.y;
@@ -719,7 +737,7 @@ dwconv_bwd_kernel(const T* __restrict__ gy, const T* __restrict__ yout, const fl
             }
         }
     }
-    if (MODE == 1) {
+    if (MODE == 1 || MODE == 2) {
         double* p1 = stat_slot(ds1, g.C);
         double* p2 = stat_slot(ds2, g.C);
         reduce_warps_emit<CPW>(red, a0, a1, [&](int c, float v) { if (c0 + c < g.C) atomicAdd(p1 + c0 + c, (double)v); });
@@ -861,15 +879,20 @@ static int dw_nt(int k) {
 
 extern "C" {
 
-// out[N,Ho,Wo,C] = dwconv(act_in(scale*x + shift)); scale == NULL: x is consumed as is (act_in must be 0).
+// out[N,Ho,Wo,C] = dwconv(act_in(scale*x + shift)); scale == NULL: x is consumed as is (act_in 0) or through a ReLU (act_in
+// DFD_ACT_RELU). A BN input takes Swish, or ReLU (k = 3, stride 1, without output statistics).
 // dsum/dsq (optional): per-channel sum / sum of squares of the rounded outputs (fp64, accumulated).
 // dt_ / dl_: the top / left pad is (k-1)/2 - dt_ / (k-1)/2 - dl_ (TF "SAME", stride 2)
 static int dw_fwd(const void* x, const float* scale, const float* shift, const float* w, void* out, int N, int H, int W,
                   int C, int k, int stride, int dt_, int dl_, int act_in, int dt, double* dsum, double* dsq,
                   const void* fin, void* stream) {
     if (C % 8 || N <= 0 || H <= 0 || W <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_dwconv_fwd: sizes");
-    if (!scale && act_in != DFD_ACT_NONE) return dfd_set_error(DFD_ERR_ARG, "dfd_dwconv_fwd: act without BN");
-    if (scale && act_in != DFD_ACT_SWISH) return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_dwconv_fwd: BN input implies Swish");
+    // a ReLU input, after a BN (scale != NULL) or alone: Xception's separable convolutions, k = 3 at stride 1, no BN behind
+    const bool relu = act_in == DFD_ACT_RELU;
+    if (relu && (k != 3 || stride != 1 || dt_ || dl_ || dsum || dsq || fin))
+        return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_dwconv_fwd: a ReLU input needs k = 3, stride 1 and no statistics");
+    if (!relu && !scale && act_in != DFD_ACT_NONE) return dfd_set_error(DFD_ERR_ARG, "dfd_dwconv_fwd: act without BN");
+    if (!relu && scale && act_in != DFD_ACT_SWISH) return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_dwconv_fwd: BN input implies Swish");
     DwGeom g;
     const int cpw = dw_cpw(C);
     int smem = fill_geom(g, N, H, W, C, k, stride, false, cpw);
@@ -902,6 +925,14 @@ static int dw_fwd(const void* x, const float* scale, const float* shift, const f
     cudaStream_t st = (cudaStream_t)stream;
 #define FW(ACT_, AFF_, CPW_) DW_LAUNCH((dwconv_fwd_kernel<T, K, S, ACT_, AFF_, NT, CPW_>), grid, smem, st, (const T*)x, scale, shift, w, (T*)out, dsum, dsq, (const BnFinDesc*)fin, g)
 #define FWC(ACT_, AFF_) do { if (cpw == 32) FW(ACT_, AFF_, 32); else if (cpw == 16) FW(ACT_, AFF_, 16); else FW(ACT_, AFF_, 8); } while (0)
+    if (relu) {
+        DW_DISPATCH_T(dt, { constexpr int K = 3, S = 1; DW_NT(3, {
+            if (scale) FWC(DFD_ACT_RELU, true);
+            else FWC(DFD_ACT_RELU, false);
+        }); });
+        DFD_LAUNCH_CHECK();
+        return DFD_OK;
+    }
     DW_DISPATCH_T(dt, DW_DISPATCH_KS(k, stride, {
         if (scale) FWC(DFD_ACT_SWISH, true);
         else FWC(DFD_ACT_NONE, false);
@@ -1014,8 +1045,10 @@ static int dw_bwd(const void* gy, const void* yout, const float* cA, const float
                   const float* w, const void* xin, const float* scale, const float* shift, const float* mean,
                   const float* rstd, const void* add, void* gx, float* dW, int N, int H, int W, int C, int k,
                   int stride, int dt_, int dl_, int dt, double* s1, double* s2, void* ws, long long ws_bytes, const void* fin,
-                  void* stream) {
+                  void* stream, bool relu = false) {
     if (C % 8 || N <= 0 || H <= 0 || W <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_dwconv_bwd: sizes");
+    if (relu && (k != 3 || stride != 1 || cA || dt_ || dl_))
+        return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_dwconv_bwd_relu: k = 3, stride 1, the BN backward not folded into gy (cA NULL)");
     if (!xin || !dW) return dfd_set_error(DFD_ERR_ARG, "dfd_dwconv_bwd: operands");
     if (scale && (!shift || !mean || !rstd || !s1 || !s2)) return dfd_set_error(DFD_ERR_ARG, "dfd_dwconv_bwd: mode 1 operands");
     DwGeom g;
@@ -1068,6 +1101,11 @@ static int dw_bwd(const void* gy, const void* yout, const float* cA, const float
         DFD_LAUNCH_CHECK();
         return DFD_OK;
     }
+    if (relu) {
+        DW_DISPATCH_T(dt, { if (scale) BW1(3, 1, false, 2); else BW1(3, 1, false, 3); });
+        DFD_LAUNCH_CHECK();
+        return DFD_OK;
+    }
     DW_DISPATCH_T(dt, {
         if (k == 3 && stride == 1) BW(3, 1);
         else if (k == 3 && stride == 2) BW(3, 2);
@@ -1090,6 +1128,17 @@ int dfd_dwconv_bwd(const void* gy, const void* yout, const float* cA, const floa
                    int stride, int dt, double* s1, double* s2, void* ws, long long ws_bytes, const void* fin, void* stream) {
     return dw_bwd(gy, yout, cA, cB, cC, w, xin, scale, shift, mean, rstd, add, gx, dW, N, H, W, C, k, stride, 0, 0, dt, s1, s2,
                   ws, ws_bytes, fin, stream);
+}
+
+// dfd_dwconv_bwd of a depthwise stage whose input passes a ReLU (Xception's separable convolutions; k = 3, stride 1, cA NULL):
+// scale != NULL: the input is relu(scale*xin + shift), gx = dgrad * 1[relu > 0] with the BN-backward sums s1 / s2 of gx;
+// scale == NULL: the input is relu(xin), gx = dgrad * 1[xin > 0] (+ add). dW and the workspace as in dfd_dwconv_bwd.
+int dfd_dwconv_bwd_relu(const void* gy, const void* yout, const float* cA, const float* cB, const float* cC,
+                        const float* w, const void* xin, const float* scale, const float* shift, const float* mean,
+                        const float* rstd, const void* add, void* gx, float* dW, int N, int H, int W, int C, int k,
+                        int stride, int dt, double* s1, double* s2, void* ws, long long ws_bytes, const void* fin, void* stream) {
+    return dw_bwd(gy, yout, cA, cB, cC, w, xin, scale, shift, mean, rstd, add, gx, dW, N, H, W, C, k, stride, 0, 0, dt, s1, s2,
+                  ws, ws_bytes, fin, stream, true);
 }
 
 // dfd_dwconv_bwd of a stage padded with pad_t rows above and pad_l columns left of the image (TF "SAME", as in

@@ -7,7 +7,7 @@ This is the host side of the hot path (dfd/runners/train.py:610-649): given an a
   * builds, once, the ordered list of C-ABI calls ("plan") for forward, backward and the optimizer, and
   * replays the plan on the caller's current CUDA stream (optionally captured into a CUDA graph).
 
-The family's plan builder (engine_efficientnet.build_efficientnet, engine_resnet.build_resnet) lays out the activations
+The family's plan builder (engine_efficientnet, engine_resnet, engine_xception) lays out the activations
 and lists the ops; the conventions every plan shares (BatchNorm statistics and finalisation, the mask generators, the
 deterministic weight-gradient reduce, validation against the ABI table) are the plan helpers of this class.
 
@@ -86,9 +86,10 @@ class Engine:
             if dist.is_available() and dist.is_initialized():
                 self.sync_world = dist.get_world_size()
             self.sync_bn = self.sync_world > 1
-        if self.sync_bn and spec.family == "resnet":
-            raise _lib.NativeError("sync_bn over %d ranks: the ResNet plan has no synchronised BatchNorm (only the "
-                                   "EfficientNet plan all-reduces its batch statistics)" % self.sync_world)
+        if self.sync_bn and spec.family in ("resnet", "xception"):
+            raise _lib.NativeError("sync_bn over %d ranks: the %s plan has no synchronised BatchNorm (only the "
+                                   "EfficientNet plan all-reduces its batch statistics)"
+                                   % (self.sync_world, "ResNet" if spec.family == "resnet" else "Xception"))
         self.bn_momentum = float(bn_momentum)
         self.bn_eps = float(bn_eps)
         # "tc": wgmma GEMMs and implicit convolutions; "mma": the mma.sync cross-check path (GEMMs over im2col columns)
@@ -411,7 +412,8 @@ class Engine:
     def _build(self):
         from .engine_efficientnet import build_efficientnet
         from .engine_resnet import build_resnet
-        (build_resnet if self.spec.family == "resnet" else build_efficientnet)(self)
+        from .engine_xception import build_xception
+        {"resnet": build_resnet, "xception": build_xception}.get(self.spec.family, build_efficientnet)(self)
 
     # ---- plan helpers shared by the family builders ---------------------------------------------------------------------
     def _stats(self, bn):

@@ -18,7 +18,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .arch import RESNET_ARCHS, SUPPORTED_ARCHS, TF_ARCHS, TF_POOL_CROP, get_spec, state_entries
+from .arch import RESNET_ARCHS, SUPPORTED_ARCHS, TF_ARCHS, TF_POOL_CROP, XCEPTION_ARCHS, get_spec, state_entries
 from .engine import Engine
 
 _DEFAULT_CFG = dict(num_classes=1000, pool_size=(7, 7), crop_pct=0.875, interpolation="bicubic",
@@ -26,6 +26,11 @@ _DEFAULT_CFG = dict(num_classes=1000, pool_size=(7, 7), crop_pct=0.875, interpol
 _INCEPTION_MEAN_STD = dict(mean=(0.5, 0.5, 0.5), std=(0.5, 0.5, 0.5))      # the AdvProp (_ap) checkpoints' normalisation
 # resnet.py:22-58: bilinear unless the entry says bicubic
 _RESNET_BICUBIC = ("resnet26", "resnet26d", "resnet50d")
+# xception.py:27-38
+_XCEPTION_CFG = dict(input_size=(3, 299, 299), crop_pct=0.8975, interpolation="bicubic", mean=(0.5, 0.5, 0.5),
+                     std=(0.5, 0.5, 0.5), first_conv="conv1", classifier="fc")
+# Xception.__init__ takes num_classes, in_chans, drop_rate and global_pool only (xception.py:132)
+_XCEPTION_KWARGS = ("drop_rate", "global_pool", "dtype", "gemm_impl")
 
 
 class _NativeForward(torch.autograd.Function):
@@ -66,17 +71,20 @@ def init_state_dict(spec, seed=None):
     EfficientNet: efficientnet_builder.py:537-575 (`_init_weight_goog`: conv N(0, 2/fan_out), depthwise fan_out / groups,
     Linear U(+-1/sqrt(fan_out)), BN 1 / 0);
     ResNet: resnet.py:410-420 (conv kaiming_normal fan_out, BN 1 / 0, the LAST BN gamma of every residual block ZERO -
-    `zero_init_last_bn=True` is the constructor default, :353 - and nn.Linear's default U(+-1/sqrt(fan_in)) for fc)."""
+    `zero_init_last_bn=True` is the constructor default, :353 - and nn.Linear's default U(+-1/sqrt(fan_in)) for fc);
+    Xception: xception.py:171-177 (every nn.Conv2d, depthwise included, kaiming_normal fan_out = out_channels * k * k - torch
+    does not divide by the groups - BN 1 / 0, nn.Linear's default init for fc)."""
     import math
     g = torch.Generator(device="cpu").manual_seed((torch.initial_seed() if seed is None else seed) % (2 ** 31))
     sd = OrderedDict()
     resnet = spec.family == "resnet"
+    fan_in_fc = spec.family in ("resnet", "xception")
     last_bn = set()
     if resnet:
         for b in spec.blocks:
             last_bn.add(b.name + (".bn2.weight" if b.kind == "basic" else ".bn3.weight"))       # resnet.py:147-148,212-213
     for name, shape, role in state_entries(spec):
-        if resnet and role in ("fc_w", "fc_b"):
+        if fan_in_fc and role in ("fc_w", "fc_b"):
             r = 1.0 / math.sqrt(spec.pooled_features)
             sd[name] = (torch.rand(shape, generator=g) * 2 - 1) * r
             continue
@@ -85,7 +93,7 @@ def init_state_dict(spec, seed=None):
             continue
         if role in ("conv_w", "dw_w", "se_w"):
             fan_out = shape[0] * shape[2] * shape[3]
-            if role == "dw_w":
+            if role == "dw_w" and spec.family != "xception":
                 fan_out = shape[2] * shape[3]           # fan_out //= groups
             sd[name] = torch.randn(shape, generator=g) * math.sqrt(2.0 / fan_out)
         elif role == "bn_w":
@@ -137,6 +145,8 @@ class NativeModel(nn.Module):
                 self.default_cfg.update(_INCEPTION_MEAN_STD)
         if arch in RESNET_ARCHS:
             self.default_cfg.update(interpolation="bicubic" if arch in _RESNET_BICUBIC else "bilinear")
+        if arch in XCEPTION_ARCHS:
+            self.default_cfg.update(_XCEPTION_CFG)
         self._engines = OrderedDict()
         self._primary = None
         self._pending_state = None
@@ -270,8 +280,22 @@ def create_model(model_name, pretrained=False, num_classes=1000, in_chans=3, che
     """dfd/timm/models/factory.py:8-64 for the architectures on the native hot path."""
     if pretrained:
         raise _lib.NativeError("pretrained weights need network access; load a checkpoint instead")
-    if model_name not in SUPPORTED_ARCHS and model_name not in TF_ARCHS and model_name not in RESNET_ARCHS:
+    if model_name not in SUPPORTED_ARCHS + TF_ARCHS + RESNET_ARCHS + XCEPTION_ARCHS:
         raise RuntimeError("Unknown model (%s)" % model_name)       # factory.py:56
+    if model_name in XCEPTION_ARCHS:
+        # factory.py:31-45: the BatchNorm arguments are dropped for every model that is not an EfficientNet, and
+        # drop_block_rate / drop_path_rate when they are None; anything else reaches Xception.__init__, which refuses it
+        for k in ("bn_tf", "bn_momentum", "bn_eps"):
+            kwargs.pop(k, None)
+        dc = kwargs.pop("drop_connect_rate", None)
+        if dc is not None and kwargs.get("drop_path_rate") is None:
+            kwargs["drop_path_rate"] = dc
+        for k in ("drop_block_rate", "drop_path_rate"):
+            if kwargs.get(k, 0) is None:
+                kwargs.pop(k)
+        bad = sorted(k for k in kwargs if k not in _XCEPTION_KWARGS)
+        if bad:
+            raise TypeError("__init__() got an unexpected keyword argument '%s'" % bad[0])
     model = NativeModel(model_name, num_classes=num_classes, in_chans=in_chans, **kwargs)
     if checkpoint_path:
         from .helpers import load_checkpoint

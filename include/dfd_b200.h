@@ -119,6 +119,13 @@ int dfd_dwconv_block_channels(int C);
 int dfd_dwconv_fwd_pad(const void* x, const float* scale, const float* shift, const float* w, void* out, int N, int H,
                        int W, int C, int k, int stride, int pad_t, int pad_l, int act_in, int dt, double* dsum, double* dsq,
                        const void* fin, void* stream);
+/* dfd_dwconv_bwd of a depthwise stage whose input passes a ReLU (Xception's separable convolutions; k = 3, stride 1, cA NULL):
+ * scale != NULL: input relu(scale*xin + shift), gx = dgrad * 1[relu > 0] plus the BN-backward sums s1 / s2 of gx;
+ * scale == NULL: input relu(xin), gx = dgrad * 1[xin > 0] (+ add). The masks test the staged 16-bit value. */
+int dfd_dwconv_bwd_relu(const void* gy, const void* yout, const float* cA, const float* cB, const float* cC,
+                        const float* w, const void* xin, const float* scale, const float* shift, const float* mean,
+                        const float* rstd, const void* add, void* gx, float* dW, int N, int H, int W, int C, int k,
+                        int stride, int dt, double* s1, double* s2, void* ws, long long ws_bytes, const void* fin, void* stream);
 int dfd_dwconv_bwd_pad(const void* gy, const void* yout, const float* cA, const float* cB, const float* cC,
                        const float* w, const void* xin, const float* scale, const float* shift, const float* mean,
                        const float* rstd, const void* add, void* gx, float* dW, int N, int H, int W, int C, int k,
@@ -234,7 +241,7 @@ int dfd_se_bwd_reduce(const void* da, const void* y, const float* scale, const f
 int dfd_act_bwd(const void* da, const void* y, const float* scale, const float* shift, const float* mean,
                 const float* rstd, const float* gate, const float* dpool, void* gu, int n, long long hw, int C,
                 int act, int dt, double* s1, double* s2, const void* fin, void* stream);
-/* dfd_act_bwd with no da and the gradient of dfd_global_pool instead of dpool (EfficientNet head, act = Swish):
+/* dfd_act_bwd with no da and the gradient of dfd_global_pool instead of dpool (EfficientNet head: act = Swish; Xception: ReLU):
  *   gu = (g_avg[n,c] / hw + (hw == argmax[n,c]) * g_max[n,c]) * act'(u), g_avg / g_max from dpooled [n, P] as in
  * dfd_gpool_bwd; the BN backward sums and `fin` as in dfd_act_bwd. pool_type != DFD_POOL_AVG. */
 int dfd_act_bwd_gpool(const void* y, const float* scale, const float* shift, const float* mean, const float* rstd,
@@ -249,6 +256,15 @@ int dfd_avgpool2_fwd(const void* x, void* y, int N, int H, int W, int C, int dt,
 /* its input gradient, added to a second source: dx[n,y,x,c] = round16(add[n,y,x,c] + dy[n,y/2,x/2,c] / count(y/2, x/2)).
  * add may be NULL (zero) or dx itself. Elementwise, no atomics. H, W = INPUT extents. */
 int dfd_avgpool2_bwd_add(const void* dy, const void* add, void* dx, int N, int H, int W, int C, int dt, void* stream);
+/* tail of a strided Xception block (xception.py:110-124): out[N, Ho, Wo, C] = maxpool3x3s2p1(scale*y + shift) + scale_s*ys +
+ * shift_s, Ho = (H - 1) / 2 + 1, rounded once; windows padded with -inf, the first maximum in row-major window order wins.
+ * idx (NULL: not written): the arg-max tap (0..8), one byte per output. */
+int dfd_bn_maxpool_add(const void* y, const float* scale, const float* shift, const void* ys, const float* scale_s,
+                       const float* shift_s, void* out, void* idx, int N, int H, int W, int C, int dt, void* stream);
+/* its backward through the pool: gx[N, H, W, C] = round16(sum of gy over the windows whose arg-max is the pixel), no atomics,
+ * and the BN-backward sums s1 += gx, s2 += gx * (y - mean) * rstd (accumulated). H, W = INPUT extents. */
+int dfd_maxpool_bn_bwd_reduce(const void* gy, const void* idx, const void* y, const float* mean, const float* rstd, void* gx,
+                              int N, int H, int W, int C, int dt, double* s1, double* s2, void* stream);
 
 /* ---- squeeze-excite FCs: SqueezeExcite.forward, efficientnet_blocks.py:104-110 ------------------------ */
 int dfd_se_fc_fwd(const float* pooled, const float* Wr, const float* br, const float* We, const float* be,
