@@ -62,6 +62,8 @@ SIGNATURES = {
     "dfd_se_fc_wgrad": "pppp" "pppp" "iii" "p",
     "dfd_pool_se": "pppp" "ppppp" "ili" "iii" "i" "p",
     "dfd_se_bwd_chain": "ppppp" "ppppp" "pppp" "ili" "ii" "p",
+    "dfd_pool_se_relu": "pppp" "ppppp" "ili" "iiii" "p",
+    "dfd_relu_se_bwd_reduce": "pppppp" "pp" "ppppp" "pppp" "ili" "iii" "p",
     "dfd_head_fwd": "pppp" "iii" "pp" "ff" "pppp" "p",
     "dfd_head_bwd": "pppppp" "iii" "p",
     "dfd_sgd_step": "ppp" "l" "fffi" "f" "ppp" "i" "p" "p",
@@ -96,6 +98,8 @@ SIGNATURES = {
     "dfd_unpack_grad": "pp" "iii" "p",
     "dfd_maxpool_fwd": "ppp" "iiii" "i" "p",
     "dfd_maxpool_bwd": "ppp" "iiii" "i" "p",
+    "dfd_maxpool_ceil_fwd": "ppp" "iiii" "i" "p",
+    "dfd_maxpool_ceil_bwd": "ppp" "iiii" "i" "p",
     "dfd_relu_bwd": "ppp" "li" "p",
     "dfd_pool_bwd": "pp" "ili" "i" "p",
     "dfd_gpool_bwd": "ppp" "ili" "ii" "p",

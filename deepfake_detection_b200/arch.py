@@ -18,6 +18,9 @@ BASELINE.json names; it builds no modules and owns no tensors.
   * ResNet-26/34/101/152, tv_*, wide_* (base_width 128) and ResNet-D (deep stem, downsample_avg): resnet.py:187,263-277,
     349-439,483-625
   * Xception: dfd/timm/models/xception.py (SeparableConv2d :58-69, Block :72-124, Xception :127-226)
+  * SE-ResNets (seresnet18/34/50/101/152): dfd/timm/models/senet.py (SEModule :67-86, SEResNetBottleneck :141-163 with the
+    stride on conv1, SEResNetBlock :190-223, SENet :226-396: layer0 7x7 s2 -> BN -> ReLU -> MaxPool2d(3, 2, ceil_mode=True),
+    1x1 downsample, `last_linear`; entrypoints :399-461)
 """
 import math
 import re
@@ -162,6 +165,7 @@ class ResBlock:
     downsample: bool     # 1x1 conv (stride) + BN on the identity path
     width: int           # bottleneck width int(planes * base_width / 64), resnet.py:187 (== planes for a BasicBlock)
     avg_down: bool = False   # ResNet-D shortcut: AvgPool2d(2, stride, ceil_mode, count_include_pad=False) -> 1x1 conv -> BN
+    cse: int = 0             # SENet: squeeze width cout // reduction of the block's SEModule (0: no SE)
 
 
 @dataclass
@@ -177,10 +181,28 @@ class ResNetSpec:
     global_pool: str = "avg"
     stem_type: str = ""          # '' (7x7 conv) or 'deep' (3x3 s2 -> 3x3 -> 3x3 of stem_width, stem_width, 64), resnet.py:365-379
     stem_width: int = 32
+    # SE-ResNet (senet.py): an SEModule in every block, the bottleneck's stride on its 1x1 conv1, the stem pool
+    # MaxPool2d(3, 2, ceil_mode=True) without padding, and the SENet key names (layer0.*, se_module.*, last_linear)
+    se_reduction: int = 0
+    stride_in_1x1: bool = False
+    stem_pool: str = "p1"        # 'p1' (3x3 s2 padding 1) or 'ceil' (3x3 s2 padding 0, ceil mode)
+    naming: str = "resnet"       # 'resnet' or 'senet'
 
     @property
     def pooled_features(self):
         return self.num_features * pool_feat_mult(self.global_pool)
+
+    @property
+    def stem_conv(self):
+        return "layer0.conv1" if self.naming == "senet" else "conv1"
+
+    @property
+    def stem_bn(self):
+        return "layer0.bn1" if self.naming == "senet" else "bn1"
+
+    @property
+    def cls_name(self):
+        return "last_linear" if self.naming == "senet" else "fc"
 
 
 def _resnet_spec(arch, kind, layers, in_chans, num_classes, input_size, base_width=64, stem_type="", avg_down=False):
@@ -198,6 +220,25 @@ def _resnet_spec(arch, kind, layers, in_chans, num_classes, input_size, base_wid
             cin = cout
     return ResNetSpec(arch=arch, in_chans=in_chans, stem=64, blocks=blocks, num_features=cin,
                       num_classes=num_classes, input_size=input_size, stem_type=stem_type)
+
+
+def _senet_spec(arch, in_chans, num_classes):
+    """SENet(block, layers, groups=1, reduction=16, inplanes=64, input_3x3=False, downsample_kernel_size=1,
+    downsample_padding=0) of the seresnet* entrypoints (senet.py:399-461)"""
+    kind, layers = _SENET_DEFS[arch]
+    spec = _resnet_spec(arch, kind, layers, in_chans, num_classes, (3, 224, 224))
+    for b in spec.blocks:
+        b.cse = b.cout // 16
+    spec.se_reduction, spec.stride_in_1x1, spec.stem_pool, spec.naming = 16, kind == "bottleneck", "ceil", "senet"
+    return spec
+
+
+def stem_pool_out(h, stem_pool):
+    """extent after the ResNet stem's max-pool: 3x3 s2 p1, or SENet's 3x3 s2 p0 ceil mode (torch's pooling_output_shape)"""
+    if stem_pool != "ceil":
+        return conv_out(h, 3, 2, 1)
+    o = (h - 3 + 1) // 2 + 1
+    return o - 1 if (o - 1) * 2 >= h else o
 
 
 # ----------------------------------------------------------------------------------------------
@@ -313,6 +354,8 @@ def _base_spec(arch, num_classes, in_chans):
                             stem_type="deep" if deep else "", avg_down=deep)
     if arch in XCEPTION_ARCHS:
         return _xception_spec(arch, in_chans, num_classes)
+    if arch in SENET_ARCHS:
+        return _senet_spec(arch, in_chans, num_classes)
     raise ValueError("arch %r is not on the native hot path (see SURVEY.md section 8)" % (arch,))
 
 
@@ -336,6 +379,16 @@ _RESNET_DEFS = {
 RESNET_ARCHS = tuple(_RESNET_DEFS)
 
 XCEPTION_ARCHS = ("xception",)      # xception.py:229-237
+
+# SE-ResNets (senet.py:399-461): arch -> (block, layers). SE-ResNeXt and senet154 (grouped 3x3 convolutions) are not here.
+_SENET_DEFS = {
+    "seresnet18": ("basic", (2, 2, 2, 2)),
+    "seresnet34": ("basic", (3, 4, 6, 3)),
+    "seresnet50": ("bottleneck", (3, 4, 6, 3)),
+    "seresnet101": ("bottleneck", (3, 4, 23, 3)),
+    "seresnet152": ("bottleneck", (3, 8, 36, 3)),
+}
+SENET_ARCHS = tuple(_SENET_DEFS)
 
 # TensorFlow-ported EfficientNets (efficientnet.py:1265-1530): the B0 generator with TF "SAME" padding and BatchNorm eps 1e-3.
 # _ap (AdvProp) and _ns (Noisy Student) share the plain variant's layers; only their default_cfg differs (models.py).
@@ -448,8 +501,8 @@ def state_entries(spec):
             out += _bn_entries("conv1.4", sw)
             out.append(("conv1.6.weight", (64, sw, 3, 3), "conv_w"))
         else:
-            out.append(("conv1.weight", (64, spec.in_chans, 7, 7), "conv_w"))
-        out += _bn_entries("bn1", 64)
+            out.append((spec.stem_conv + ".weight", (64, spec.in_chans, 7, 7), "conv_w"))
+        out += _bn_entries(spec.stem_bn, 64)
         for b in spec.blocks:
             p = b.name
             if b.kind == "basic":
@@ -464,13 +517,19 @@ def state_entries(spec):
                 out += _bn_entries(p + ".bn2", b.width)
                 out.append((p + ".conv3.weight", (b.cout, b.width, 1, 1), "conv_w"))
                 out += _bn_entries(p + ".bn3", b.cout)
+            if b.cse:
+                # SEModule fc1 / fc2: 1x1 convolutions with a bias, registered after the last BN (senet.py:72-76,161,202)
+                out.append((p + ".se_module.fc1.weight", (b.cse, b.cout, 1, 1), "se_w"))
+                out.append((p + ".se_module.fc1.bias", (b.cse,), "se_b"))
+                out.append((p + ".se_module.fc2.weight", (b.cout, b.cse, 1, 1), "se_w"))
+                out.append((p + ".se_module.fc2.bias", (b.cout,), "se_b"))
             if b.downsample:
                 # downsample_avg puts the pool (nn.Identity at stride 1: no keys) at index 0, resnet.py:263-277
                 i = 1 if b.avg_down else 0
                 out.append((p + ".downsample.%d.weight" % i, (b.cout, b.cin, 1, 1), "conv_w"))
                 out += _bn_entries(p + ".downsample.%d" % (i + 1), b.cout)
-        out.append(("fc.weight", (spec.num_classes, spec.pooled_features), "fc_w"))
-        out.append(("fc.bias", (spec.num_classes,), "fc_b"))
+        out.append((spec.cls_name + ".weight", (spec.num_classes, spec.pooled_features), "fc_w"))
+        out.append((spec.cls_name + ".bias", (spec.num_classes,), "fc_b"))
     return out
 
 

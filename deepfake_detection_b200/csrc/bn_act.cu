@@ -251,7 +251,8 @@ __global__ void bn_act_kernel(const T* __restrict__ y, const float* __restrict__
 // ---------------------------------------------------------------------------------------------
 // pooled[n,c] = mean_hw act(scale*y + shift)       (one CTA per image: deterministic, no atomics)
 // ---------------------------------------------------------------------------------------------
-template <typename T, int ACT>
+// SE_ACT: inner activation of the squeeze-excite chain behind the pooling (se.Wr != NULL)
+template <typename T, int ACT, int SE_ACT = DFD_ACT_SWISH>
 __global__ void pool_kernel(const T* __restrict__ y, const float* __restrict__ scale,
                             const float* __restrict__ shift, float* __restrict__ pooled,
                             long long hw, long long rows_per_block, const SeFwdArgs se) {
@@ -322,7 +323,7 @@ __global__ void pool_kernel(const T* __restrict__ y, const float* __restrict__ s
     if (!se.Wr) return;
     __syncthreads();
     // the CTA that completed this image's squeeze carries on with its excite FCs (efficientnet_blocks.py:104-110)
-    se_fwd_chain(pv, pv + C, se.Wr, se.br, se.We, se.be, se.gate + (size_t)blockIdx.y * C, C, se.Cse, tid, nt);
+    se_fwd_chain<SE_ACT>(pv, pv + C, se.Wr, se.br, se.We, se.be, se.gate + (size_t)blockIdx.y * C, C, se.Cse, tid, nt);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -673,6 +674,100 @@ __global__ void se_bwd_reduce_kernel(const T* __restrict__ da, const T* __restri
     __syncthreads();
     se_bwd_chain(cs, cs + C, se.Wr, se.br, se.We, se.be, se.d_e + n * C, se.r + n * se.Cse, se.d_rpre + n * se.Cse,
                  se.dpool + n * C, C, se.Cse, tid, nt);
+}
+
+// ---------------------------------------------------------------------------------------------
+// SE-ResNet block tail backward (senet.py:111-112, 220-221: out = relu(a * gate[n,c] + residual), a = act(scale*y + shift),
+// act = identity for the bottleneck, ReLU for the basic block, :213-215):
+//   gm = round16(g + g2) * (out > 0), stored (the gradient of the residual path and, times the gate, of a)
+//   draw[n,c] = sum_hw gm * a                                             (dL/dgate)
+// and the CTA that completes an image's draw runs the SEModule's backward FC chain with the ReLU inner activation.
+// ---------------------------------------------------------------------------------------------
+template <typename T, int ACT>
+__global__ void relu_se_bwd_reduce_kernel(const T* __restrict__ g, const T* __restrict__ g2, const T* __restrict__ y,
+                                          const T* __restrict__ out, const float* __restrict__ scale,
+                                          const float* __restrict__ shift, T* __restrict__ gm, float* __restrict__ draw,
+                                          long long hw, long long rows_per_block, const SeBwdArgs se) {
+    extern __shared__ float sm[];
+    const int V = blockDim.x, C = V * 8;
+    const int c0 = threadIdx.x * 8;
+    float sc[8], sh[8], acc[8];
+#pragma unroll
+    for (int i = 0; i < 8; i++) acc[i] = 0.f;
+    ldg_f8(scale + c0, sc);
+    ldg_f8(shift + c0, sh);
+    const size_t img = (size_t)blockIdx.y * hw * C + c0;
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    long long r1 = r0 + rows_per_block;
+    if (r1 > hw) r1 = hw;
+    constexpr int U = 2;
+    for (long long r = r0 + threadIdx.y; r < r1; r += (long long)U * blockDim.y) {
+        uint4 graw[U], g2raw[U], yraw[U], oraw[U];
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+            const long long rr = r + (long long)u * blockDim.y;
+            if (rr < r1) {
+                const size_t off = img + (size_t)rr * C;
+                graw[u] = ldg16(g + off);
+                if (g2) g2raw[u] = ldg16(g2 + off);
+                yraw[u] = ldg16(y + off);
+                oraw[u] = ldg16(out + off);
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+            const long long rr = r + (long long)u * blockDim.y;
+            if (rr >= r1) break;
+            float gg[8], yy[8], oo[8];
+            unpack8<T>(graw[u], gg);
+            unpack8<T>(yraw[u], yy);
+            unpack8<T>(oraw[u], oo);
+            if (g2) {
+                float hh[8];
+                unpack8<T>(g2raw[u], hh);
+#pragma unroll
+                for (int i = 0; i < 8; i++) gg[i] = round_t<T>(gg[i] + hh[i]);
+            }
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                gg[i] = oo[i] > 0.f ? gg[i] : 0.f;
+                acc[i] = fmaf(gg[i], act_fwd<ACT>(fmaf(yy[i], sc[i], sh[i])), acc[i]);
+            }
+            stg16(gm + img + (size_t)rr * C, pack8<T>(gg));
+        }
+    }
+    float* dst = draw + (size_t)blockIdx.y * C;
+    const int tid = threadIdx.y * blockDim.x + threadIdx.x, nt = blockDim.x * blockDim.y;
+    float* cs = sm + (size_t)blockDim.y * C;        // chain scratch, as in se_bwd_reduce_kernel
+    if (gridDim.x == 1) {
+        reduce_rows_and_emit(sm, acc, [&](int c, float v) { dst[c] = v; cs[C + c] = v; });
+    } else {
+        // fixed-slot partials [chunk][image][C], added in chunk order by the last chunk of the image to arrive
+        float* part = g_rowred_ws + ((size_t)blockIdx.x * gridDim.y + blockIdx.y) * C;
+        reduce_rows_and_emit(sm, acc, [&](int c, float v) { part[c] = v; });
+        __shared__ int s_last;
+        __threadfence();
+        __syncthreads();
+        if (tid == 0) {
+            const int t = atomicAdd(g_rowred_tk + blockIdx.y, 1);
+            s_last = (t == (int)gridDim.x - 1);
+            if (s_last) g_rowred_tk[blockIdx.y] = 0;
+        }
+        __syncthreads();
+        if (!s_last) return;
+        __threadfence();
+        for (int c = tid; c < C; c += nt) {
+            float v = 0.f;
+            for (int k = 0; k < (int)gridDim.x; k++) v += __ldcg(g_rowred_ws + ((size_t)k * gridDim.y + blockIdx.y) * C + c);
+            dst[c] = v;
+            cs[C + c] = v;
+        }
+    }
+    const size_t n = blockIdx.y;
+    for (int c = tid; c < C; c += nt) cs[c] = se.pooled[n * C + c];
+    __syncthreads();
+    se_bwd_chain<DFD_ACT_RELU>(cs, cs + C, se.Wr, se.br, se.We, se.be, se.d_e + n * C, se.r + n * se.Cse,
+                               se.d_rpre + n * se.Cse, se.dpool + n * C, C, se.Cse, tid, nt);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1281,6 +1376,7 @@ int dfd_bn_act(const void* y, const float* scale, const float* shift, const floa
             case 10: LAUNCH(0, true, 0); break;        // drop-path scaling of a gradient (unit affine, per-sample gate)
             case 11: LAUNCH(0, true, 1); break;        // block tail with drop path: (scale*y + shift) * gate[n] + residual
             case 12: LAUNCH(0, true, 2); break;        // ResNet block tail with drop path: relu((scale*y + shift) * gate[n] + residual)
+            case 212: LAUNCH(2, true, 2); break;       // SE-ResNet basic block tail: relu(relu(scale*y + shift) * gate[n,c] + residual)
             case 100: LAUNCH(1, false, 0); break;
             case 110: LAUNCH(1, true, 0); break;
             case 200: LAUNCH(2, false, 0); break;
@@ -1309,7 +1405,7 @@ static RowGeom pool_geom(int C, long long hw, int n, int max_chunks) {
 }
 
 static int launch_pool(const void* y, const float* scale, const float* shift, float* pooled, int n, long long hw, int C,
-                       int act, int dt, int max_chunks, const SeFwdArgs& se, void* stream) {
+                       int act, int dt, int max_chunks, const SeFwdArgs& se, void* stream, int se_act = DFD_ACT_SWISH) {
     if (C % 8 || C <= 0 || hw <= 0 || n <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_pool: C%8, sizes");
     const RowGeom g = pool_geom(C, hw, n, max_chunks);
     cudaStream_t st = (cudaStream_t)stream;
@@ -1317,7 +1413,9 @@ static int launch_pool(const void* y, const float* scale, const float* shift, fl
     const size_t smem = reduce_smem(g) + (size_t)(C + se.Cse) * sizeof(float);
     if (smem > 48 * 1024) return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_pool: channel count exceeds shared memory");
     DISPATCH_T(dt, {
-        if (act == DFD_ACT_SWISH) pool_kernel<T, 1><<<g.grid, g.block, smem, st>>>((const T*)y, scale, shift, pooled, hw, rpb, se);
+        if (se_act == DFD_ACT_RELU && act == DFD_ACT_RELU) pool_kernel<T, 2, DFD_ACT_RELU><<<g.grid, g.block, smem, st>>>((const T*)y, scale, shift, pooled, hw, rpb, se);
+        else if (se_act == DFD_ACT_RELU) pool_kernel<T, 0, DFD_ACT_RELU><<<g.grid, g.block, smem, st>>>((const T*)y, scale, shift, pooled, hw, rpb, se);
+        else if (act == DFD_ACT_SWISH) pool_kernel<T, 1><<<g.grid, g.block, smem, st>>>((const T*)y, scale, shift, pooled, hw, rpb, se);
         else if (act == DFD_ACT_RELU) pool_kernel<T, 2><<<g.grid, g.block, smem, st>>>((const T*)y, scale, shift, pooled, hw, rpb, se);
         else pool_kernel<T, 0><<<g.grid, g.block, smem, st>>>((const T*)y, scale, shift, pooled, hw, rpb, se);
     });
@@ -1370,6 +1468,18 @@ int dfd_pool_se(const void* y, const float* scale, const float* shift, float* po
     if (!Wr || !br || !We || !be || !gate || Cse <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_pool_se: operands");
     SeFwdArgs se = {Wr, br, We, be, gate, Cse};
     return launch_pool(y, scale, shift, pooled, n, hw, C, act, dt, max_chunks, se, stream);
+}
+
+// SENet's SEModule (senet.py:67-86) on a BatchNorm output: pooled[n,c] = mean_hw act(scale*y + shift) (act NONE or RELU), then
+// gate[n,:] = sigmoid(We * relu(Wr * pooled[n,:] + br) + be) by the CTA that completed image n
+int dfd_pool_se_relu(const void* y, const float* scale, const float* shift, float* pooled, const float* Wr, const float* br,
+                     const float* We, const float* be, float* gate, int n, long long hw, int C, int Cse, int act, int dt,
+                     int max_chunks, void* stream) {
+    if (!scale || !shift || !Wr || !br || !We || !be || !gate || Cse <= 0)
+        return dfd_set_error(DFD_ERR_ARG, "dfd_pool_se_relu: operands");
+    if (act != DFD_ACT_NONE && act != DFD_ACT_RELU) return dfd_set_error(DFD_ERR_ARG, "dfd_pool_se_relu: act");
+    SeFwdArgs se = {Wr, br, We, be, gate, Cse};
+    return launch_pool(y, scale, shift, pooled, n, hw, C, act, dt, max_chunks, se, stream, DFD_ACT_RELU);
 }
 
 int dfd_bn_bwd_reduce(const void* g_, const void* y, const void* out, const float* mean, const float* rstd, int n,
@@ -1466,6 +1576,34 @@ int dfd_se_bwd_chain(const void* da, const void* y, const float* scale, const fl
         return dfd_set_error(DFD_ERR_ARG, "dfd_se_bwd_chain: operands");
     SeBwdArgs se = {pooled, Wr, br, We, be, d_e, r, d_rpre, dpool, Cse};
     return launch_se_bwd_reduce(da, y, scale, shift, draw, n, hw, C, dt, se, stream);
+}
+
+// SE-ResNet block tail backward in one pass over the block output (relu_se_bwd_reduce_kernel), its SE chain with the ReLU
+// inner activation in the CTA that completes each image; geometry and chunk order as dfd_se_bwd_chain
+int dfd_relu_se_bwd_reduce(const void* g_, const void* g2, const void* y, const void* out, const float* scale, const float* shift,
+                           void* gm, float* draw, const float* pooled, const float* Wr, const float* br, const float* We,
+                           const float* be, float* d_e, float* r, float* d_rpre, float* dpool, int n, long long hw, int C,
+                           int Cse, int act, int dt, void* stream) {
+    if (C % 8 || C <= 0 || hw <= 0 || n <= 0 || Cse <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_relu_se_bwd_reduce: C%8, sizes");
+    if (act != DFD_ACT_NONE && act != DFD_ACT_RELU) return dfd_set_error(DFD_ERR_ARG, "dfd_relu_se_bwd_reduce: act");
+    if (!g_ || !y || !out || !scale || !shift || !gm || !draw || !pooled || !Wr || !br || !We || !be || !d_e || !r || !d_rpre ||
+        !dpool)
+        return dfd_set_error(DFD_ERR_ARG, "dfd_relu_se_bwd_reduce: operands");
+    RowGeom g = make_geom(C, hw, n, n >= 296 ? 1 : 592, row_maxt(hw, true));
+    if ((long long)g.grid.x * n * C > ROWRED_WS_FLOATS || n > ROWRED_TICKETS) g = make_geom(C, hw, n, 1, row_maxt(hw, true));
+    const int nw = (int)(g.block.x * g.block.y) / 32;
+    const size_t smem = reduce_smem(g) + (size_t)(2 * C + (3 + nw) * Cse) * sizeof(float);
+    if (smem > 48 * 1024) return dfd_set_error(DFD_ERR_UNSUPPORTED, "dfd_relu_se_bwd_reduce: channel count exceeds shared memory");
+    SeBwdArgs se = {pooled, Wr, br, We, be, d_e, r, d_rpre, dpool, Cse};
+    cudaStream_t st = (cudaStream_t)stream;
+#define RSE_ARGS (const T*)g_, (const T*)g2, (const T*)y, (const T*)out, scale, shift, (T*)gm, draw, hw, (long long)g.rows_per_block, se
+    DISPATCH_T(dt, {
+        if (act == DFD_ACT_RELU) relu_se_bwd_reduce_kernel<T, DFD_ACT_RELU><<<g.grid, g.block, smem, st>>>(RSE_ARGS);
+        else relu_se_bwd_reduce_kernel<T, DFD_ACT_NONE><<<g.grid, g.block, smem, st>>>(RSE_ARGS);
+    });
+#undef RSE_ARGS
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
 }
 
 int dfd_act_bwd(const void* da, const void* y, const float* scale, const float* shift, const float* mean,

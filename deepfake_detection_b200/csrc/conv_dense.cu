@@ -133,6 +133,88 @@ __global__ void unpack_grad_kernel(const float* __restrict__ gperm, float* __res
     }
 }
 
+// 3x3 stride-2 max-pool WITHOUT padding in ceil mode (SENet's layer0.pool, senet.py:297-299: nn.MaxPool2d(3, 2,
+// ceil_mode=True)): Ho = ceil((H - 3) / 2) + 1, so over an even extent the last window starts at H - 2 and is clipped to two
+// rows. Arg-max byte and first-maximum tie-break as maxpool_fwd_kernel.
+template <typename T>
+__global__ void maxpool_ceil_fwd_kernel(const T* __restrict__ x, T* __restrict__ out, unsigned char* __restrict__ idx, int N,
+                                        int H, int W, int C, int Ho, int Wo) {
+    const int V = C / 8;
+    const long long total = (long long)N * Ho * Wo * V;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        int v = (int)(i % V);
+        long long t = i / V;
+        int ox = (int)(t % Wo);
+        long long t2 = t / Wo;
+        int oy = (int)(t2 % Ho);
+        int n = (int)(t2 / Ho);
+        float best[8];
+        unsigned char bi[8];
+#pragma unroll
+        for (int j = 0; j < 8; j++) { best[j] = -INFINITY; bi[j] = 0; }
+        for (int kh = 0; kh < 3; kh++) {
+            int iy = oy * 2 + kh;
+            if (iy >= H) break;
+            for (int kw = 0; kw < 3; kw++) {
+                int ix = ox * 2 + kw;
+                if (ix >= W) break;
+                float f[8];
+                unpack8<T>(ldg16(x + (((size_t)n * H + iy) * W + ix) * C + v * 8), f);
+#pragma unroll
+                for (int j = 0; j < 8; j++)
+                    if (f[j] > best[j]) { best[j] = f[j]; bi[j] = (unsigned char)(kh * 3 + kw); }
+            }
+        }
+        stg16(out + (size_t)t * C + v * 8, pack8<T>(best));
+        uint2 pk;
+        pk.x = bi[0] | (bi[1] << 8) | (bi[2] << 16) | (bi[3] << 24);
+        pk.y = bi[4] | (bi[5] << 8) | (bi[6] << 16) | (bi[7] << 24);
+        *reinterpret_cast<uint2*>(idx + (size_t)t * C + v * 8) = pk;
+    }
+}
+// its gradient, gathered per input pixel (no atomics): gx[iy, ix] = sum of gy over the windows (oy, ox) with iy = 2 oy + kh,
+// ix = 2 ox + kw whose arg-max is (kh, kw)
+template <typename T>
+__global__ void maxpool_ceil_bwd_kernel(const T* __restrict__ gy, const unsigned char* __restrict__ idx, T* __restrict__ gx,
+                                        int N, int H, int W, int C, int Ho, int Wo) {
+    const int V = C / 8;
+    const long long total = (long long)N * H * W * V;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        int v = (int)(i % V);
+        long long t = i / V;
+        int ix = (int)(t % W);
+        long long t2 = t / W;
+        int iy = (int)(t2 % H);
+        int n = (int)(t2 / H);
+        float acc[8];
+#pragma unroll
+        for (int j = 0; j < 8; j++) acc[j] = 0.f;
+        for (int kh = 0; kh < 3; kh++) {
+            int a = iy - kh;
+            if (a < 0 || (a & 1)) continue;
+            int oy = a >> 1;
+            if (oy >= Ho) continue;
+            for (int kw = 0; kw < 3; kw++) {
+                int b = ix - kw;
+                if (b < 0 || (b & 1)) continue;
+                int ox = b >> 1;
+                if (ox >= Wo) continue;
+                size_t o = (((size_t)n * Ho + oy) * Wo + ox) * C + v * 8;
+                uint2 pk = *reinterpret_cast<const uint2*>(idx + o);
+                float g[8];
+                unpack8<T>(ldg16(gy + o), g);
+                const unsigned char want = (unsigned char)(kh * 3 + kw);
+#pragma unroll
+                for (int j = 0; j < 8; j++) {
+                    unsigned char bj = (unsigned char)(((j < 4 ? pk.x : pk.y) >> ((j & 3) * 8)) & 0xff);
+                    if (bj == want) acc[j] += g[j];
+                }
+            }
+        }
+        stg16(gx + (size_t)t * C + v * 8, pack8<T>(acc));
+    }
+}
+
 // 3x3 stride-2 pad-1 max-pool; the arg-max (first maximum in row-major window order, as ATen's CPU/CUDA kernels) is kept
 // in one byte per output so that backward routes ties (frequent after ReLU) exactly like the reference.
 template <typename T>
@@ -407,6 +489,32 @@ int dfd_maxpool_bwd(const void* gy, const void* idx, void* gx, int N, int H, int
     int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
     long long total = (long long)N * H * W * (C / 8);
     CD_T(dt, (maxpool_bwd_kernel<T><<<nblocks(total), 256, 0, (cudaStream_t)stream>>>((const T*)gy, (const unsigned char*)idx, (T*)gx, N, H, W, C, Ho, Wo)));
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+// output extent of nn.MaxPool2d(3, 2, padding=0, ceil_mode=True) over an input extent h >= 3 (torch's pooling_output_shape:
+// ceil((h - 3) / 2) + 1, less one when the last window would start outside the input)
+static int ceil_pool_out(int h) {
+    int o = (h - 3 + 1) / 2 + 1;
+    if ((o - 1) * 2 >= h) o--;
+    return o;
+}
+
+int dfd_maxpool_ceil_fwd(const void* x, void* out, void* idx, int N, int H, int W, int C, int dt, void* stream) {
+    if (C % 8 || C <= 0 || N <= 0 || H < 3 || W < 3) return dfd_set_error(DFD_ERR_ARG, "dfd_maxpool_ceil_fwd: C%8, sizes");
+    int Ho = ceil_pool_out(H), Wo = ceil_pool_out(W);
+    long long total = (long long)N * Ho * Wo * (C / 8);
+    CD_T(dt, (maxpool_ceil_fwd_kernel<T><<<nblocks(total), 256, 0, (cudaStream_t)stream>>>((const T*)x, (T*)out, (unsigned char*)idx, N, H, W, C, Ho, Wo)));
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+int dfd_maxpool_ceil_bwd(const void* gy, const void* idx, void* gx, int N, int H, int W, int C, int dt, void* stream) {
+    if (C % 8 || C <= 0 || N <= 0 || H < 3 || W < 3) return dfd_set_error(DFD_ERR_ARG, "dfd_maxpool_ceil_bwd: C%8, sizes");
+    int Ho = ceil_pool_out(H), Wo = ceil_pool_out(W);
+    long long total = (long long)N * H * W * (C / 8);
+    CD_T(dt, (maxpool_ceil_bwd_kernel<T><<<nblocks(total), 256, 0, (cudaStream_t)stream>>>((const T*)gy, (const unsigned char*)idx, (T*)gx, N, H, W, C, Ho, Wo)));
     DFD_LAUNCH_CHECK();
     return DFD_OK;
 }

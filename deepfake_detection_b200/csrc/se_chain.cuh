@@ -8,8 +8,20 @@
 
 __device__ __forceinline__ float se_swish_precise(float x) { return x * sigmoid_precise(x); }
 
+// inner activation of the chain: DFD_ACT_SWISH (EfficientNet's SqueezeExcite) or DFD_ACT_RELU (SENet's SEModule,
+// senet.py:67-86); its derivative in terms of the pre-activation x
+template <int INNER> __device__ __forceinline__ float se_inner(float x) {
+    return INNER == DFD_ACT_RELU ? fmaxf(x, 0.f) : se_swish_precise(x);
+}
+template <int INNER> __device__ __forceinline__ float se_inner_grad(float x) {
+    if (INNER == DFD_ACT_RELU) return x > 0.f ? 1.f : 0.f;
+    const float sg = sigmoid_precise(x);
+    return sg * (1.f + x * (1.f - sg));
+}
+
 // p: [C] pooled activations of this image in SHARED memory; r: [Cse] shared scratch.
-// gate[c] = sigmoid(be[c] + sum_j We[c,j] * swish(br[j] + sum_c' Wr[j,c'] p[c']))
+// gate[c] = sigmoid(be[c] + sum_j We[c,j] * inner(br[j] + sum_c' Wr[j,c'] p[c'])), inner = swish or ReLU
+template <int INNER = DFD_ACT_SWISH>
 __device__ __forceinline__ void se_fwd_chain(const float* p, float* r, const float* __restrict__ Wr,
                                              const float* __restrict__ br, const float* __restrict__ We,
                                              const float* __restrict__ be, float* __restrict__ gate_out, int C, int Cse,
@@ -21,7 +33,7 @@ __device__ __forceinline__ void se_fwd_chain(const float* p, float* r, const flo
             float s = 0.f;
             for (int c = lane; c < C; c += 32) s = fmaf(w[c], p[c], s);
             s = warp_sum(s);
-            if (lane == 0) r[j] = se_swish_precise(s + br[j]);
+            if (lane == 0) r[j] = se_inner<INNER>(s + br[j]);
         }
     __syncthreads();
     // one thread per output row: a row is Cse consecutive floats, so the warp's 32 rows stay L1-resident across the j loop
@@ -36,6 +48,7 @@ __device__ __forceinline__ void se_fwd_chain(const float* p, float* r, const flo
 // shared scratch `sm`: p [C] (in), de [C], rpre / r / drp [Cse] each, r_part [nw][Cse]   = 2C + (3 + nw) Cse floats.
 // draw: dL/dgate of this image in SHARED or global memory (read once per channel).
 // Emits d_e [C], r [Cse], d_rpre [Cse] (operands of the SE parameter gradients) and dpool [C] to global memory.
+template <int INNER = DFD_ACT_SWISH>
 __device__ __forceinline__ void se_bwd_chain(float* sm, const float* draw, const float* __restrict__ Wr,
                                              const float* __restrict__ br, const float* __restrict__ We,
                                              const float* __restrict__ be, float* __restrict__ d_e_out,
@@ -54,7 +67,7 @@ __device__ __forceinline__ void se_bwd_chain(float* sm, const float* draw, const
             float s = 0.f;
             for (int c = lane; c < C; c += 32) s = fmaf(w[c], p[c], s);
             s = warp_sum(s);
-            if (lane == 0) { rpre[j] = s + br[j]; r[j] = se_swish_precise(s + br[j]); }
+            if (lane == 0) { rpre[j] = s + br[j]; r[j] = se_inner<INNER>(s + br[j]); }
         }
     __syncthreads();
     for (int c = tid; c < C; c += nt) {
@@ -82,9 +95,7 @@ __device__ __forceinline__ void se_bwd_chain(float* sm, const float* draw, const
     for (int j = tid; j < Cse; j += nt) {
         float s = 0.f;
         for (int w = 0; w < nw; w++) s += r_part[w * Cse + j];
-        const float x = rpre[j];
-        const float sg = sigmoid_precise(x);
-        const float v = s * (sg * (1.f + x * (1.f - sg)));
+        const float v = s * se_inner_grad<INNER>(rpre[j]);
         drp[j] = v;
         d_rpre_out[j] = v;
         r_out[j] = r[j];

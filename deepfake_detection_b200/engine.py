@@ -62,7 +62,7 @@ class Engine:
                                    "there is no CPU path")
         self.L = _lib.lib()
         self.spec = spec = get_spec(arch, num_classes=num_classes, in_chans=in_chans, global_pool=global_pool)
-        self.cls_name = "classifier" if spec.family == "efficientnet" else "fc"
+        self.cls_name = "classifier" if spec.family == "efficientnet" else (spec.cls_name if spec.family == "resnet" else "fc")
         self.device = torch.device(device if device is not None else "cuda:%d" % torch.cuda.current_device())
         self.N = int(batch)
         self.H = int(height or spec.input_size[1])

@@ -25,6 +25,15 @@ a gathered copy of its input.
 
 1x1 convolutions are plain GEMMs on the NHWC tensors. BN + ReLU outputs are materialised (`dfd_bn_act`) because three
 consumers read them.
+
+SE-ResNets (seresnet18/34/50/101/152, senet.py): the stem pool is MaxPool2d(3, 2, ceil_mode=True) without padding
+(`dfd_maxpool_ceil_fwd` / `_bwd`); the bottleneck's stride sits on its 1x1 conv1 (the strided implicit GEMM of the downsample,
+whose input gradient is added by `dfd_conv1x1_dgrad_add` into the zeroed block-input gradient together with the downsample's);
+every block ends in an SEModule on its last BN output (after a ReLU in the basic block, senet.py:213-215): `dfd_pool_se_relu`
+pools it and computes the gate [N, C] (training and eval), and the tail `dfd_bn_act` (gate, residual, ReLU) applies it.
+Backward: `dfd_relu_se_bwd_reduce` forms the masked gradient gm of the block output, dL/dgate and the SE chain in one pass;
+`dfd_act_bwd` (gate and dpool) forms the last BN's input gradient (gm * gate + dpool / HW) * act' with its BN-backward sums;
+`dfd_se_fc_wgrad` the SE parameter gradients.
 """
 import struct
 from collections import OrderedDict
@@ -33,7 +42,8 @@ from functools import partial
 import torch
 
 from . import _lib
-from .engine import ACT_NONE, ACT_RELU, _ptr
+from .arch import stem_pool_out
+from .engine import ACT_NONE, ACT_RELU, POOL_CHUNKS, _ptr
 
 
 def conv_out(h, k, s, p):
@@ -83,7 +93,7 @@ def build_resnet(e):
     pk_off, off = {}, 0
     for n in e.param_names:
         o, s, k = e.p_off[n]
-        if len(s) == 4 and s[2] > 1 and n not in ("conv1.weight", "conv1.0.weight"):    # not the stem-GEMM weights
+        if len(s) == 4 and s[2] > 1 and n not in (spec.stem_conv + ".weight", "conv1.0.weight"):    # not the stem-GEMM weights
             pk_off[n] = (off, s[0], s[1], s[2])
             off += (k + 7) // 8 * 8
     ar = e.arena        # the packed layouts depend on the parameter shapes only: owned and refreshed by the arena engine
@@ -116,13 +126,17 @@ def build_resnet(e):
         raise ValueError("stem_impl=%r: the deep stem's first convolution is planned through dfd_stem_im2col (stem_impl='gemm')"
                          % (e.stem_impl,))
     sw = spec.stem_width
+    stem_w, stem_bn = spec.stem_conv + ".weight", spec.stem_bn
+    se = spec.se_reduction > 0
+    if se and (e.drop_path_rate > 0.0 or (e.drop_block_rate or 0.0) > 0.0):
+        raise ValueError("%s: the SE-ResNet has no drop path or DropBlock (SENet takes neither, senet.py:226-230)" % spec.arch)
 
     # ---- shapes ------------------------------------------------------------------------------------------
     if deep:
         H1, W1 = conv_out(e.H, 3, 2, 1), conv_out(e.W, 3, 2, 1)
     else:
         H1, W1 = conv_out(e.H, 7, 2, 3), conv_out(e.W, 7, 2, 3)
-    H2, W2 = conv_out(H1, 3, 2, 1), conv_out(W1, 3, 2, 1)
+    H2, W2 = stem_pool_out(H1, spec.stem_pool), stem_pool_out(W1, spec.stem_pool)
     shapes = []
     h, w = H2, W2
     for b in spec.blocks:
@@ -132,7 +146,7 @@ def build_resnet(e):
     Hf, Wf = h, w
 
     # ---- BN arenas ---------------------------------------------------------------------------------------
-    bn_specs = ([("conv1.1", sw), ("conv1.4", sw)] if deep else []) + [("bn1", 64)]
+    bn_specs = ([("conv1.1", sw), ("conv1.4", sw)] if deep else []) + [(stem_bn, 64)]
     for b in spec.blocks:
         if b.kind == "basic":
             bn_specs += [(b.name + ".bn1", b.planes), (b.name + ".bn2", b.cout)]
@@ -218,7 +232,7 @@ def build_resnet(e):
     a0 = e._alloc16(N, H1, W1, 64)
     x0 = e._alloc16(N, H2, W2, 64)
     e.pool_idx = torch.zeros(N * H2 * W2 * 64, dtype=torch.uint8, device=dev)
-    bn0 = bns["bn1"]
+    bn0 = bns[stem_bn]
     if deep:
         # conv1.0 (3x3 s2, in_chans -> sw) as im2col + GEMM, conv1.3 / conv1.6 (Cin = sw) through conv3x3's im2col route
         bs0, bs1 = bns["conv1.1"], bns["conv1.4"]
@@ -234,18 +248,26 @@ def build_resnet(e):
         fwd.append(bn_relu(ys1, bs1, as1, H1 * W1, sw))
         fwd += conv3x3(_ptr(as1), "conv1.6.weight", _ptr(y0), H1, W1, sw, 64, 1, bn0)
     elif e.stem_impl == "gemm":
-        taps, Kp = e._stem_gemm_setup("conv1.weight", 64, 7, N * H1 * W1)
+        taps, Kp = e._stem_gemm_setup(stem_w, 64, 7, N * H1 * W1)
         fwd.append(("dfd_stem_im2col", (_ptr(e.x_in), _ptr(e.stem_cols), N, spec.in_chans, e.H, e.W, 7, 2, 3, Kp, dt)))
         fwd.append(gemm(_ptr(e.stem_cols), _ptr(e.stem_wpad), _ptr(y0), N * H1 * W1, 64, Kp, bn0))
     else:
-        fwd.append(("dfd_stem_fwd", (_ptr(e.x_in), P32("conv1.weight"), _ptr(y0), N, spec.in_chans, e.H, e.W, 64, 7, 2, 3, dt)
+        fwd.append(("dfd_stem_fwd", (_ptr(e.x_in), P32(stem_w), _ptr(y0), N, spec.in_chans, e.H, e.W, 64, 7, 2, 3, dt)
                     + e._stats(bn0)))
     fwd += finalize(bn0, N * H1 * W1)
     fwd.append(bn_relu(y0, bn0, a0, H1 * W1, 64))
-    fwd.append(("dfd_maxpool_fwd", (_ptr(a0), _ptr(x0), _ptr(e.pool_idx), N, H1, W1, 64, dt)))
+    pool_op = "dfd_maxpool_ceil" if spec.stem_pool == "ceil" else "dfd_maxpool"
+    fwd.append((pool_op + "_fwd", (_ptr(a0), _ptr(x0), _ptr(e.pool_idx), N, H1, W1, 64, dt)))
     e.acts["stem.out"] = x0
     x = x0
     recs = []
+    if se:
+        # per-image SE vectors of the backward, shared by the blocks (consumed within the block): dL/dgate, d_e, dpool [N, C];
+        # r, d_rpre [N, Cse]
+        cmax, rmax = max(b.cout for b in spec.blocks), max(b.cse for b in spec.blocks)
+        e.se_tmp = torch.zeros(3 * N * cmax + 2 * N * rmax, dtype=torch.float32, device=dev)
+        se_draw, se_de, se_dpool = [_ptr(e.se_tmp, i * N * cmax) for i in range(3)]
+        se_r, se_drp = _ptr(e.se_tmp, 3 * N * cmax), _ptr(e.se_tmp, 3 * N * cmax + N * rmax)
     for b, h, w, ho, wo in shapes:
         p = b.name
         M1, M2 = N * h * w, N * ho * wo
@@ -263,20 +285,34 @@ def build_resnet(e):
             rec.update(y1=y1, a1=a1, ylast=y2, bnlast=bn2, site_last=p + ".bn2")
         else:
             bn1, bn2, bn3 = bns[p + ".bn1"], bns[p + ".bn2"], bns[p + ".bn3"]
-            y1 = e._alloc16(N, h, w, b.width)
-            a1 = e._alloc16(N, h, w, b.width)
+            # SE-ResNet bottleneck: the stride on the 1x1 conv1, conv2 at stride 1 (senet.py:141-163)
+            s1x1 = spec.stride_in_1x1 and b.stride != 1
+            h1, w1 = (ho, wo) if s1x1 else (h, w)
+            M1b = N * h1 * w1
+            y1 = e._alloc16(N, h1, w1, b.width)
+            a1 = e._alloc16(N, h1, w1, b.width)
             y2 = e._alloc16(N, ho, wo, b.width)
             a2 = e._alloc16(N, ho, wo, b.width)
             y3 = e._alloc16(N, ho, wo, b.cout)
-            fwd.append(gemm(_ptr(x), P16(p + ".conv1.weight"), _ptr(y1), M1, b.width, b.cin, bn1))
-            fwd += finalize(bn1, M1)
-            fwd.append(bn_relu(y1, bn1, a1, h * w, b.width, p + ".bn1"))
-            fwd += conv3x3(_ptr(a1), p + ".conv2.weight", _ptr(y2), h, w, b.width, b.width, b.stride, bn2)
+            xs1 = None
+            if not s1x1:
+                fwd.append(gemm(_ptr(x), P16(p + ".conv1.weight"), _ptr(y1), M1, b.width, b.cin, bn1))
+            elif implicit and b.cin % 64 == 0 and b.width % 64 == 0:
+                # strided 1x1 straight from the block input, as the downsample below
+                fwd.append(("dfd_conv_tc", (_ptr(x), P16(p + ".conv1.weight"), _ptr(y1), N, h, w, b.cin, b.width, 1, b.stride, dt)
+                            + e._stats(bn1) + (None,)))
+            else:
+                xs1 = e._alloc16(N, ho, wo, b.cin)
+                fwd.append(("dfd_im2col", (_ptr(x), _ptr(xs1), N, h, w, b.cin, 1, b.stride, 0, dt)))
+                fwd.append(gemm(_ptr(xs1), P16(p + ".conv1.weight"), _ptr(y1), M2, b.width, b.cin, bn1))
+            fwd += finalize(bn1, M1b)
+            fwd.append(bn_relu(y1, bn1, a1, h1 * w1, b.width, p + ".bn1"))
+            fwd += conv3x3(_ptr(a1), p + ".conv2.weight", _ptr(y2), h1, w1, b.width, b.width, 1 if s1x1 else b.stride, bn2)
             fwd += finalize(bn2, M2)
             fwd.append(bn_relu(y2, bn2, a2, ho * wo, b.width, p + ".bn2"))
             fwd.append(gemm(_ptr(a2), P16(p + ".conv3.weight"), _ptr(y3), M2, b.cout, b.width, bn3))
             fwd += finalize(bn3, M2)
-            rec.update(y1=y1, a1=a1, y2=y2, a2=a2, ylast=y3, bnlast=bn3, site_last=p + ".bn3")
+            rec.update(y1=y1, a1=a1, y2=y2, a2=a2, ylast=y3, bnlast=bn3, site_last=p + ".bn3", s1x1=s1x1, xs1=xs1)
         res = x
         if b.downsample:
             dsw, dsbn = [p + n for n in ds_names(b)]
@@ -309,7 +345,21 @@ def build_resnet(e):
         bl = rec["bnlast"]
         gate = e.drop_masks.get(p)
         rec["gate"] = gate
-        if rec["site_last"] in sites:
+        if b.cse:
+            # SEModule on the last BN output: pooled [N, C] and the gate [N, C], in eval plans too
+            sep = p + ".se_module."
+            pooled = torch.zeros(N, b.cout, dtype=torch.float32, device=dev)
+            sgate = torch.zeros(N, b.cout, dtype=torch.float32, device=dev)
+            e._keep += [pooled, sgate]
+            rec.update(se_pooled=pooled, se_gate=sgate, se_w=[sep + n for n in ("fc1.weight", "fc1.bias", "fc2.weight", "fc2.bias")])
+            # the SE input: the bare bn3 output of a bottleneck, ReLU(bn2) of a basic block (senet.py:94-114, 206-223)
+            se_act = ACT_RELU if b.kind == "basic" else ACT_NONE
+            rec["se_act"] = se_act
+            fwd.append(("dfd_pool_se_relu", (_ptr(rec["ylast"]), bl.scale, bl.shift, _ptr(pooled))
+                        + tuple(P32(n) for n in rec["se_w"]) + (_ptr(sgate), N, ho * wo, b.cout, b.cse, se_act, dt, POOL_CHUNKS)))
+            fwd.append(("dfd_bn_act", (_ptr(rec["ylast"]), bl.scale, bl.shift, _ptr(sgate), _ptr(res), _ptr(out), N, ho * wo,
+                                       b.cout, se_act, 2, dt)))
+        elif rec["site_last"] in sites:
             m, k, numel = site_args(rec["site_last"])
             fwd.append(("dfd_bn_act_drop", [_ptr(rec["ylast"]), bl.scale, bl.shift, ("TRAIN_ONLY", m), k, numel,
                                             ("TRAIN_ONLY", _ptr(gate)) if gate is not None else None, _ptr(res), _ptr(out), N,
@@ -382,7 +432,8 @@ def build_resnet(e):
         pending_unpack.append((gp, name, Cout, Cin))     # complete after the block's ordered reduce (flush_block)
         return ops
 
-    bwd.append(("dfd_head_bwd", (_ptr(e.dlogits), _ptr(e.pooled), P32("fc.weight"), G32("fc.weight"), G32("fc.bias"),
+    bwd.append(("dfd_head_bwd", (_ptr(e.dlogits), _ptr(e.pooled), P32(e.cls_name + ".weight"), G32(e.cls_name + ".weight"),
+                                 G32(e.cls_name + ".bias"),
                                  _ptr(e.dpooled), N, P, K)))
     if e.drop_rate > 0.0:
         bwd.append(("dfd_mul_f32", (_ptr(e.dpooled), _ptr(e.dropout_mask), N * P)))
@@ -410,7 +461,18 @@ def build_resnet(e):
         M1, M2 = N * h * w, N * ho * wo
         gm, t1, t2, t3 = [g for g in bufs if g not in (dout, dout2)][:4]
         bl = rec["bnlast"]
-        if rec["site_last"] in sites or rec["gate"] is not None:
+        if b.cse:
+            # gm = (dout + dout2) * (out > 0) stored, dL/dgate and the SE backward chain in one pass; then the last BN's input
+            # gradient (gm * gate + dpool / HW) * act' (with its BN-backward sums) in t2 and the SE parameter gradients
+            Wr, br, We, be = rec["se_w"]
+            bwd.append(("dfd_relu_se_bwd_reduce", (dout, dout2, _ptr(rec["ylast"]), _ptr(rec["out"]), bl.scale, bl.shift, gm, se_draw,
+                                                   _ptr(rec["se_pooled"]), P32(Wr), P32(br), P32(We), P32(be), se_de, se_r, se_drp,
+                                                   se_dpool, N, ho * wo, b.cout, b.cse, rec["se_act"], dt)))
+            bwd.append(("dfd_act_bwd", (gm, _ptr(rec["ylast"]), bl.scale, bl.shift, bl.mean, bl.rstd, _ptr(rec["se_gate"]), se_dpool,
+                                        t2, N, ho * wo, b.cout, rec["se_act"], dt, bl.bs1, bl.bs2, None)))
+            bwd.append(("dfd_se_fc_wgrad", (se_de, se_r, se_drp, _ptr(rec["se_pooled"]), G32(Wr), G32(br), G32(We), G32(be), N,
+                                            b.cout, b.cse)))
+        elif rec["site_last"] in sites or rec["gate"] is not None:
             # gm goes unmasked to the identity / downsample path; the last BN sees gd = gm * (DropBlock) * (drop path) in t2
             m, k, numel = site_args(rec["site_last"]) if rec["site_last"] in sites else (None, None, 0)
             gate = _ptr(rec["gate"]) if rec["gate"] is not None else None
@@ -421,7 +483,7 @@ def build_resnet(e):
             # the residual add, the ReLU backward and the reduction)
             bwd.append(("dfd_relu_bn_bwd_reduce", (dout, dout2, _ptr(rec["ylast"]), _ptr(rec["out"]), gm, bl.mean, bl.rstd, N, ho * wo,
                                                    b.cout, dt, bl.bs1, bl.bs2)))
-        gd = t2 if (rec["site_last"] in sites or rec["gate"] is not None) else gm
+        gd = t2 if (b.cse or rec["site_last"] in sites or rec["gate"] is not None) else gm
         bwd += bwd_finalize(bl, M2)
         bwd.append(("dfd_bn_bwd_apply", (gd, _ptr(rec["ylast"]), None, bl.cA, bl.cB, bl.cC, t1, N, ho * wo, b.cout, dt)))
         if b.kind == "basic":
@@ -441,14 +503,30 @@ def build_resnet(e):
             bwd.append(relu_bwd(t2, rec["y2"], bn2, t1, ho * wo, b.width, p + ".bn2"))
             bwd += bwd_finalize(bn2, M2)
             bwd.append(("dfd_bn_bwd_apply", (t1, _ptr(rec["y2"]), None, bn2.cA, bn2.cB, bn2.cC, t2, N, ho * wo, b.width, dt)))
-            # conv2 (3x3 stride s): dy2 = t2 -> da1 = t1 [M1, width]
-            bwd += conv3x3_bwd(p + ".conv2.weight", t2, M2, b.width, b.width, rec["a1"], h, w, b.stride, t1)
-            bwd.append(relu_bwd(t1, rec["y1"], bn1, t2, h * w, b.width, p + ".bn1"))
-            bwd += bwd_finalize(bn1, M1)
-            bwd.append(("dfd_bn_bwd_apply", (t2, _ptr(rec["y1"]), None, bn1.cA, bn1.cB, bn1.cC, t1, N, h * w, b.width, dt)))
-            # conv1 (1x1): dy1 = t1 -> dx = t3 [M1, cin]
-            bwd.append(gemm(t1, T16(p + ".conv1.weight"), t3, M1, b.cin, b.width))
-            bwd.append(e._wgrad(t1, _ptr(xin), G32(p + ".conv1.weight"), M1, b.width, b.cin))
+            s1x1 = rec["s1x1"]
+            h1, w1 = (ho, wo) if s1x1 else (h, w)
+            M1b = N * h1 * w1
+            # conv2 (3x3 stride s, or 1 when the stride is on conv1): dy2 = t2 -> da1 = t1 [M1b, width]
+            bwd += conv3x3_bwd(p + ".conv2.weight", t2, M2, b.width, b.width, rec["a1"], h1, w1, 1 if s1x1 else b.stride, t1)
+            bwd.append(relu_bwd(t1, rec["y1"], bn1, t2, h1 * w1, b.width, p + ".bn1"))
+            bwd += bwd_finalize(bn1, M1b)
+            bwd.append(("dfd_bn_bwd_apply", (t2, _ptr(rec["y1"]), None, bn1.cA, bn1.cB, bn1.cC, t1, N, h1 * w1, b.width, dt)))
+            c1 = p + ".conv1.weight"
+            if not s1x1:
+                # conv1 (1x1): dy1 = t1 -> dx = t3 [M1, cin]
+                bwd.append(gemm(t1, T16(c1), t3, M1, b.cin, b.width))
+                bwd.append(e._wgrad(t1, _ptr(xin), G32(c1), M1, b.width, b.cin))
+            elif rec["xs1"] is None:
+                # strided 1x1 conv1: its input gradient only reaches the stride-2 pixels, added into the zeroed t3 (the downsample's
+                # gradient is added into the same buffer below)
+                bwd.append(("dfd_memset_async", (t3, 0, M1 * b.cin * e.gbuf[0].element_size())))
+                bwd.append(("dfd_conv1x1_dgrad_add", (t1, T16(c1), t3, N, h, w, b.cin, b.width, b.stride, dt)))
+                bwd.append(e._wgrad_conv(t1, _ptr(xin), G32(c1), N, h, w, b.cin, b.width, 1, b.stride))
+            else:
+                # explicit formulation: the gradient of the gathered input, scattered onto the input grid (zeros elsewhere)
+                bwd.append(gemm(t1, T16(c1), t2, M2, b.cin, b.width))
+                bwd.append(("dfd_col2im", (t2, None, t3, N, h, w, b.cin, 1, b.stride, 0, dt)))
+                bwd.append(e._wgrad(t1, _ptr(rec["xs1"]), G32(c1), M2, b.width, b.cin))
         # identity / downsample path: gradient gm flows to the block input too
         if b.downsample:
             bnd = rec["bnd"]
@@ -491,7 +569,7 @@ def build_resnet(e):
     if dout2 is not None:
         bwd.append(("dfd_add_inplace", (dout, dout2, N * H2 * W2 * 64, dt)))
     t1, t2 = [g for g in bufs if g != dout][:2]
-    bwd.append(("dfd_maxpool_bwd", (dout, _ptr(e.pool_idx), t1, N, H1, W1, 64, dt)))
+    bwd.append((pool_op + "_bwd", (dout, _ptr(e.pool_idx), t1, N, H1, W1, 64, dt)))
     bwd.append(("dfd_act_bwd", (t1, _ptr(y0), bn0.scale, bn0.shift, bn0.mean, bn0.rstd, None, None, t2, N, H1 * W1, 64,
                                 ACT_RELU, dt, bn0.bs1, bn0.bs2, None)))
     bwd += bwd_finalize(bn0, N * H1 * W1)
@@ -517,8 +595,8 @@ def build_resnet(e):
         bwd.append(("dfd_memset_async", (_ptr(e.stem_gpad), 0, 64 * Kp * 4)))
         bwd.append(e._wgrad(t1, _ptr(e.stem_cols), _ptr(e.stem_gpad), N * H1 * W1, 64, Kp))
         e._flush_reduce(bwd)
-        bwd.append(("dfd_unpad_grad", (_ptr(e.stem_gpad), G32("conv1.weight"), 64, taps, Kp)))
+        bwd.append(("dfd_unpad_grad", (_ptr(e.stem_gpad), G32(stem_w), 64, taps, Kp)))
     else:
-        bwd.append(("dfd_stem_wgrad", (_ptr(e.x_in), t2, _ptr(y0), bn0.cA, bn0.cB, bn0.cC, G32("conv1.weight"), N, spec.in_chans,
+        bwd.append(("dfd_stem_wgrad", (_ptr(e.x_in), t2, _ptr(y0), bn0.cA, bn0.cB, bn0.cC, G32(stem_w), N, spec.in_chans,
                                        e.H, e.W, 64, 7, 2, 3, dt)))
     e._finish_plan(fwd, bwd)

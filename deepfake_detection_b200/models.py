@@ -18,7 +18,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .arch import RESNET_ARCHS, SUPPORTED_ARCHS, TF_ARCHS, TF_POOL_CROP, XCEPTION_ARCHS, get_spec, state_entries
+from .arch import RESNET_ARCHS, SENET_ARCHS, SUPPORTED_ARCHS, TF_ARCHS, TF_POOL_CROP, XCEPTION_ARCHS, get_spec, state_entries
 from .engine import Engine
 
 _DEFAULT_CFG = dict(num_classes=1000, pool_size=(7, 7), crop_pct=0.875, interpolation="bicubic",
@@ -29,8 +29,10 @@ _RESNET_BICUBIC = ("resnet26", "resnet26d", "resnet50d")
 # xception.py:27-38
 _XCEPTION_CFG = dict(input_size=(3, 299, 299), crop_pct=0.8975, interpolation="bicubic", mean=(0.5, 0.5, 0.5),
                      std=(0.5, 0.5, 0.5), first_conv="conv1", classifier="fc")
-# Xception.__init__ takes num_classes, in_chans, drop_rate and global_pool only (xception.py:132)
+# Xception.__init__ takes num_classes, in_chans, drop_rate and global_pool only (xception.py:132); so does SENet.__init__ beyond
+# what the seresnet* entrypoints pass themselves (senet.py:228-230, 399-461)
 _XCEPTION_KWARGS = ("drop_rate", "global_pool", "dtype", "gemm_impl")
+SENET_DROP_RATE = 0.2       # SENet.__init__'s default (senet.py:228): dropout on the pooled vector unless drop_rate is given
 
 
 class _NativeForward(torch.autograd.Function):
@@ -73,14 +75,17 @@ def init_state_dict(spec, seed=None):
     ResNet: resnet.py:410-420 (conv kaiming_normal fan_out, BN 1 / 0, the LAST BN gamma of every residual block ZERO -
     `zero_init_last_bn=True` is the constructor default, :353 - and nn.Linear's default U(+-1/sqrt(fan_in)) for fc);
     Xception: xception.py:171-177 (every nn.Conv2d, depthwise included, kaiming_normal fan_out = out_channels * k * k - torch
-    does not divide by the groups - BN 1 / 0, nn.Linear's default init for fc)."""
+    does not divide by the groups - BN 1 / 0, nn.Linear's default init for fc);
+    SE-ResNet: senet.py:59-64,344-345 (every nn.Conv2d, the SE FCs included, kaiming_normal fan_out, BN 1 / 0 with no zero-init
+    of the last gamma; the SE biases keep nn.Conv2d's default U(+-1/sqrt(fan_in)) and last_linear nn.Linear's default)."""
     import math
     g = torch.Generator(device="cpu").manual_seed((torch.initial_seed() if seed is None else seed) % (2 ** 31))
     sd = OrderedDict()
     resnet = spec.family == "resnet"
+    senet = resnet and spec.naming == "senet"
     fan_in_fc = spec.family in ("resnet", "xception")
     last_bn = set()
-    if resnet:
+    if resnet and not senet:
         for b in spec.blocks:
             last_bn.add(b.name + (".bn2.weight" if b.kind == "basic" else ".bn3.weight"))       # resnet.py:147-148,212-213
     for name, shape, role in state_entries(spec):
@@ -90,6 +95,10 @@ def init_state_dict(spec, seed=None):
             continue
         if name in last_bn:
             sd[name] = torch.zeros(shape)
+            continue
+        if senet and role == "se_b":
+            r = 1.0 / math.sqrt(sd[name[: -len("bias")] + "weight"].shape[1])     # fan_in of the 1x1 FC
+            sd[name] = (torch.rand(shape, generator=g) * 2 - 1) * r
             continue
         if role in ("conv_w", "dw_w", "se_w"):
             fan_out = shape[0] * shape[2] * shape[3]
@@ -138,6 +147,9 @@ class NativeModel(nn.Module):
         self.default_cfg = dict(_DEFAULT_CFG, input_size=self.spec.input_size,
                                 first_conv="conv_stem" if self.spec.family == "efficientnet" else "conv1",
                                 classifier="classifier" if self.spec.family == "efficientnet" else "fc")
+        if arch in SENET_ARCHS:     # senet.py:25-48
+            self.default_cfg.update(first_conv="layer0.conv1", classifier="last_linear",
+                                    interpolation="bicubic" if arch == "seresnet18" else "bilinear")
         if arch in TF_ARCHS:        # efficientnet.py:112-195
             pool_size, crop_pct = TF_POOL_CROP[int(arch[len("tf_efficientnet_b")])]
             self.default_cfg.update(pool_size=pool_size, crop_pct=crop_pct)
@@ -280,11 +292,12 @@ def create_model(model_name, pretrained=False, num_classes=1000, in_chans=3, che
     """dfd/timm/models/factory.py:8-64 for the architectures on the native hot path."""
     if pretrained:
         raise _lib.NativeError("pretrained weights need network access; load a checkpoint instead")
-    if model_name not in SUPPORTED_ARCHS + TF_ARCHS + RESNET_ARCHS + XCEPTION_ARCHS:
+    if model_name not in SUPPORTED_ARCHS + TF_ARCHS + RESNET_ARCHS + XCEPTION_ARCHS + SENET_ARCHS:
         raise RuntimeError("Unknown model (%s)" % model_name)       # factory.py:56
-    if model_name in XCEPTION_ARCHS:
+    if model_name in XCEPTION_ARCHS + SENET_ARCHS:
         # factory.py:31-45: the BatchNorm arguments are dropped for every model that is not an EfficientNet, and
-        # drop_block_rate / drop_path_rate when they are None; anything else reaches Xception.__init__, which refuses it
+        # drop_block_rate / drop_path_rate when they are None; anything else reaches Xception.__init__ / SENet.__init__, which
+        # refuse it
         for k in ("bn_tf", "bn_momentum", "bn_eps"):
             kwargs.pop(k, None)
         dc = kwargs.pop("drop_connect_rate", None)
@@ -296,6 +309,12 @@ def create_model(model_name, pretrained=False, num_classes=1000, in_chans=3, che
         bad = sorted(k for k in kwargs if k not in _XCEPTION_KWARGS)
         if bad:
             raise TypeError("__init__() got an unexpected keyword argument '%s'" % bad[0])
+    if model_name in SENET_ARCHS:
+        if kwargs.get("global_pool") == "catavgmax":
+            # the reference builds last_linear over num_features, not num_features * 2 (senet.py:340-342): its forward fails
+            raise ValueError("%s with global_pool='catavgmax': the reference's last_linear takes num_features inputs, not the "
+                             "2 * num_features of the concatenated pool, so its forward fails" % model_name)
+        kwargs.setdefault("drop_rate", SENET_DROP_RATE)
     model = NativeModel(model_name, num_classes=num_classes, in_chans=in_chans, **kwargs)
     if checkpoint_path:
         from .helpers import load_checkpoint

@@ -193,6 +193,11 @@ int dfd_conv1x1_dgrad_add(const void* dy, const void* wT, void* dx, int N, int H
 int dfd_unpack_grad(const float* g_ohwi, float* g_oihw_accum, int O, int I, int k, void* stream);
 int dfd_maxpool_fwd(const void* x, void* out, void* argmax_u8, int N, int H, int W, int C, int dt, void* stream);
 int dfd_maxpool_bwd(const void* gy, const void* argmax_u8, void* gx, int N, int H, int W, int C, int dt, void* stream);
+/* nn.MaxPool2d(3, 2, ceil_mode=True) without padding (SENet's stem pool, senet.py:297-299): Ho = ceil((H - 3) / 2) + 1 (less
+ * one if the last window would start outside the input), so the last window of an even extent is clipped; H, W >= 3 are the
+ * INPUT extents for both directions. Arg-max byte and first-maximum tie-break as dfd_maxpool_fwd / dfd_maxpool_bwd. */
+int dfd_maxpool_ceil_fwd(const void* x, void* out, void* argmax_u8, int N, int H, int W, int C, int dt, void* stream);
+int dfd_maxpool_ceil_bwd(const void* gy, const void* argmax_u8, void* gx, int N, int H, int W, int C, int dt, void* stream);
 int dfd_relu_bwd(const void* g, const void* out, void* gm, long long numel, int dt, void* stream);
 int dfd_pool_bwd(const float* dpooled, void* dout, int N, long long hw, int C, int dt, void* stream);
 /* backward of dfd_global_pool on a stored tensor (ResNet): dout[n,hw,c] = round16(g_avg[n,c] / HW + (hw == argmax[n,c]) *
@@ -287,6 +292,22 @@ int dfd_pool_se(const void* y, const float* scale, const float* shift, float* po
 int dfd_se_bwd_chain(const void* da, const void* y, const float* scale, const float* shift, float* draw, const float* pooled,
                      const float* Wr, const float* br, const float* We, const float* be, float* d_e, float* r, float* d_rpre,
                      float* dpool, int n, long long hw, int C, int Cse, int dt, void* stream);
+/* SENet's SEModule (senet.py:67-86: avg-pool, fc1 + bias, ReLU, fc2 + bias, sigmoid) on a = act(scale*y + shift), act NONE
+ * (SEResNetBottleneck: the bare bn3 output) or RELU (SEResNetBlock, :213-215): pooled[n,c] = mean_hw a, gate[n,:] =
+ * sigmoid(We relu(Wr pooled[n,:] + br) + be), fp32 [n, C]. Chunking for small batches as dfd_pool (max_chunks), the FC chain in
+ * the CTA that completes the image. The block tail is dfd_bn_act(y, scale, shift, gate, res, act, res_mode 2). */
+int dfd_pool_se_relu(const void* y, const float* scale, const float* shift, float* pooled, const float* Wr, const float* br,
+                     const float* We, const float* be, float* gate, int n, long long hw, int C, int Cse, int act, int dt,
+                     int max_chunks, void* stream);
+/* Backward of the SE-ResNet block tail out = relu(a * gate[n,c] + res), a = act(scale*y + shift) (senet.py:111-112,220-221), in
+ * one pass over the block output: gm = round16(g + g2) * (out > 0) is stored (g2 optional, as dfd_relu_bn_bwd_reduce),
+ * draw[n,c] = sum_hw gm * a (fp32, chunk partials in fixed slots), and the CTA completing image n runs the SE backward chain
+ * with the ReLU inner activation: d_e [n,C], r [n,Cse], d_rpre [n,Cse] for dfd_se_fc_wgrad and dpool [n,C] = dL/dpooled.
+ * The last BatchNorm's input gradient is then gz = (gm * gate + dpool / hw) * act'(u): dfd_act_bwd (act, da = gm, gate, dpool). */
+int dfd_relu_se_bwd_reduce(const void* g, const void* g2, const void* y, const void* out, const float* scale, const float* shift,
+                           void* gm, float* draw, const float* pooled, const float* Wr, const float* br, const float* We,
+                           const float* be, float* d_e, float* r, float* d_rpre, float* dpool, int n, long long hw, int C,
+                           int Cse, int act, int dt, void* stream);
 
 /* ---- classifier + loss + accuracy: nn.Linear (efficientnet.py:348, resnet.py:467), LabelSmoothing /
  *      SoftTarget / nn.CrossEntropyLoss (loss/cross_entropy.py:20-36, train.py:509-520), accuracy
