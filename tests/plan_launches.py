@@ -25,6 +25,9 @@ CONFIGS = [
     ("dfv4", "efficientnet_deepfake_v4", 3, 600, "bf16", {"in_chans": 12}),
 ]
 
+# configuration tables by name: tests/family_launches.py registers the model families' table as "family"
+TABLES = {"shipped": CONFIGS}
+
 Launch = namedtuple("Launch", "kernel shape ptrs")
 
 
@@ -43,18 +46,18 @@ def _split(name, args):
 
 
 @functools.lru_cache(maxsize=2)         # the training and the eval harvest of one plan share its engine
-def _plan_engine(tag, batch, dtype):
+def _plan_engine(tag, batch, dtype, table="shipped"):
     from deepfake_detection_b200.engine import Engine
-    _, arch, b, res, dt, kw = next(c for c in CONFIGS if c[0] == tag)
+    _, arch, b, res, dt, kw = next(c for c in TABLES[table] if c[0] == tag)
     return Engine(arch, batch or b, res, res, device="plan-only", dtype=dtype or dt, **kw)
 
 
 @functools.lru_cache(maxsize=None)
-def plan_launches(tag, batch=None, training=True, dtype=None):
-    """OrderedDict Launch -> number of times one step issues it, for one configuration (at another batch / 16-bit type when
-    given). Training: the forward and backward plan as built. Eval: the forward ops as Engine.launch_args rewrites them for
-    eval mode, then the logits-only head (Engine.head(False))."""
-    eng = _plan_engine(tag, batch, dtype)
+def plan_launches(tag, batch=None, training=True, dtype=None, table="shipped"):
+    """OrderedDict Launch -> number of times one step issues it, for one configuration of TABLES[table] (at another batch /
+    16-bit type when given). Training: the forward and backward plan as built. Eval: the forward ops as Engine.launch_args
+    rewrites them for eval mode, then the logits-only head (Engine.head(False))."""
+    eng = _plan_engine(tag, batch, dtype, table)
     out = OrderedDict()
 
     def add(la):
@@ -208,6 +211,14 @@ def _case_of(la, dtype, plan=None):
     if k == "dfd_gemm_wgrad":
         M, Nw, Kw, nbytes = s[0], s[1], s[2], s[4]
         return "wgrad", dict(M=M, Nw=Nw, Kw=Kw, splits=nbytes // (4 * Nw * Kw)), None, ("wgrad", Kw >= 128, Kw % 16 != 0, Nw > 128)
+    if k == "dfd_dwconv_fwd":
+        # act_in and the BatchNorm operands together select the staged input (dwconv.cu:891-895): raw, BN + Swish, BN + ReLU or
+        # ReLU only; any other pattern is a form no checker runs
+        assert la.ptrs[2] == la.ptrs[1] and la.ptrs[3:5] == "pp" and la.ptrs[6] == la.ptrs[5], la
+        assert la.ptrs[7] == "0" or la.ptrs[5] == "p", la
+        form = {(0, "0"): "raw", (1, "p"): "bn_swish", (2, "p"): "bn_relu", (2, "0"): "relu"}[(s[6], la.ptrs[1])]
+        if form in ("bn_relu", "relu"):
+            return _dw_relu_case(la)
     if k in ("dfd_dwconv_fwd", "dfd_dwconv_bwd"):
         N, H, W, C, kk, st = s[:6]
         affine = (s[6] == 1) if k == "dfd_dwconv_fwd" else la.ptrs[7] == "p"
@@ -221,7 +232,12 @@ def _case_of(la, dtype, plan=None):
             return "dwconv", kw, N, ("dw_fwd", dw_cpw(C), dw_tile(H, W, kk, st), kk, st, affine)
         kw["ws_bytes"] = s[7]
         return "dwconv", kw, N, ("dw_bwd", dw_cpw(C), dw_bwd_tile(H, W), kk, st, affine, add)
+    if k == "dfd_dwconv_bwd_relu":
+        return _dw_relu_case(la)
     if k in ("dfd_conv_tc", "dfd_conv_wgrad_tc"):
+        # dfd_conv_tc with statistics or without (the eval form, and the stride-1 input gradient): check_conv_implicit runs
+        # both and holds them to the same bits
+        assert k != "dfd_conv_tc" or la.ptrs in ("ppppp0", "pppppp", "ppp000"), la
         N, H, W, Cin, Cout, kk, st = s[:7]
         kw = dict(N=N, H=H, W=W, Cin=Cin, Cout=Cout, k=kk, stride=st)
         if k == "dfd_conv_wgrad_tc":
@@ -263,6 +279,26 @@ def _case_of(la, dtype, plan=None):
         assert s[3] == 0 and la.ptrs[:2] == "00", la
         return "bn_finalize_eval", dict(C=s[4]), None, None
     raise KeyError(k)
+
+
+def _dw_relu_case(la):
+    """the depthwise pair of a separable convolution whose input passes a ReLU (dwconv.cu:571-575): `bn` = the input is
+    relu(scale*x + shift) (mode 2, BN-backward sums of gx), else relu(x) (mode 3, the identity-path gradient `add` when given).
+    The forward does not say whether its backward adds: its case runs the backward with `add` in mode 3."""
+    s, p = la.shape, la.ptrs
+    N, H, W, C, kk, st = s[:6]
+    if la.kernel == "dfd_dwconv_fwd":
+        bn = p[1] == "p"
+        assert p[5:8] == "000", la                     # no statistics: the ReLU forward rejects them (dwconv.cu:892)
+        kw = dict(N=N, H=H, W=W, C=C, k=kk, s=st, bn=bn, add=not bn)
+        return "dwconv_relu", kw, N, ("dw_relu_fwd", dw_cpw(C), dw_tile(H, W, kk, st), bn)
+    assert la.kernel == "dfd_dwconv_bwd_relu", la
+    # gy is the gradient of the depthwise output itself: no folded BatchNorm backward (yout, cA, cB, cC absent), no fin
+    bn = p[7] == "p"
+    assert p[:5] == "p0000" and p[5:7] == "pp" and p[7:11] == ("pppp" if bn else "0000") and p[12:14] == "pp", la
+    assert p[14:16] == ("pp" if bn else "00") and p[16] == "p" and p[17] == "0" and not (bn and p[11] == "p"), la
+    kw = dict(N=N, H=H, W=W, C=C, k=kk, s=st, bn=bn, add=p[11] == "p", ws_bytes=s[7])
+    return "dwconv_relu", kw, N, ("dw_relu_bwd", dw_cpw(C), dw_bwd_tile(H, W), bn, p[11] == "p")
 
 
 def _stem_gemm_form(N, Cin, H, W, k, s, pad, Kp, plan=None):

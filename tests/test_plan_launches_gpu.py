@@ -80,6 +80,7 @@ def _check_conv(kw, dt):
     k, s = kw["k"], kw["stride"]
     r = _gc().check_conv_implicit(kw["N"], kw["H"], kw["W"], kw["Cin"], kw["Cout"], k, dtype=TDT[dt], stride=s)
     assert r["nan"] == 0 and r["nan_b"] == 0 and r["fwd_max"] < OUT16 and r["vs_im2col_mismatch"] == 0, str(r)
+    assert r["nostats_mismatch"] == 0, str(r)
     assert r["sum_rel"] < 1e-6 and r["sq_rel"] < 1e-6, str(r)
     assert r["dgrad_rel"] < 6e-3, str(r)
     if s == 2 and k == 3:

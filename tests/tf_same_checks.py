@@ -23,10 +23,11 @@ def _ordered_reduce(ws, dW, C, k, parts, cw):
     _lib.call("dfd_ordered_reduce", P(table), cbs, P(dW), (cw * k * k // 4 + 7) // 8 if parts > 64 else 1, st())
 
 
-def check_dw_pad(N, H, W, C, k, s, pt, pl, dtype=torch.bfloat16, seed=0, bwd=True):
+def check_dw_pad(N, H, W, C, k, s, pt, pl, dtype=torch.bfloat16, seed=0, bwd=True, stats=True):
     """dfd_dwconv_fwd_pad (BN + Swish input, statistics) and dfd_dwconv_bwd_pad (mode 1, order-deterministic workspace + the
     ordered reduce, as the training plan runs them) against fp64 torch. At symmetric pads also the symmetric entry points,
-    which must give the same bits (`sym_*_mismatch`). Two runs of the backward give the same bits (`bwd_bitwise`)."""
+    which must give the same bits (`sym_*_mismatch`). Two runs of the backward give the same bits (`bwd_bitwise`).
+    stats=False: also the eval form of the forward (no statistics), which must store the same bits (`nostats_mismatch`)."""
     g = torch.Generator(device="cuda").manual_seed(seed)
     d = DT[dtype]
     ho_, wo_ = -(-H // s), -(-W // s)
@@ -42,6 +43,12 @@ def check_dw_pad(N, H, W, C, k, s, pt, pl, dtype=torch.bfloat16, seed=0, bwd=Tru
     _lib.call("dfd_dwconv_fwd_pad", P(x), P(scale), P(shift), P(w), P(out), N, H, W, C, k, s, pt, pl, 1, d, P(s1), P(s2), None, st())
     torch.cuda.synchronize()
     res = dict(nan=int(torch.isnan(out.float()).sum()))
+    if not stats:
+        o2 = torch.full_like(out, float("nan"))
+        _lib.call("dfd_dwconv_fwd_pad", P(x), P(scale), P(shift), P(w), P(o2), N, H, W, C, k, s, pt, pl, 1, d, None, None, None, st())
+        torch.cuda.synchronize()
+        res["nostats_mismatch"] = int((o2.view(torch.int16) != out.view(torch.int16)).sum())
+        del o2
     sym = (pt, pl) == ((k - 1) // 2, (k - 1) // 2)
     if sym:
         o2, t1, t2 = torch.full_like(out, float("nan")), stat_buf(C), stat_buf(C)
@@ -103,6 +110,7 @@ def check_dw_pad(N, H, W, C, k, s, pt, pl, dtype=torch.bfloat16, seed=0, bwd=Tru
         res["sym_bwd_mismatch"] = int((gx3.view(torch.int16) != gx.view(torch.int16)).sum()) + int((dW3 != dW).sum())
         del gx3, dW3
     res["nan_b"] = int(torch.isnan(gx.float()).sum())
+    res["ws_bytes"] = cbs * parts * cw * k * k * 4
     # xr.grad = scale * (dgrad * swish'(u)); the kernel stores gu = dgrad * swish'(u), rounded to the 16-bit type
     gu_ref = xr.grad / scale.double().view(1, C, 1, 1)
     res["dgrad_rel"] = relerr(nchw(gx.double()), gu_ref)
