@@ -872,7 +872,7 @@ def check_transpose(dtype=torch.bfloat16):
     shapes = [(96, 16), (24, 144), (1280, 320), (40, 240)]
     srcs = [torch.randn(o, i, device="cuda").to(dtype) for o, i in shapes]
     dsts = [torch.zeros(i, o, device="cuda", dtype=dtype) for o, i in shapes]
-    raw = b"".join(struct.pack("<QQii", s.data_ptr(), d.data_ptr(), o, i) for s, d, (o, i) in zip(srcs, dsts, shapes))
+    raw = b"".join(struct.pack("<QQii", P(s), P(d), o, i) for s, d, (o, i) in zip(srcs, dsts, shapes))
     table = torch.frombuffer(bytearray(raw), dtype=torch.uint8).cuda()
     _lib.call("dfd_transpose_weights", P(table), len(shapes), DT[dtype], st())
     torch.cuda.synchronize()
@@ -890,7 +890,7 @@ def check_conv_dense(N, H, W, Cin, Cout, k, s, dtype=torch.bfloat16, seed=0):
     w = (torch.randn(Cout, Cin, k, k, device="cuda", generator=g) / math.sqrt(Cin * k * k)).to(dtype)
     wp = torch.zeros(Cout * k * k * Cin, device="cuda", dtype=dtype)
     wpT = torch.zeros_like(wp)
-    table = torch.frombuffer(bytearray(struct.pack("<QQQQiiii", w.data_ptr(), wp.data_ptr(), wpT.data_ptr(), 0, Cout, Cin, k, 0)),
+    table = torch.frombuffer(bytearray(struct.pack("<QQQQiiii", P(w), P(wp), P(wpT), 0, Cout, Cin, k, 0)),
                              dtype=torch.uint8).cuda()
     d = DT[dtype]
     _lib.call("dfd_repack_weights", P(table), 1, d, st())
@@ -933,7 +933,7 @@ def check_conv_implicit(N, H, W, Cin, Cout, k=3, dtype=torch.bfloat16, seed=0, s
     w = (torch.randn(Cout, Cin, k, k, device="cuda", generator=g) / math.sqrt(Cin * k * k)).to(dtype)
     wp = torch.zeros(Cout * k * k * Cin, device="cuda", dtype=dtype)
     wpT, wpD = torch.zeros_like(wp), torch.zeros_like(wp)
-    table = torch.frombuffer(bytearray(struct.pack("<QQQQiiii", w.data_ptr(), wp.data_ptr(), wpT.data_ptr(), wpD.data_ptr(),
+    table = torch.frombuffer(bytearray(struct.pack("<QQQQiiii", P(w), P(wp), P(wpT), P(wpD),
                                                    Cout, Cin, k, 0)), dtype=torch.uint8).cuda()
     d = DT[dtype]
     _lib.call("dfd_repack_weights", P(table), 1, d, st())
