@@ -38,8 +38,6 @@ SIGNATURES = {
     "dfd_dwconv_fwd_pad": "ppppp" "iiiiiiii" "ii" "ppp" "p",
     "dfd_dwconv_bwd_pad": "ppppp" "pppppp" "ppp" "iiiiiiii" "i" "pp" "pl" "p" "p",
     "dfd_dwconv_bwd_relu": "ppppp" "pppppp" "ppp" "iiiiii" "i" "pp" "pl" "p" "p",
-    "dfd_stem_fwd": "ppp" "iiiiiiii" "i" "ppp",
-    "dfd_stem_wgrad": "ppppppp" "iiiiiiii" "i" "p",
     "dfd_colstats": "p" "ili" "i" "ppp",
     "dfd_bn_finalize": "ppd" "ppppp" "ffii" "ppppp",
     "dfd_bn_act": "pppppp" "ili" "iii" "p",

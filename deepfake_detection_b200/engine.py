@@ -8,8 +8,9 @@ This is the host side of the hot path (dfd/runners/train.py:610-649): given an a
   * replays the plan on the caller's current CUDA stream (optionally captured into a CUDA graph).
 
 The family's plan builder (engine_efficientnet, engine_resnet, engine_xception) lays out the activations
-and lists the ops; the conventions every plan shares (BatchNorm statistics and finalisation, the mask generators, the
-deterministic weight-gradient reduce, validation against the ABI table) are the plan helpers of this class.
+and lists the ops; the conventions every plan shares (BatchNorm statistics, finalisation and backward apply, the mask
+generators, the deterministic weight-gradient reduce, the stem as im2col + GEMM, the pooled classifier head, the packed k x k
+weights, validation against the ABI table) are the plan helpers of this class.
 
 A plan op is (name, args). `base_name(name)` is the C-ABI entry point it calls: `<entry>_train` runs in training mode
 only and `dfd_bn_finalize_sync` finalises the summed statistics of all ranks. In args, ("TRAIN_ONLY", ptr) is an operand
@@ -51,8 +52,8 @@ class _BN:
 
 class Engine:
     def __init__(self, arch, batch, height=None, width=None, num_classes=2, in_chans=3, dtype="bf16",
-                 bn_momentum=0.1, bn_eps=1e-5, device=None, gemm_impl="tc", share_from=None, stem_impl="gemm",
-                 params_only=False, drop_rate=0.0, drop_path_rate=0.0, sync_bn=False, global_pool="avg", drop_block_rate=0.0):
+                 bn_momentum=0.1, bn_eps=1e-5, device=None, gemm_impl="tc", share_from=None, params_only=False,
+                 drop_rate=0.0, drop_path_rate=0.0, sync_bn=False, global_pool="avg", drop_block_rate=0.0):
         # _plan_only: build the arenas and the call plan on the CPU for host-logic tests; nothing can be executed
         self._plan_only = device == "plan-only"
         if self._plan_only:
@@ -94,7 +95,6 @@ class Engine:
         self.bn_eps = float(bn_eps)
         # "tc": wgmma GEMMs and implicit convolutions; "mma": the mma.sync cross-check path (GEMMs over im2col columns)
         self.gemm_impl = gemm_impl
-        self.stem_impl = stem_impl
         self.training = True
         self.n_launch = {"fwd": 0, "bwd": 0, "opt": 0}
         self._shared_from = share_from
@@ -363,8 +363,34 @@ class Engine:
             _lib.call("dfd_blockdiag_weights", _ptr(o._bd_table), len(reg), o.dt, stream)
         o._derived_dirty = False
 
-    def _stem_gemm_setup(self, wname, Cout, k, M):
-        """stem convolution as im2col + tensor-core GEMM (K = Cin*k*k padded to a multiple of 8)"""
+    def _packed_weights(self, names):
+        """the k x k weights `names` in the packed layouts of the dense convolutions: wpack16 [Cout][kh][kw][Cin] (forward),
+        wpackT16 its transpose (input gradient over im2col columns) and wpackD16 the tap-flipped [Cin][kh][kw][Cout] (implicit
+        input gradient). They depend on the parameter shapes only, so the arena engine registers them once; returns each
+        weight's element offset into the three buffers"""
+        offs, off = OrderedDict(), 0
+        for n in names:
+            offs[n] = off
+            off += (self.p_off[n][2] + 7) // 8 * 8
+        ar = self.arena
+        if getattr(ar, "wpack16", None) is None:
+            ar.wpack16, ar.wpackT16, ar.wpackD16 = [torch.zeros(max(off, 8), dtype=self.tdtype, device=self.device)
+                                                    for _ in range(3)]
+            raw = b"".join(struct.pack("<QQQQiiii", _ptr(self.params16, self.p_off[n][0]), _ptr(ar.wpack16, o),
+                                       _ptr(ar.wpackT16, o), _ptr(ar.wpackD16, o), *self.p_off[n][1][:3], 0)
+                           for n, o in offs.items())
+            ar._rtable = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(self.device)
+            ar._rtable_count = len(offs)
+            ar._derived_dirty = True
+            ar.layout_gen += 1
+        self.wpack16, self.wpackT16, self.wpackD16 = ar.wpack16, ar.wpackT16, ar.wpackD16
+        return offs
+
+    def _stem_gemm(self, wname, Cout, k, stride, pad, y, M, bn, rowpack=True):
+        """forward ops of the stem convolution of x_in as im2col + tensor-core GEMM into y [M, Cout], with the batch statistics
+        of `bn`. The columns and a padded copy of the weight have K = Cin*k*k zero-padded to a multiple of 8. `pad` is the
+        padding of every side, or the (top, left) padding of TF "SAME" (the bottom / right padding follows from the output
+        extents)."""
         taps = self.spec.in_chans * k * k
         Kp = (taps + 7) // 8 * 8
         o = self.arena
@@ -377,7 +403,23 @@ class Engine:
         self.stem_wpad = reg[key]
         self.stem_gpad = torch.zeros(Cout * Kp, dtype=torch.float32, device=self.device)
         self.stem_cols = self._alloc16(M, Kp)
-        return taps, Kp
+        self._stem = (wname, Cout, M, taps, Kp)
+        same = isinstance(pad, tuple)
+        im2col = ("dfd_stem_im2col_pad" if same else "dfd_stem_im2col",
+                  (_ptr(self.x_in), _ptr(self.stem_cols), self.N, self.spec.in_chans, self.H, self.W, k, stride)
+                  + (pad if same else (pad,)) + (Kp, self.dt))
+        return [im2col, self._gemm(_ptr(self.stem_cols), _ptr(self.stem_wpad), _ptr(y), M, Cout, Kp, bn, rowpack)]
+
+    def _stem_wgrad(self, dy):
+        """ops of the stem's weight gradient from dy [M, Cout] into the padded fp32 buffer. It is complete after the next
+        ordered reduce; _stem_unpad then adds it into the gradient arena."""
+        _, Cout, M, _, Kp = self._stem
+        return [("dfd_memset_async", (_ptr(self.stem_gpad), 0, Cout * Kp * 4)),
+                self._wgrad(dy, _ptr(self.stem_cols), _ptr(self.stem_gpad), M, Cout, Kp)]
+
+    def _stem_unpad(self):
+        wname, Cout, _, taps, Kp = self._stem
+        return ("dfd_unpad_grad", (_ptr(self.stem_gpad), self._g32(wname), Cout, taps, Kp))
 
     def _alloc_bn(self, bn_specs):
         """per-BN pointers into the parameter / running-stat arenas + the per-step statistic and coefficient arenas"""
@@ -413,9 +455,25 @@ class Engine:
         from .engine_efficientnet import build_efficientnet
         from .engine_resnet import build_resnet
         from .engine_xception import build_xception
+        self._keep, self.acts = [], {}
+        self._masks = []            # dfd_rng_masks table: (tensor, rows, width, keep_prob), see _mask_head
+        self.x_in = torch.zeros(self.N, self.spec.in_chans, self.H, self.W, dtype=self.tdtype, device=self.device)
         {"resnet": build_resnet, "xception": build_xception}.get(self.spec.family, build_efficientnet)(self)
 
     # ---- plan helpers shared by the family builders ---------------------------------------------------------------------
+    # pointers to a parameter's fp32 value and gradient, its 16-bit copy and the transposed 16-bit copy of a 1x1 weight
+    def _p32(self, name):
+        return _ptr(self.params32, self.p_off[name][0])
+
+    def _g32(self, name):
+        return _ptr(self.grads32, self.p_off[name][0])
+
+    def _p16(self, name):
+        return _ptr(self.params16, self.p_off[name][0])
+
+    def _t16(self, name):
+        return _ptr(self.paramsT16, self.t_off[name][0])
+
     def _stats(self, bn):
         """a forward producer's (sum, sum of squares) operands for `bn`, training-only (NULL in eval mode). Every producer
         passes NULL for its finalisation-descriptor operand: a finalise op of its own follows it."""
@@ -455,11 +513,70 @@ class Engine:
             return [("ALLREDUCE", (self.stats[bn.stat_off + 2 * S * bn.C:bn.stat_off + 4 * S * bn.C], "avg")), op]
         return [op]
 
-    def _mask_head(self, masks, n_drop_block=0):
+    def _bn_apply(self, g, y, bn, out, hw, C):
+        """out = the gradient of the input y of `bn` from the gradient g of its output (the coefficients of _bwd_finalize)"""
+        return ("dfd_bn_bwd_apply", (g, _ptr(y), None, bn.cA, bn.cB, bn.cC, out, self.N, hw, C, self.dt))
+
+    def _pool_head(self, feat, bn, act, hw, drop_rate, partial=None):
+        """forward ops from the features feat [N, hw, F] to the classifier's input `pooled` [N, P]: the global pool (with `bn`,
+        feat is that BatchNorm's input and the BatchNorm and `act` are applied on load), then dropout at `drop_rate` (a
+        mask drawn at the head of the training forward). Allocates the head's tensors; `partial` goes to dfd_pool as is."""
+        spec, N, dev = self.spec, self.N, self.device
+        F, P, K = spec.num_features, spec.pooled_features, spec.num_classes
+        pool_t = _lib.POOL_TYPES[spec.global_pool]
+        scale, shift = (bn.scale, bn.shift) if bn is not None else (None, None)
+        self._head = (feat, bn, act, hw)
+        self.pooled = torch.zeros(N, P, dtype=torch.float32, device=dev)
+        if pool_t == _lib.POOL_TYPES["avg"]:
+            ops = [("dfd_pool", (_ptr(feat), scale, shift, _ptr(self.pooled), N, hw, F, act, self.dt, partial, POOL_CHUNKS))]
+        else:
+            # max / avgmax / catavgmax: one pass gives the mean (dfd_pool's order), the max and its argmax for the backward
+            self.pool_argmax = torch.zeros(N, F, dtype=torch.int32, device=dev)
+            ops = [("dfd_global_pool", (_ptr(feat), scale, shift, _ptr(self.pooled), _ptr(self.pool_argmax), N, hw, F, act,
+                                        pool_t, self.dt, POOL_CHUNKS))]
+        self.dropout_mask = None
+        if drop_rate > 0.0:
+            # F.dropout on the pooled vector, with a mask already divided by keep
+            self.dropout_mask = torch.ones(N, P, dtype=torch.float32, device=dev)
+            self._masks.append((self.dropout_mask, N * P, 1, 1.0 - drop_rate))
+            ops.append(("dfd_mul_f32_train", (_ptr(self.pooled), _ptr(self.dropout_mask), N * P)))
+        self.logits = torch.zeros(N, K, dtype=torch.float32, device=dev)
+        self.dlogits = torch.zeros(N, K, dtype=torch.float32, device=dev)
+        self.dpooled = torch.zeros(N, P, dtype=torch.float32, device=dev)
+        self.target_i = torch.zeros(N, dtype=torch.int64, device=dev)
+        self.target_f = torch.zeros(N, K, dtype=torch.float32, device=dev)
+        return ops
+
+    def _pool_head_bwd(self, gx):
+        """backward ops of _pool_head from dlogits into gx [N, hw, F]: the classifier's gradients, the dropout mask, the pool.
+        With a BatchNorm, gx is the gradient of the BatchNorm's output (through `act`), and its backward sums are reduced."""
+        feat, bn, act, hw = self._head
+        spec, N, dt = self.spec, self.N, self.dt
+        F, P, K = spec.num_features, spec.pooled_features, spec.num_classes
+        pool_t = _lib.POOL_TYPES[spec.global_pool]
+        avg = pool_t == _lib.POOL_TYPES["avg"]
+        ops = [("dfd_head_bwd", (_ptr(self.dlogits), _ptr(self.pooled), self._p32(self.cls_name + ".weight"),
+                                 self._g32(self.cls_name + ".weight"), self._g32(self.cls_name + ".bias"), _ptr(self.dpooled),
+                                 N, P, K))]
+        if self.dropout_mask is not None:
+            ops.append(("dfd_mul_f32", (_ptr(self.dpooled), _ptr(self.dropout_mask), N * P)))
+        if bn is None and avg:
+            ops.append(("dfd_pool_bwd", (_ptr(self.dpooled), gx, N, hw, F, dt)))
+        elif bn is None:
+            ops.append(("dfd_gpool_bwd", (_ptr(self.dpooled), _ptr(self.pool_argmax), gx, N, hw, F, pool_t, dt)))
+        elif avg:
+            ops.append(("dfd_act_bwd", (None, _ptr(feat), bn.scale, bn.shift, bn.mean, bn.rstd, None, _ptr(self.dpooled), gx,
+                                        N, hw, F, act, dt, bn.bs1, bn.bs2, None)))
+        else:
+            ops.append(("dfd_act_bwd_gpool", (_ptr(feat), bn.scale, bn.shift, bn.mean, bn.rstd, _ptr(self.dpooled),
+                                              _ptr(self.pool_argmax), gx, N, hw, F, act, pool_t, dt, bn.bs1, bn.bs2, None)))
+        return ops
+
+    def _mask_head(self, n_drop_block=0):
         """the ops at the head of the training forward that draw the step's masks: the DropBlock sites of
-        self._drop_block_table, then the dropout / drop-path masks (tensor, rows, width, keep_prob); the generator's step then
-        advances on the device"""
-        head = []
+        self._drop_block_table, then the dropout / drop-path masks of self._masks; the generator's step then advances on the
+        device"""
+        head, masks = [], self._masks
         if n_drop_block:
             head.append(("dfd_memset_async_train", (_ptr(self.drop_block_kept), 0, 8 * n_drop_block)))
             head.append(("dfd_drop_block_masks_train", (_ptr(self._drop_block_table), n_drop_block, _ptr(self.rng_state))))
@@ -471,9 +588,10 @@ class Engine:
             head.append(("dfd_rng_tick_train", (_ptr(self.rng_state),)))
         return head
 
-    def _finish_plan(self, fwd, bwd):
-        """resolve the workspace, check every op against the ABI table and publish the plan as fwd_ops / bwd_ops:
-        (function, name, args)"""
+    def _finish_plan(self, fwd, bwd, n_drop_block=0):
+        """put the mask draws at the head of the forward, resolve the workspace, check every op against the ABI table and
+        publish the plan as fwd_ops / bwd_ops: (function, name, args)"""
+        fwd = self._mask_head(n_drop_block) + fwd
         bwd = self._patch_workspace(bwd)
         for n, a in fwd + bwd:
             if n.startswith("ALLREDUCE"):

@@ -10,15 +10,12 @@ from collections import OrderedDict
 
 import torch
 
-from . import _lib
 from .arch import conv_pads
 from .engine import ACT_NONE, ACT_SWISH, POOL_CHUNKS, _ptr
 
 
 def build_efficientnet(e):
     spec, N, dev, dt = e.spec, e.N, e.device, e.dt
-    e._keep = []
-    e.acts = {}
     fwd, bwd = [], []
 
     # ---- pass 1: shapes --------------------------------------------------------------------
@@ -38,9 +35,6 @@ def build_efficientnet(e):
     e.conv_pads = conv_pads(spec, e.H, e.W)
     pads = {name: (pt, pl) for name, k, s_, h_, w_, pt, pl, ho_, wo_ in e.conv_pads}
     asym = lambda name, k: pads[name] != ((k - 1) // 2, (k - 1) // 2)
-    if asym("conv_stem", 3) and e.stem_impl != "gemm":
-        raise ValueError("stem_impl=%r: TF 'SAME' padding of the stem is planned through dfd_stem_im2col_pad (stem_impl='gemm')"
-                         % (e.stem_impl,))
 
     # ---- BN bookkeeping arenas ---------------------------------------------------------------
     bn_specs = [("bn1", spec.stem)]
@@ -52,10 +46,7 @@ def build_efficientnet(e):
     bn_specs.append(("bn2", spec.num_features))
     e._alloc_bn(bn_specs)
 
-    P32 = lambda n: _ptr(e.params32, e.p_off[n][0])
-    G32 = lambda n: _ptr(e.grads32, e.p_off[n][0])
-    P16 = lambda n: _ptr(e.params16, e.p_off[n][0])
-    T16 = lambda n: _ptr(e.paramsT16, e.t_off[n][0])
+    P32, G32, P16, T16 = e._p32, e._g32, e._p16, e._t16
     gemm, finalize, bwd_finalize = e._gemm, e._finalize, e._bwd_finalize
 
     # ---- scratch for backward ----------------------------------------------------------------
@@ -72,30 +63,19 @@ def build_efficientnet(e):
     se_max_r = max([b.cse for b in spec.blocks if b.cse] + [8])
     e.se_tmp = torch.zeros(3 * N * se_max_c + 2 * N * se_max_r, dtype=torch.float32, device=dev)
     se_draw = _ptr(e.se_tmp)
-    e.pool_partial = torch.zeros(POOL_CHUNKS * N * max(se_max_c, spec.num_features), dtype=torch.float32, device=dev)
     se_de = _ptr(e.se_tmp, N * se_max_c)
     se_dpool = _ptr(e.se_tmp, 2 * N * se_max_c)
     se_r = _ptr(e.se_tmp, 3 * N * se_max_c)
     se_drp = _ptr(e.se_tmp, 3 * N * se_max_c + N * se_max_r)
 
     # ---- forward -----------------------------------------------------------------------------
-    e.x_in = torch.zeros(N, spec.in_chans, e.H, e.W, dtype=e.tdtype, device=dev)
     y0 = e._alloc16(N, Hs, Ws, spec.stem)
     stem_out = e._alloc16(N, Hs, Ws, spec.stem)
     e.acts["conv_stem"] = y0
     e.acts["stem.out"] = stem_out
     bn = e.bns["bn1"]
-    if e.stem_impl == "gemm":
-        taps, Kp = e._stem_gemm_setup("conv_stem.weight", spec.stem, 3, N * Hs * Ws)
-        if asym("conv_stem", 3):
-            fwd.append(("dfd_stem_im2col_pad", (_ptr(e.x_in), _ptr(e.stem_cols), N, spec.in_chans, e.H, e.W, 3, 2)
-                        + pads["conv_stem"] + (Kp, dt)))
-        else:
-            fwd.append(("dfd_stem_im2col", (_ptr(e.x_in), _ptr(e.stem_cols), N, spec.in_chans, e.H, e.W, 3, 2, 1, Kp, dt)))
-        fwd.append(gemm(_ptr(e.stem_cols), _ptr(e.stem_wpad), _ptr(y0), N * Hs * Ws, spec.stem, Kp, bn))
-    else:
-        fwd.append(("dfd_stem_fwd", (_ptr(e.x_in), P32("conv_stem.weight"), _ptr(y0), N, spec.in_chans, e.H, e.W,
-                                     spec.stem, 3, 2, 1, dt) + e._stats(bn)))
+    fwd += e._stem_gemm("conv_stem.weight", spec.stem, 3, 2, pads["conv_stem"] if asym("conv_stem", 3) else 1, y0,
+                        N * Hs * Ws, bn)
     fwd += finalize(bn, N * Hs * Ws)
     fwd.append(("dfd_bn_act", (_ptr(y0), bn.scale, bn.shift, None, None, _ptr(stem_out), N, Hs * Ws, spec.stem,
                                ACT_SWISH, 0, dt)))
@@ -105,7 +85,6 @@ def build_efficientnet(e):
     # (rate = drop_path_rate * block_idx / n_blocks, efficientnet_builder.py:228-230,343) and the classifier dropout mask;
     # the gates are [N, C] fp32 tensors (one draw per sample replicated over the channels) filled by ONE dfd_rng_masks
     # launch at the head of the forward plan, consumed through the GATE operand of dfd_bn_act
-    masks = []               # (tensor, rows, width, keep_prob)
     n_blocks = len(blocks)
     for bi, (b, h, w, ho, wo) in enumerate(blocks):
         p = b.name
@@ -155,7 +134,7 @@ def build_efficientnet(e):
         if dp_rate > 0.0:
             dp_gate = torch.ones(N, b.cout, dtype=torch.float32, device=dev)
             e._keep.append(dp_gate)
-            masks.append((dp_gate, N, b.cout, 1.0 - dp_rate))
+            e._masks.append((dp_gate, N, b.cout, 1.0 - dp_rate))
         fwd.append(("dfd_bn_act", [_ptr(y3), bn_out.scale, bn_out.shift, ("TRAIN_ONLY", _ptr(dp_gate)) if dp_gate is not None else None,
                                    _ptr(x) if b.has_residual else None,
                                    _ptr(out), N, ho * wo, b.cout, ACT_NONE, 1 if b.has_residual else 0, dt]))
@@ -171,51 +150,21 @@ def build_efficientnet(e):
     e.acts["conv_head"] = yh
     fwd.append(gemm(_ptr(x), P16("conv_head.weight"), _ptr(yh), Mf, F, spec.head_in, bnh))
     fwd += finalize(bnh, Mf)
-    P, pool_t = spec.pooled_features, _lib.POOL_TYPES[spec.global_pool]
-    e.pooled = torch.zeros(N, P, dtype=torch.float32, device=dev)
-    if pool_t == _lib.POOL_TYPES["avg"]:
-        fwd.append(("dfd_pool", (_ptr(yh), bnh.scale, bnh.shift, _ptr(e.pooled), N, Hf * Wf, F, ACT_SWISH, dt,
-                                 None, POOL_CHUNKS)))
-    else:
-        # max / avgmax / catavgmax: one pass gives the mean (dfd_pool's order), the max and its argmax for the backward
-        e.pool_argmax = torch.zeros(N, F, dtype=torch.int32, device=dev)
-        fwd.append(("dfd_global_pool", (_ptr(yh), bnh.scale, bnh.shift, _ptr(e.pooled), _ptr(e.pool_argmax), N,
-                                        Hf * Wf, F, ACT_SWISH, pool_t, dt, POOL_CHUNKS)))
+    fwd += e._pool_head(yh, bnh, ACT_SWISH, Hf * Wf, e.drop_rate)
     e.drop_masks = OrderedDict()
-    if e.drop_rate > 0.0:
-        e.dropout_mask = torch.ones(N, P, dtype=torch.float32, device=dev)
-        masks.append((e.dropout_mask, N * P, 1, 1.0 - e.drop_rate))
-        fwd.append(("dfd_mul_f32_train", (_ptr(e.pooled), _ptr(e.dropout_mask), N * P)))
     for r_ in recs:
         if r_["dp_gate"] is not None:
             e.drop_masks[r_["b"].name] = r_["dp_gate"]
-    fwd = e._mask_head(masks) + fwd
-    if masks:
-        cmax = max(t.shape[-1] for t, _, _, _ in masks)
+    if e._masks:
+        cmax = max(t.shape[-1] for t, _, _, _ in e._masks)
         e._unit_affine = torch.cat([torch.ones(cmax, device=dev), torch.zeros(cmax, device=dev)]).float()
         e._keep.append(e._unit_affine)
-    K = spec.num_classes
-    e.logits = torch.zeros(N, K, dtype=torch.float32, device=dev)
-    e.dlogits = torch.zeros(N, K, dtype=torch.float32, device=dev)
-    e.dpooled = torch.zeros(N, P, dtype=torch.float32, device=dev)
-    e.target_i = torch.zeros(N, dtype=torch.int64, device=dev)
-    e.target_f = torch.zeros(N, K, dtype=torch.float32, device=dev)
     e._head_in = x
 
     # ---- backward ----------------------------------------------------------------------------
-    bwd.append(("dfd_head_bwd", (_ptr(e.dlogits), _ptr(e.pooled), P32("classifier.weight"),
-                                 G32("classifier.weight"), G32("classifier.bias"), _ptr(e.dpooled), N, P, K)))
-    if e.drop_rate > 0.0:
-        bwd.append(("dfd_mul_f32", (_ptr(e.dpooled), _ptr(e.dropout_mask), N * P)))
-    if pool_t == _lib.POOL_TYPES["avg"]:
-        bwd.append(("dfd_act_bwd", (None, _ptr(yh), bnh.scale, bnh.shift, bnh.mean, bnh.rstd, None, _ptr(e.dpooled),
-                                    mid_a, N, Hf * Wf, F, ACT_SWISH, dt, bnh.bs1, bnh.bs2, None)))
-    else:
-        bwd.append(("dfd_act_bwd_gpool", (_ptr(yh), bnh.scale, bnh.shift, bnh.mean, bnh.rstd, _ptr(e.dpooled),
-                                          _ptr(e.pool_argmax), mid_a, N, Hf * Wf, F, ACT_SWISH, pool_t, dt, bnh.bs1,
-                                          bnh.bs2, None)))
+    bwd += e._pool_head_bwd(mid_a)
     bwd += bwd_finalize(bnh, Mf)
-    bwd.append(("dfd_bn_bwd_apply", (mid_a, _ptr(yh), None, bnh.cA, bnh.cB, bnh.cC, mid_b, N, Hf * Wf, F, dt)))
+    bwd.append(e._bn_apply(mid_a, yh, bnh, mid_b, Hf * Wf, F))
     cur = 0
     bwd.append(gemm(mid_b, T16("conv_head.weight"), sm[cur], Mf, spec.head_in, F))
     bwd.append(e._wgrad(mid_b, _ptr(e._head_in), G32("conv_head.weight"), Mf, F, spec.head_in))
@@ -239,7 +188,7 @@ def build_efficientnet(e):
         bwd.append(("dfd_bn_bwd_reduce", (gbn, _ptr(y3), None, bn_out.mean, bn_out.rstd, N, ho * wo, b.cout, dt,
                                           bn_out.bs1, bn_out.bs2, None)))
         bwd += bwd_finalize(bn_out, M2)
-        bwd.append(("dfd_bn_bwd_apply", (gbn, _ptr(y3), None, bn_out.cA, bn_out.cB, bn_out.cC, t1, N, ho * wo, b.cout, dt)))
+        bwd.append(e._bn_apply(gbn, y3, bn_out, t1, ho * wo, b.cout))
         bwd.append(gemm(t1, T16(p + pw_name + ".weight"), mid_a, M2, b.cmid, b.cout))
         bwd.append(e._wgrad(t1, _ptr(a2), G32(p + pw_name + ".weight"), M2, b.cout, b.cmid))
         gate_ptr = dpool_ptr = None
@@ -265,7 +214,7 @@ def build_efficientnet(e):
                                  (dt, dw_bn.bs1, dw_bn.bs2), N, h, w, b.cmid, b.k, b.stride,
                                  name="dfd_dwconv_bwd" + ("_pad" if dw_pad else "")))
             bwd += bwd_finalize(dw_bn, M1)
-            bwd.append(("dfd_bn_bwd_apply", (mid_a, _ptr(y1), None, dw_bn.cA, dw_bn.cB, dw_bn.cC, mid_b, N, h * w, b.cmid, dt)))
+            bwd.append(e._bn_apply(mid_a, y1, dw_bn, mid_b, h * w, b.cmid))
             bwd.append(gemm(mid_b, T16(p + ".conv_pw.weight"), t2, M1, b.cin, b.cmid))
             if b.has_residual:
                 bwd.append(("dfd_add_inplace", (t2, dout, M1 * b.cin, dt)))
@@ -285,13 +234,8 @@ def build_efficientnet(e):
     bwd.append(("dfd_act_bwd", (sm[cur], _ptr(y0), bn.scale, bn.shift, bn.mean, bn.rstd, None, None, mid_a, N, Hs * Ws,
                                 spec.stem, ACT_SWISH, dt, bn.bs1, bn.bs2, None)))
     bwd += bwd_finalize(bn, N * Hs * Ws)
-    if e.stem_impl == "gemm":
-        bwd.append(("dfd_bn_bwd_apply", (mid_a, _ptr(y0), None, bn.cA, bn.cB, bn.cC, mid_b, N, Hs * Ws, spec.stem, dt)))
-        bwd.append(("dfd_memset_async", (_ptr(e.stem_gpad), 0, spec.stem * Kp * 4)))
-        bwd.append(e._wgrad(mid_b, _ptr(e.stem_cols), _ptr(e.stem_gpad), N * Hs * Ws, spec.stem, Kp))
-        e._flush_reduce(bwd)          # the padded gradient must be complete before it is un-padded into the arena
-        bwd.append(("dfd_unpad_grad", (_ptr(e.stem_gpad), G32("conv_stem.weight"), spec.stem, taps, Kp)))
-    else:
-        bwd.append(("dfd_stem_wgrad", (_ptr(e.x_in), mid_a, _ptr(y0), bn.cA, bn.cB, bn.cC, G32("conv_stem.weight"), N,
-                                       spec.in_chans, e.H, e.W, spec.stem, 3, 2, 1, dt)))
+    bwd.append(e._bn_apply(mid_a, y0, bn, mid_b, Hs * Ws, spec.stem))
+    bwd += e._stem_wgrad(mid_b)
+    e._flush_reduce(bwd)          # the padded gradient must be complete before it is un-padded into the arena
+    bwd.append(e._stem_unpad())
     e._finish_plan(fwd, bwd)

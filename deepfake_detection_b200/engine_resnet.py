@@ -41,7 +41,6 @@ from functools import partial
 
 import torch
 
-from . import _lib
 from .arch import stem_pool_out
 from .engine import ACT_NONE, ACT_RELU, POOL_CHUNKS, _ptr
 
@@ -85,46 +84,18 @@ def ds_names(b):
 
 def build_resnet(e):
     spec, N, dev, dt = e.spec, e.N, e.device, e.dt
-    e._keep = []
-    e.acts = {}
     fwd, bwd = [], []
 
-    # ---- packed (kh, kw, ci) copies of the k x k weights -------------------------------------------------
-    pk_off, off = {}, 0
-    for n in e.param_names:
-        o, s, k = e.p_off[n]
-        if len(s) == 4 and s[2] > 1 and n not in (spec.stem_conv + ".weight", "conv1.0.weight"):    # not the stem-GEMM weights
-            pk_off[n] = (off, s[0], s[1], s[2])
-            off += (k + 7) // 8 * 8
-    ar = e.arena        # the packed layouts depend on the parameter shapes only: owned and refreshed by the arena engine
-    if getattr(ar, "wpack16", None) is None:
-        ar.wpack16 = torch.zeros(max(off, 8), dtype=e.tdtype, device=dev)
-        ar.wpackT16 = torch.zeros(max(off, 8), dtype=e.tdtype, device=dev)
-        ar.wpackD16 = torch.zeros(max(off, 8), dtype=e.tdtype, device=dev)
-        raw = b"".join(struct.pack("<QQQQiiii", _ptr(e.params16, e.p_off[n][0]), _ptr(ar.wpack16, o), _ptr(ar.wpackT16, o),
-                                   _ptr(ar.wpackD16, o), O, I, k, 0)
-                       for n, (o, O, I, k) in pk_off.items())
-        ar._rtable = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(dev)
-        ar._rtable_count = len(pk_off)
-        ar._derived_dirty = True
-        ar.layout_gen += 1
-    e.wpack16, e.wpackT16, e.wpackD16 = ar.wpack16, ar.wpackT16, ar.wpackD16
+    # ---- packed (kh, kw, ci) copies of every k x k weight but the stem-GEMM weights ----------------------------------------
+    pk = e._packed_weights([n for n in e.param_names if len(e.p_off[n][1]) == 4 and e.p_off[n][1][2] > 1
+                            and n not in (spec.stem_conv + ".weight", "conv1.0.weight")])
     # two regions: a BasicBlock has two 3x3 convolutions whose packed gradients wait for the block's single ordered reduce
-    gperm_max = max([O * I * k * k for (_, O, I, k) in pk_off.values()] + [8])
+    gperm_max = max([e.p_off[n][2] for n in pk] + [8])
     e.gperm = torch.zeros(2 * gperm_max, dtype=torch.float32, device=dev)
 
-    P32 = lambda n: _ptr(e.params32, e.p_off[n][0])
-    G32 = lambda n: _ptr(e.grads32, e.p_off[n][0])
-    P16 = lambda n: _ptr(e.params16, e.p_off[n][0])
-    T16 = lambda n: _ptr(e.paramsT16, e.t_off[n][0])
-    PK = lambda n: _ptr(e.wpack16, pk_off[n][0])
-    PKT = lambda n: _ptr(e.wpackT16, pk_off[n][0])
-    PKD = lambda n: _ptr(e.wpackD16, pk_off[n][0])
+    P32, G32, P16, T16 = e._p32, e._g32, e._p16, e._t16
 
     deep = spec.stem_type == "deep"
-    if deep and e.stem_impl != "gemm":
-        raise ValueError("stem_impl=%r: the deep stem's first convolution is planned through dfd_stem_im2col (stem_impl='gemm')"
-                         % (e.stem_impl,))
     sw = spec.stem_width
     stem_w, stem_bn = spec.stem_conv + ".weight", spec.stem_bn
     se = spec.se_reduction > 0
@@ -166,10 +137,11 @@ def build_resnet(e):
     def conv3x3(xin, name, y, h, w, cin, cout, stride, bn):
         """3x3 / padding 1 forward into y (+ BatchNorm statistics of y)"""
         if implicit and cin % 64 == 0 and cout % 64 == 0:
-            return [("dfd_conv_tc", (xin, PK(name), y, N, h, w, cin, cout, 3, stride, dt) + e._stats(bn) + (None,))]
+            return [("dfd_conv_tc", (xin, _ptr(e.wpack16, pk[name]), y, N, h, w, cin, cout, 3, stride, dt) + e._stats(bn)
+                     + (None,))]
         ho, wo = conv_out(h, 3, stride, 1), conv_out(w, 3, stride, 1)
         return [("dfd_im2col", (xin, COLS, N, h, w, cin, 3, stride, 1, dt)),
-                gemm(COLS, PK(name), y, N * ho * wo, cout, 9 * cin, bn)]
+                gemm(COLS, _ptr(e.wpack16, pk[name]), y, N * ho * wo, cout, 9 * cin, bn)]
 
     # ---- stochastic regularisation (training only): DropBlock sites, drop-path gates, classifier dropout ---------------
     dp_rate, db_rate = e.drop_path_rate, e.drop_block_rate
@@ -197,12 +169,11 @@ def build_resnet(e):
         e._drop_block_table = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(dev)
     e.drop_block_sites = sites
     e.drop_masks = OrderedDict()            # block -> drop-path gate [N, cout] (0 or 1 / keep per sample)
-    masks = []                              # dfd_rng_masks table: (tensor, rows, width, keep_prob)
     if dp_rate > 0.0:
         for b in spec.blocks:               # one DropPath(drop_path_rate) shared by every block, resnet.py:385
             gate = torch.ones(N, b.cout, dtype=torch.float32, device=dev)
             e.drop_masks[b.name] = gate
-            masks.append((gate, N, b.cout, 1.0 - dp_rate))
+            e._masks.append((gate, N, b.cout, 1.0 - dp_rate))
 
     def site_args(name):
         """(mask, kept, numel) operands of a DropBlock site"""
@@ -227,7 +198,6 @@ def build_resnet(e):
     gA, gB, gC, gD, gE, gF = [_ptr(t) for t in e.gbuf]
 
     # ---- forward -----------------------------------------------------------------------------------------
-    e.x_in = torch.zeros(N, spec.in_chans, e.H, e.W, dtype=e.tdtype, device=dev)
     y0 = e._alloc16(N, H1, W1, 64)
     a0 = e._alloc16(N, H1, W1, 64)
     x0 = e._alloc16(N, H2, W2, 64)
@@ -238,22 +208,15 @@ def build_resnet(e):
         bs0, bs1 = bns["conv1.1"], bns["conv1.4"]
         ys0, as0 = e._alloc16(N, H1, W1, sw), e._alloc16(N, H1, W1, sw)
         ys1, as1 = e._alloc16(N, H1, W1, sw), e._alloc16(N, H1, W1, sw)
-        taps, Kp = e._stem_gemm_setup("conv1.0.weight", sw, 3, N * H1 * W1)
-        fwd.append(("dfd_stem_im2col", (_ptr(e.x_in), _ptr(e.stem_cols), N, spec.in_chans, e.H, e.W, 3, 2, 1, Kp, dt)))
-        fwd.append(gemm(_ptr(e.stem_cols), _ptr(e.stem_wpad), _ptr(ys0), N * H1 * W1, sw, Kp, bs0))
+        fwd += e._stem_gemm("conv1.0.weight", sw, 3, 2, 1, ys0, N * H1 * W1, bs0, rowpack=False)
         fwd += finalize(bs0, N * H1 * W1)
         fwd.append(bn_relu(ys0, bs0, as0, H1 * W1, sw))
         fwd += conv3x3(_ptr(as0), "conv1.3.weight", _ptr(ys1), H1, W1, sw, sw, 1, bs1)
         fwd += finalize(bs1, N * H1 * W1)
         fwd.append(bn_relu(ys1, bs1, as1, H1 * W1, sw))
         fwd += conv3x3(_ptr(as1), "conv1.6.weight", _ptr(y0), H1, W1, sw, 64, 1, bn0)
-    elif e.stem_impl == "gemm":
-        taps, Kp = e._stem_gemm_setup(stem_w, 64, 7, N * H1 * W1)
-        fwd.append(("dfd_stem_im2col", (_ptr(e.x_in), _ptr(e.stem_cols), N, spec.in_chans, e.H, e.W, 7, 2, 3, Kp, dt)))
-        fwd.append(gemm(_ptr(e.stem_cols), _ptr(e.stem_wpad), _ptr(y0), N * H1 * W1, 64, Kp, bn0))
     else:
-        fwd.append(("dfd_stem_fwd", (_ptr(e.x_in), P32(stem_w), _ptr(y0), N, spec.in_chans, e.H, e.W, 64, 7, 2, 3, dt)
-                    + e._stats(bn0)))
+        fwd += e._stem_gemm(stem_w, 64, 7, 2, 3, y0, N * H1 * W1, bn0, rowpack=False)
     fwd += finalize(bn0, N * H1 * W1)
     fwd.append(bn_relu(y0, bn0, a0, H1 * W1, 64))
     pool_op = "dfd_maxpool_ceil" if spec.stem_pool == "ceil" else "dfd_maxpool"
@@ -374,27 +337,9 @@ def build_resnet(e):
         rec["out"] = out
         recs.append(rec)
         x = out
-    F, K = spec.num_features, spec.num_classes
-    P, pool_t = spec.pooled_features, _lib.POOL_TYPES[spec.global_pool]
-    e.pooled = torch.zeros(N, P, dtype=torch.float32, device=dev)
-    e.pool_partial = torch.zeros(8 * N * F, dtype=torch.float32, device=dev)
-    if pool_t == _lib.POOL_TYPES["avg"]:
-        fwd.append(("dfd_pool", (_ptr(x), None, None, _ptr(e.pooled), N, Hf * Wf, F, ACT_NONE, dt, _ptr(e.pool_partial), 8)))
-    else:
-        e.pool_argmax = torch.zeros(N, F, dtype=torch.int32, device=dev)
-        fwd.append(("dfd_global_pool", (_ptr(x), None, None, _ptr(e.pooled), _ptr(e.pool_argmax), N, Hf * Wf, F, ACT_NONE,
-                                        pool_t, dt, 8)))
-    if e.drop_rate > 0.0:
-        # F.dropout on the pooled vector before fc (resnet.py:465-466), with a mask already divided by keep
-        e.dropout_mask = torch.ones(N, P, dtype=torch.float32, device=dev)
-        masks.append((e.dropout_mask, N * P, 1, 1.0 - e.drop_rate))
-        fwd.append(("dfd_mul_f32_train", (_ptr(e.pooled), _ptr(e.dropout_mask), N * P)))
-    fwd = e._mask_head(masks, len(sites)) + fwd
-    e.logits = torch.zeros(N, K, dtype=torch.float32, device=dev)
-    e.dlogits = torch.zeros(N, K, dtype=torch.float32, device=dev)
-    e.dpooled = torch.zeros(N, P, dtype=torch.float32, device=dev)
-    e.target_i = torch.zeros(N, dtype=torch.int64, device=dev)
-    e.target_f = torch.zeros(N, K, dtype=torch.float32, device=dev)
+    e.pool_partial = torch.zeros(8 * N * spec.num_features, dtype=torch.float32, device=dev)
+    # global pool, then F.dropout on the pooled vector before fc (resnet.py:465-466)
+    fwd += e._pool_head(x, None, ACT_NONE, Hf * Wf, e.drop_rate, partial=_ptr(e.pool_partial))
 
     # ---- backward ----------------------------------------------------------------------------------------
     pending_unpack = []         # (gperm region pointer, name, Cout, Cin): unpacked after the block's ordered reduce
@@ -413,12 +358,12 @@ def build_resnet(e):
         """dy [M_out, Cout] -> dx_out [N, n_h, n_w, Cin] (+dx_add) and the weight gradient of `name`"""
         if implicit and stride == 1 and dx_add is None and Cin % 64 == 0 and Cout % 64 == 0:
             # input gradient = the same implicit GEMM on dY with the tap-flipped [Cin][kh'][kw'][Cout] weights
-            ops = [("dfd_conv_tc", (dy, PKD(name), dx_out, N, n_h, n_w, Cout, Cin, 3, 1, dt, None, None, None))]
+            ops = [("dfd_conv_tc", (dy, _ptr(e.wpackD16, pk[name]), dx_out, N, n_h, n_w, Cout, Cin, 3, 1, dt, None, None, None))]
         elif implicit and stride == 2 and dx_add is None and Cin % 64 == 0 and Cout % 64 == 0:
             # strided input gradient: four parity-class implicit GEMMs storing through strided views of dx
-            ops = [("dfd_conv_dgrad_s2_tc", (dy, PKD(name), dx_out, N, n_h, n_w, Cin, Cout, dt))]
+            ops = [("dfd_conv_dgrad_s2_tc", (dy, _ptr(e.wpackD16, pk[name]), dx_out, N, n_h, n_w, Cin, Cout, dt))]
         else:
-            ops = [gemm(dy, PKT(name), COLS, M_out, 9 * Cin, Cout),
+            ops = [gemm(dy, _ptr(e.wpackT16, pk[name]), COLS, M_out, 9 * Cin, Cout),
                    ("dfd_col2im", (COLS, dx_add, dx_out, N, n_h, n_w, Cin, 3, stride, 1, dt))]
         gp = _ptr(e.gperm, len(pending_unpack) * gperm_max)         # this block's next free region
         assert len(pending_unpack) < 2
@@ -432,15 +377,7 @@ def build_resnet(e):
         pending_unpack.append((gp, name, Cout, Cin))     # complete after the block's ordered reduce (flush_block)
         return ops
 
-    bwd.append(("dfd_head_bwd", (_ptr(e.dlogits), _ptr(e.pooled), P32(e.cls_name + ".weight"), G32(e.cls_name + ".weight"),
-                                 G32(e.cls_name + ".bias"),
-                                 _ptr(e.dpooled), N, P, K)))
-    if e.drop_rate > 0.0:
-        bwd.append(("dfd_mul_f32", (_ptr(e.dpooled), _ptr(e.dropout_mask), N * P)))
-    if pool_t == _lib.POOL_TYPES["avg"]:
-        bwd.append(("dfd_pool_bwd", (_ptr(e.dpooled), gA, N, Hf * Wf, F, dt)))
-    else:
-        bwd.append(("dfd_gpool_bwd", (_ptr(e.dpooled), _ptr(e.pool_argmax), gA, N, Hf * Wf, F, pool_t, dt)))
+    bwd += e._pool_head_bwd(gA)
     # The gradient entering a block is kept as up to TWO tensors (main-path dx + identity-path gm of the block above): the
     # fused ReLU / BN-backward reduction adds them on the fly (dfd_relu_bn_bwd_reduce), which removes the materialised
     # residual add of every block without a downsample branch.
@@ -485,14 +422,14 @@ def build_resnet(e):
                                                    b.cout, dt, bl.bs1, bl.bs2)))
         gd = t2 if (b.cse or rec["site_last"] in sites or rec["gate"] is not None) else gm
         bwd += bwd_finalize(bl, M2)
-        bwd.append(("dfd_bn_bwd_apply", (gd, _ptr(rec["ylast"]), None, bl.cA, bl.cB, bl.cC, t1, N, ho * wo, b.cout, dt)))
+        bwd.append(e._bn_apply(gd, rec["ylast"], bl, t1, ho * wo, b.cout))
         if b.kind == "basic":
             bn1 = bns[p + ".bn1"]
             # conv2 (3x3 s1): dy2 = t1 -> da1 = t2
             bwd += conv3x3_bwd(p + ".conv2.weight", t1, M2, b.planes, b.cout, rec["a1"], ho, wo, 1, t2)
             bwd.append(relu_bwd(t2, rec["y1"], bn1, t1, ho * wo, b.planes, p + ".bn1"))
             bwd += bwd_finalize(bn1, M2)
-            bwd.append(("dfd_bn_bwd_apply", (t1, _ptr(rec["y1"]), None, bn1.cA, bn1.cB, bn1.cC, t2, N, ho * wo, b.planes, dt)))
+            bwd.append(e._bn_apply(t1, rec["y1"], bn1, t2, ho * wo, b.planes))
             # conv1 (3x3 stride s): dy1 = t2 -> dx = t3 [M1, cin]
             bwd += conv3x3_bwd(p + ".conv1.weight", t2, M2, b.cin, b.planes, xin, h, w, b.stride, t3)
         else:
@@ -502,7 +439,7 @@ def build_resnet(e):
             bwd.append(e._wgrad(t1, _ptr(rec["a2"]), G32(p + ".conv3.weight"), M2, b.cout, b.width))
             bwd.append(relu_bwd(t2, rec["y2"], bn2, t1, ho * wo, b.width, p + ".bn2"))
             bwd += bwd_finalize(bn2, M2)
-            bwd.append(("dfd_bn_bwd_apply", (t1, _ptr(rec["y2"]), None, bn2.cA, bn2.cB, bn2.cC, t2, N, ho * wo, b.width, dt)))
+            bwd.append(e._bn_apply(t1, rec["y2"], bn2, t2, ho * wo, b.width))
             s1x1 = rec["s1x1"]
             h1, w1 = (ho, wo) if s1x1 else (h, w)
             M1b = N * h1 * w1
@@ -510,7 +447,7 @@ def build_resnet(e):
             bwd += conv3x3_bwd(p + ".conv2.weight", t2, M2, b.width, b.width, rec["a1"], h1, w1, 1 if s1x1 else b.stride, t1)
             bwd.append(relu_bwd(t1, rec["y1"], bn1, t2, h1 * w1, b.width, p + ".bn1"))
             bwd += bwd_finalize(bn1, M1b)
-            bwd.append(("dfd_bn_bwd_apply", (t2, _ptr(rec["y1"]), None, bn1.cA, bn1.cB, bn1.cC, t1, N, h1 * w1, b.width, dt)))
+            bwd.append(e._bn_apply(t2, rec["y1"], bn1, t1, h1 * w1, b.width))
             c1 = p + ".conv1.weight"
             if not s1x1:
                 # conv1 (1x1): dy1 = t1 -> dx = t3 [M1, cin]
@@ -532,7 +469,7 @@ def build_resnet(e):
             bnd = rec["bnd"]
             bwd.append(("dfd_bn_bwd_reduce", (gm, _ptr(rec["yd"]), None, bnd.mean, bnd.rstd, N, ho * wo, b.cout, dt, bnd.bs1, bnd.bs2, None)))
             bwd += bwd_finalize(bnd, M2)
-            bwd.append(("dfd_bn_bwd_apply", (gm, _ptr(rec["yd"]), None, bnd.cA, bnd.cB, bnd.cC, t1, N, ho * wo, b.cout, dt)))
+            bwd.append(e._bn_apply(gm, rec["yd"], bnd, t1, ho * wo, b.cout))
             pooled = b.avg_down and b.stride != 1
             ds_add = implicit and b.cin % 64 == 0 and b.cout % 64 == 0 and not pooled
             dsw = rec["dsw"]
@@ -573,30 +510,19 @@ def build_resnet(e):
     bwd.append(("dfd_act_bwd", (t1, _ptr(y0), bn0.scale, bn0.shift, bn0.mean, bn0.rstd, None, None, t2, N, H1 * W1, 64,
                                 ACT_RELU, dt, bn0.bs1, bn0.bs2, None)))
     bwd += bwd_finalize(bn0, N * H1 * W1)
+    bwd.append(e._bn_apply(t2, y0, bn0, t1, H1 * W1, 64))
     if deep:
-        M0 = N * H1 * W1
-        bwd.append(("dfd_bn_bwd_apply", (t2, _ptr(y0), None, bn0.cA, bn0.cB, bn0.cC, t1, N, H1 * W1, 64, dt)))
         # conv1.6 and conv1.3 take the two packed-gradient regions; conv1.0's gradient goes through the padded stem buffer.
-        # One ordered reduce for the three, then the unpack / unpad passes.
+        M0 = N * H1 * W1
         bwd += conv3x3_bwd("conv1.6.weight", t1, M0, sw, 64, as1, H1, W1, 1, t2)
         bwd.append(relu_bwd(t2, ys1, bs1, t1, H1 * W1, sw, None))
         bwd += bwd_finalize(bs1, M0)
-        bwd.append(("dfd_bn_bwd_apply", (t1, _ptr(ys1), None, bs1.cA, bs1.cB, bs1.cC, t2, N, H1 * W1, sw, dt)))
+        bwd.append(e._bn_apply(t1, ys1, bs1, t2, H1 * W1, sw))
         bwd += conv3x3_bwd("conv1.3.weight", t2, M0, sw, sw, as0, H1, W1, 1, t1)
         bwd.append(relu_bwd(t1, ys0, bs0, t2, H1 * W1, sw, None))
         bwd += bwd_finalize(bs0, M0)
-        bwd.append(("dfd_bn_bwd_apply", (t2, _ptr(ys0), None, bs0.cA, bs0.cB, bs0.cC, t1, N, H1 * W1, sw, dt)))
-        bwd.append(("dfd_memset_async", (_ptr(e.stem_gpad), 0, sw * Kp * 4)))
-        bwd.append(e._wgrad(t1, _ptr(e.stem_cols), _ptr(e.stem_gpad), M0, sw, Kp))
-        flush_block(bwd)
-        bwd.append(("dfd_unpad_grad", (_ptr(e.stem_gpad), G32("conv1.0.weight"), sw, taps, Kp)))
-    elif e.stem_impl == "gemm":
-        bwd.append(("dfd_bn_bwd_apply", (t2, _ptr(y0), None, bn0.cA, bn0.cB, bn0.cC, t1, N, H1 * W1, 64, dt)))
-        bwd.append(("dfd_memset_async", (_ptr(e.stem_gpad), 0, 64 * Kp * 4)))
-        bwd.append(e._wgrad(t1, _ptr(e.stem_cols), _ptr(e.stem_gpad), N * H1 * W1, 64, Kp))
-        e._flush_reduce(bwd)
-        bwd.append(("dfd_unpad_grad", (_ptr(e.stem_gpad), G32(stem_w), 64, taps, Kp)))
-    else:
-        bwd.append(("dfd_stem_wgrad", (_ptr(e.x_in), t2, _ptr(y0), bn0.cA, bn0.cB, bn0.cC, G32(stem_w), N, spec.in_chans,
-                                       e.H, e.W, 64, 7, 2, 3, dt)))
-    e._finish_plan(fwd, bwd)
+        bwd.append(e._bn_apply(t2, ys0, bs0, t1, H1 * W1, sw))
+    bwd += e._stem_wgrad(t1)
+    flush_block(bwd)            # one ordered reduce for the stem's weight gradients, then the unpack / unpad passes
+    bwd.append(e._stem_unpad())
+    e._finish_plan(fwd, bwd, len(sites))

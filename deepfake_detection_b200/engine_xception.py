@@ -22,43 +22,21 @@ Plan:
     which masks by the staged 16-bit input and reduces the preceding BN's backward sums (or adds the identity gradient).
 Dropout: the reference calls F.dropout and discards its result (xception.py:214-215); `drop_rate` changes nothing here.
 """
-import struct
-
 import torch
 
-from . import _lib
 from .arch import xception_extents
-from .engine import ACT_NONE, ACT_RELU, POOL_CHUNKS, _ptr
+from .engine import ACT_NONE, ACT_RELU, _ptr
 
 
 def build_xception(e):
     spec, N, dev, dt = e.spec, e.N, e.device, e.dt
-    e._keep = []
-    e.acts = {}
     fwd, bwd = [], []
-    if e.stem_impl != "gemm":
-        raise ValueError("stem_impl=%r: the Xception stem is planned through dfd_stem_im2col (stem_impl='gemm')" % (e.stem_impl,))
 
     # ---- packed (kh, kw, ci) copy of conv2's weight (the im2col GEMM's B operand, its transpose and the dgrad layout) -------
-    o2, O2, I2, k2 = e.p_off["conv2.weight"][0], 64, 32, 3
-    ar = e.arena
-    if getattr(ar, "wpack16", None) is None:
-        n2 = O2 * I2 * k2 * k2
-        ar.wpack16 = torch.zeros(n2, dtype=e.tdtype, device=dev)
-        ar.wpackT16 = torch.zeros(n2, dtype=e.tdtype, device=dev)
-        ar.wpackD16 = torch.zeros(n2, dtype=e.tdtype, device=dev)
-        raw = struct.pack("<QQQQiiii", _ptr(e.params16, o2), _ptr(ar.wpack16), _ptr(ar.wpackT16), _ptr(ar.wpackD16), O2, I2, k2, 0)
-        ar._rtable = torch.frombuffer(bytearray(raw), dtype=torch.uint8).to(dev)
-        ar._rtable_count = 1
-        ar._derived_dirty = True
-        ar.layout_gen += 1
-    e.wpack16, e.wpackT16 = ar.wpack16, ar.wpackT16
-    e.gperm = torch.zeros(O2 * I2 * k2 * k2, dtype=torch.float32, device=dev)
+    e._packed_weights(["conv2.weight"])
+    e.gperm = torch.zeros(e.p_off["conv2.weight"][2], dtype=torch.float32, device=dev)
 
-    P32 = lambda n: _ptr(e.params32, e.p_off[n][0])
-    G32 = lambda n: _ptr(e.grads32, e.p_off[n][0])
-    P16 = lambda n: _ptr(e.params16, e.p_off[n][0])
-    T16 = lambda n: _ptr(e.paramsT16, e.t_off[n][0])
+    P32, G32, P16, T16 = e._p32, e._g32, e._p16, e._t16
 
     # ---- shapes ------------------------------------------------------------------------------------------
     ext = xception_extents(e.H, e.W)
@@ -97,13 +75,10 @@ def build_xception(e):
     COLS = _ptr(e.cols)
 
     # ---- forward: stem -------------------------------------------------------------------------------------
-    e.x_in = torch.zeros(N, spec.in_chans, e.H, e.W, dtype=e.tdtype, device=dev)
     bn1, bn2 = bns["bn1"], bns["bn2"]
     y1, a1 = e._alloc16(N, H1, W1, 32), e._alloc16(N, H1, W1, 32)
     y2, a2 = e._alloc16(N, H2, W2, 64), e._alloc16(N, H2, W2, 64)
-    taps, Kp = e._stem_gemm_setup("conv1.weight", 32, 3, N * H1 * W1)
-    fwd.append(("dfd_stem_im2col", (_ptr(e.x_in), _ptr(e.stem_cols), N, spec.in_chans, e.H, e.W, 3, 2, 0, Kp, dt)))
-    fwd.append(gemm(_ptr(e.stem_cols), _ptr(e.stem_wpad), _ptr(y1), N * H1 * W1, 32, Kp, bn1))
+    fwd += e._stem_gemm("conv1.weight", 32, 3, 2, 0, y1, N * H1 * W1, bn1, rowpack=False)
     fwd += finalize(bn1, N * H1 * W1)
     fwd.append(("dfd_bn_act", (_ptr(y1), bn1.scale, bn1.shift, None, None, _ptr(a1), N, H1 * W1, 32, ACT_RELU, 0, dt)))
     fwd.append(("dfd_im2col", (_ptr(a1), COLS, N, H1, W1, 32, 3, 1, 0, dt)))
@@ -163,7 +138,7 @@ def build_xception(e):
 
     # ---- forward: conv3 / conv4 and the head -----------------------------------------------------------------
     bn3, bn4 = bns["bn3"], bns["bn4"]
-    F, K = spec.num_features, spec.num_classes
+    F = spec.num_features
     d3, y3 = e._alloc16(N, Hf, Wf, 1024), e._alloc16(N, Hf, Wf, 1536)
     d4, y4 = e._alloc16(N, Hf, Wf, 1536), e._alloc16(N, Hf, Wf, F)
     fwd.append(dw_fwd(_ptr(x), None, None, "conv3.conv1.weight", d3, Hf, Wf, 1024, ACT_NONE))
@@ -173,30 +148,14 @@ def build_xception(e):
     fwd.append(gemm(_ptr(d4), P16("conv4.pointwise.weight"), _ptr(y4), Mf, F, 1536, bn4))
     fwd += finalize(bn4, Mf)
     e.acts["conv4"] = y4
-    P, pool_t = spec.pooled_features, _lib.POOL_TYPES[spec.global_pool]
-    e.pooled = torch.zeros(N, P, dtype=torch.float32, device=dev)
-    if pool_t == _lib.POOL_TYPES["avg"]:
-        fwd.append(("dfd_pool", (_ptr(y4), bn4.scale, bn4.shift, _ptr(e.pooled), N, Hf * Wf, F, ACT_RELU, dt, None,
-                                 POOL_CHUNKS)))
-    else:
-        e.pool_argmax = torch.zeros(N, F, dtype=torch.int32, device=dev)
-        fwd.append(("dfd_global_pool", (_ptr(y4), bn4.scale, bn4.shift, _ptr(e.pooled), _ptr(e.pool_argmax), N, Hf * Wf, F,
-                                        ACT_RELU, pool_t, dt, POOL_CHUNKS)))
+    fwd += e._pool_head(y4, bn4, ACT_RELU, Hf * Wf, 0.0)         # no dropout: see the module docstring
     e.drop_masks = {}
-    e.logits = torch.zeros(N, K, dtype=torch.float32, device=dev)
-    e.dlogits = torch.zeros(N, K, dtype=torch.float32, device=dev)
-    e.dpooled = torch.zeros(N, P, dtype=torch.float32, device=dev)
-    e.target_i = torch.zeros(N, dtype=torch.int64, device=dev)
-    e.target_f = torch.zeros(N, K, dtype=torch.float32, device=dev)
 
     # ---- backward ----------------------------------------------------------------------------------------
     bufs = [_ptr(t) for t in e.gbuf]
 
     def free(*used):
         return [g for g in bufs if g not in used]
-
-    def bn_apply(g, y, bn, out, hw, C):
-        return ("dfd_bn_bwd_apply", (g, _ptr(y), None, bn.cA, bn.cB, bn.cC, out, N, hw, C, dt))
 
     def dw_bwd(gy, name, xin, bn_in, add, gx, h, w, C, mode):
         """fused depthwise backward: mode "bn_relu" (input relu(bn_in(xin)), bn_in's backward sums), "relu" (input relu(xin),
@@ -218,21 +177,14 @@ def build_xception(e):
                 e._wgrad(gy, _ptr(s["d"]), G32(s["name"] + ".pointwise.weight"), M, s["co"], s["ci"]),
                 dw_bwd(gd, s["name"] + ".conv1.weight", xin, bn_in, add, gx, h, w, s["ci"], mode)]
 
-    bwd.append(("dfd_head_bwd", (_ptr(e.dlogits), _ptr(e.pooled), P32("fc.weight"), G32("fc.weight"), G32("fc.bias"),
-                                 _ptr(e.dpooled), N, P, K)))
     gA, gB, gC, gD = bufs[:4]
-    if pool_t == _lib.POOL_TYPES["avg"]:
-        bwd.append(("dfd_act_bwd", (None, _ptr(y4), bn4.scale, bn4.shift, bn4.mean, bn4.rstd, None, _ptr(e.dpooled), gA, N,
-                                    Hf * Wf, F, ACT_RELU, dt, bn4.bs1, bn4.bs2, None)))
-    else:
-        bwd.append(("dfd_act_bwd_gpool", (_ptr(y4), bn4.scale, bn4.shift, bn4.mean, bn4.rstd, _ptr(e.dpooled), _ptr(e.pool_argmax),
-                                          gA, N, Hf * Wf, F, ACT_RELU, pool_t, dt, bn4.bs1, bn4.bs2, None)))
+    bwd += e._pool_head_bwd(gA)
     bwd += bwd_finalize(bn4, Mf)
-    bwd.append(bn_apply(gA, y4, bn4, gB, Hf * Wf, F))
+    bwd.append(e._bn_apply(gA, y4, bn4, gB, Hf * Wf, F))
     s4 = dict(name="conv4", ci=1536, co=F, d=d4)
     bwd += sep_bwd(gB, s4, bn3, y3, None, gC, Hf, Wf, "bn_relu")
     bwd += bwd_finalize(bn3, Mf)
-    bwd.append(bn_apply(gC, y3, bn3, gB, Hf * Wf, 1536))
+    bwd.append(e._bn_apply(gC, y3, bn3, gB, Hf * Wf, 1536))
     s3 = dict(name="conv3", ci=1024, co=1536, d=d3)
     bwd += sep_bwd(gB, s3, None, x, None, gC, Hf, Wf, "plain")
     e._flush_reduce(bwd)
@@ -248,16 +200,16 @@ def build_xception(e):
             bwd.append(("dfd_maxpool_bn_bwd_reduce", (dout, _ptr(rec["idx"]), _ptr(last["y"]), last["bn"].mean, last["bn"].rstd,
                                                       gbn, N, h, w, b.cout, dt, last["bn"].bs1, last["bn"].bs2)))
             bwd += bwd_finalize(last["bn"], M1)
-            bwd.append(bn_apply(gbn, last["y"], last["bn"], gy, h * w, b.cout))
+            bwd.append(e._bn_apply(gbn, last["y"], last["bn"], gy, h * w, b.cout))
             bwd.append(("dfd_bn_bwd_reduce", (dout, _ptr(rec["yd"]), None, bnd.mean, bnd.rstd, N, ho * wo, b.cout, dt, bnd.bs1,
                                               bnd.bs2, None)))
             bwd += bwd_finalize(bnd, M2)
-            bwd.append(bn_apply(dout, rec["yd"], bnd, gyd, ho * wo, b.cout))
+            bwd.append(e._bn_apply(dout, rec["yd"], bnd, gyd, ho * wo, b.cout))
         else:
             bwd.append(("dfd_bn_bwd_reduce", (dout, _ptr(last["y"]), None, last["bn"].mean, last["bn"].rstd, N, h * w, b.cout, dt,
                                               last["bn"].bs1, last["bn"].bs2, None)))
             bwd += bwd_finalize(last["bn"], M1)
-            bwd.append(bn_apply(dout, last["y"], last["bn"], gy, h * w, b.cout))
+            bwd.append(e._bn_apply(dout, last["y"], last["bn"], gy, h * w, b.cout))
             gyd = None
         # separable convolutions, last to first: gy is the gradient of the current pointwise output
         for j in range(len(seps) - 1, 0, -1):
@@ -265,7 +217,7 @@ def build_xception(e):
             gu = free(dout, gy, gyd)[0]
             bwd += sep_bwd(gy, seps[j], prev["bn"], prev["y"], None, gu, h, w, "bn_relu", keep=(dout, gyd))
             bwd += bwd_finalize(prev["bn"], M1)
-            bwd.append(bn_apply(gu, prev["y"], prev["bn"], gy, h * w, prev["co"]))
+            bwd.append(e._bn_apply(gu, prev["y"], prev["bn"], gy, h * w, prev["co"]))
         mode = "relu" if b.start_with_relu else "plain"
         gx = free(dout, gy, gyd)[0]
         bwd += sep_bwd(gy, seps[0], None, xin, None if b.skip else dout, gx, h, w, mode, keep=(gyd,))
@@ -289,7 +241,7 @@ def build_xception(e):
     bwd.append(("dfd_act_bwd", (dout, _ptr(y2), bn2.scale, bn2.shift, bn2.mean, bn2.rstd, None, None, gu, N, H2 * W2, 64,
                                 ACT_RELU, dt, bn2.bs1, bn2.bs2, None)))
     bwd += bwd_finalize(bn2, N * H2 * W2)
-    bwd.append(bn_apply(gu, y2, bn2, gy, H2 * W2, 64))
+    bwd.append(e._bn_apply(gu, y2, bn2, gy, H2 * W2, 64))
     ga1 = free(gy)[0]
     bwd.append(gemm(gy, _ptr(e.wpackT16), COLS, N * H2 * W2, 9 * 32, 64))
     bwd.append(("dfd_col2im", (COLS, None, ga1, N, H1, W1, 32, 3, 1, 0, dt)))
@@ -300,10 +252,9 @@ def build_xception(e):
     bwd.append(("dfd_act_bwd", (ga1, _ptr(y1), bn1.scale, bn1.shift, bn1.mean, bn1.rstd, None, None, gu, N, H1 * W1, 32,
                                 ACT_RELU, dt, bn1.bs1, bn1.bs2, None)))
     bwd += bwd_finalize(bn1, N * H1 * W1)
-    bwd.append(bn_apply(gu, y1, bn1, gy1, H1 * W1, 32))
-    bwd.append(("dfd_memset_async", (_ptr(e.stem_gpad), 0, 32 * Kp * 4)))
-    bwd.append(e._wgrad(gy1, _ptr(e.stem_cols), _ptr(e.stem_gpad), N * H1 * W1, 32, Kp))
+    bwd.append(e._bn_apply(gu, y1, bn1, gy1, H1 * W1, 32))
+    bwd += e._stem_wgrad(gy1)
     e._flush_reduce(bwd)
     bwd.append(("dfd_unpack_grad", (_ptr(e.gperm), G32("conv2.weight"), 64, 32, 3)))
-    bwd.append(("dfd_unpad_grad", (_ptr(e.stem_gpad), G32("conv1.weight"), 32, taps, Kp)))
+    bwd.append(e._stem_unpad())
     e._finish_plan(fwd, bwd)

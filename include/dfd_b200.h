@@ -132,15 +132,9 @@ int dfd_dwconv_bwd_pad(const void* gy, const void* yout, const float* cA, const 
                        int stride, int pad_t, int pad_l, int dt, double* s1, double* s2, void* ws, long long ws_bytes,
                        const void* fin, void* stream);
 
-/* ---- stem convolution: conv_stem 3x3 s2 (efficientnet.py:275,321) / conv1 7x7 s2 (resnet.py:379,451) ---- */
-int dfd_stem_fwd(const void* x_nchw, const float* w, void* out_nhwc, int N, int Cin, int H, int W, int Cout, int k,
-                 int stride, int pad, int dt, double* dsum, double* dsq, void* stream);
-int dfd_stem_wgrad(const void* x_nchw, const void* g, const void* y, const float* cA, const float* cB,
-                   const float* cC, float* dW, int N, int Cin, int H, int W, int Cout, int k, int stride, int pad,
-                   int dt, void* stream);
-
-/* stem as a GEMM (round-1 perf path): im2col of the NCHW image, column order (ci,kh,kw) == OIHW flattening, K padded to
- * Kp % 8 == 0; weights padded to [Cout, Kp]; fp32 gradient un-padded (accumulating) into the OIHW arena */
+/* ---- stem convolution: conv_stem 3x3 s2 (efficientnet.py:275,321) / conv1 7x7 s2 (resnet.py:379,451) ----
+ * as a GEMM: im2col of the NCHW image, column order (ci,kh,kw) == OIHW flattening, K padded to Kp % 8 == 0; weights padded
+ * to [Cout, Kp]; fp32 gradient un-padded (accumulating) into the OIHW arena */
 int dfd_stem_im2col(const void* x_nchw, void* cols, int N, int Cin, int H, int W, int k, int stride, int pad, int Kp, int dt,
                     void* stream);
 /* the same with TF "SAME" padding: Ho = ceil(H/stride), Wo = ceil(W/stride); pad_t / pad_l must be the begin sides,

@@ -287,7 +287,7 @@ def _dwconv_bwd_det(launch, w, dW_atomic, gx_ref, N, H, W, C, k, s, with_stats):
 
 
 def check_stem_gemm(N, Cin, H, W, Cout, k, s, pad, dtype=torch.bfloat16, seed=0, pack=1):
-    """the stem as the training plan runs it (stem_impl="gemm"): dfd_stem_im2col -> dfd_pad_weight -> the tensor-core GEMM with
+    """the stem as the training plan runs it: dfd_stem_im2col -> dfd_pad_weight -> the tensor-core GEMM with
     the BatchNorm statistics (pack 1: dfd_gemm_tn; else dfd_gemm_tn_rowpack on the block-diagonal copy of the padded weight,
     the plan's form for small Kp) -> order-deterministic dfd_gemm_wgrad into the Kp-padded gradient -> dfd_unpad_grad. im2col
     exact against F.unfold; output and weight gradient against fp64 products of the same rounded operands."""
@@ -366,35 +366,6 @@ def check_stem_im2col(N, Cin, H, W, k, s, pad, dtype=torch.bfloat16, seed=0):
     ref = F.unfold(x.float(), k, padding=pad, stride=s).transpose(1, 2).reshape(N * Ho * Wo, taps)
     return dict(diff=float((cols[:, :taps].float() - ref).abs().max()), pad_max=float(cols[:, taps:].float().abs().max()) if Kp > taps else 0.0,
                 nan=int(torch.isnan(cols.float()).sum()))
-
-
-def check_stem(N, Cin, H, W, Cout, k, dtype=torch.bfloat16, seed=0):
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    pad = (k - 1) // 2 if k == 3 else 3
-    x = torch.randn(N, Cin, H, W, device="cuda", generator=g).to(dtype)
-    w = (torch.randn(Cout, Cin, k, k, device="cuda", generator=g) / math.sqrt(Cin * k * k)).contiguous()
-    Ho, Wo = (H + 2 * pad - k) // 2 + 1, (W + 2 * pad - k) // 2 + 1
-    out = torch.full((N, Ho, Wo, Cout), float("nan"), device="cuda", dtype=dtype)
-    s1, s2 = stat_buf(Cout), stat_buf(Cout)
-    _lib.call("dfd_stem_fwd", P(x), P(w), P(out), N, Cin, H, W, Cout, k, 2, pad, DT[dtype], P(s1), P(s2), st())
-    torch.cuda.synchronize()
-    wr = w.clone().requires_grad_(True)
-    ref = F.conv2d(x.float(), wr, stride=2, padding=pad)
-    res = dict(fwd_max=maxerr_scaled(nchw(out.float()), ref.detach()), nan=int(torch.isnan(out.float()).sum()))
-    of = out.double()
-    res["sum_rel"] = relerr(s1.sum(0), of.sum((0, 1, 2)))
-    res["sq_rel"] = relerr(s2.sum(0), (of * of).sum((0, 1, 2)))
-    gy = (torch.randn(N, Ho, Wo, Cout, device="cuda", generator=g) * 0.1).to(dtype)
-    cA = 1.0 + 0.1 * torch.randn(Cout, device="cuda", generator=g)
-    cB = 0.05 * torch.randn(Cout, device="cuda", generator=g)
-    cC = 0.01 * torch.randn(Cout, device="cuda", generator=g)
-    dy = cA * gy.float() + cB * out.float() + cC
-    ref.backward(nchw(dy))
-    dW = torch.zeros_like(w)
-    _lib.call("dfd_stem_wgrad", P(x), P(gy), P(out), P(cA), P(cB), P(cC), P(dW), N, Cin, H, W, Cout, k, 2, pad, DT[dtype], st())
-    torch.cuda.synchronize()
-    res["wgrad_rel"] = relerr(dW, wr.grad)
-    return res
 
 
 def check_bn_chain(N, HW, C, dtype=torch.bfloat16, seed=0):

@@ -89,12 +89,6 @@ def test_dwconv_fp16():
     assert r["fwd_rel"] < 2e-3 and r["dgrad_rel"] < 4e-3 and r["wgrad_rel"] < RED, r
 
 
-@pytest.mark.parametrize("N,Cin,H,Cout,k", [(2, 3, 32, 32, 3), (2, 3, 38, 48, 3), (1, 12, 20, 256, 3), (2, 3, 32, 64, 7)])
-def test_stem(N, Cin, H, Cout, k):
-    r = _gc().check_stem(N, Cin, H, H, Cout, k)
-    assert r["nan"] == 0 and r["fwd_max"] < OUT16 and r["sum_rel"] < RED and r["sq_rel"] < RED and r["wgrad_rel"] < 1e-4, r
-
-
 @pytest.mark.parametrize("N,Cin,H,W,k,s,pad", [(2, 3, 32, 32, 3, 2, 1), (3, 3, 37, 45, 3, 2, 1), (2, 3, 64, 64, 7, 2, 3), (1, 4, 19, 23, 3, 1, 1)])
 def test_stem_im2col(N, Cin, H, W, k, s, pad):
     r = _gc().check_stem_im2col(N, Cin, H, W, k, s, pad)

@@ -92,7 +92,6 @@ def test_plan_builds_at_224(arch, in_chans):
     names = Counter(n for _, n, _ in e.fwd_ops + e.bwd_ops)
     deep = arch.endswith("d")
     assert names["dfd_avgpool2_fwd"] == names["dfd_avgpool2_bwd_add"] == (3 if deep else 0)
-    assert ("dfd_stem_fwd" in names) is False
     assert names["dfd_stem_im2col"] == 1 and names["dfd_unpad_grad"] == 1
     # every 3x3 with 64-multiple channels stays an implicit GEMM; the deep stem's two 32-channel 3x3s take im2col
     assert names["dfd_im2col"] == (4 if deep else 0)
@@ -142,12 +141,6 @@ def test_deep_stem_plan():
     assert tail.count("dfd_ordered_reduce") == 1 and tail[-4:] == ["dfd_ordered_reduce", "dfd_unpack_grad", "dfd_unpack_grad",
                                                                    "dfd_unpad_grad"]
     assert tail.count("dfd_col2im") == 2
-
-
-@pytest.mark.parametrize("stem_impl", ["fwd", "direct"])
-def test_deep_stem_refuses_other_stem_impls(stem_impl):
-    with pytest.raises(ValueError, match="deep stem"):
-        Engine("resnet26d", 2, 64, 64, device="plan-only", stem_impl=stem_impl)
 
 
 def test_drop_block_sites_and_drop_path():

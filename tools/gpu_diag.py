@@ -67,10 +67,10 @@ def main():
             run("dwconv_%d_%d_%d_%d_k%d_s%d_%s" % (N, H, W, C, k, s, aff), GC.check_dwconv, N, H, W, C, k, s, affine=aff)
         run("dwconv_fp16", GC.check_dwconv, 2, 14, 14, 80, 3, 1, dtype=torch.float16)
     if want("stem"):
-        run("stem_3", GC.check_stem, 2, 3, 32, 32, 32, 3)
-        run("stem_3_odd", GC.check_stem, 2, 3, 38, 38, 48, 3)
-        run("stem_12", GC.check_stem, 1, 12, 20, 20, 256, 3)
-        run("stem_7", GC.check_stem, 2, 3, 32, 32, 64, 7)
+        run("stem_3", GC.check_stem_gemm, 2, 3, 32, 32, 32, 3, 2, 1)
+        run("stem_3_odd", GC.check_stem_gemm, 2, 3, 38, 38, 48, 3, 2, 1)
+        run("stem_12", GC.check_stem_gemm, 1, 12, 20, 20, 256, 3, 2, 1)
+        run("stem_7", GC.check_stem_gemm, 2, 3, 32, 32, 64, 7, 2, 3)
     if want("bn"):
         for (N, HW, C) in [(3, 64, 32), (2, 49, 1152), (4, 200, 144), (2, 1000, 16)]:
             run("bn_chain_%d_%d_%d" % (N, HW, C), GC.check_bn_chain, N, HW, C)

@@ -36,21 +36,32 @@ SMALL = [
     ("efficientnet_b0", 2, 64, 64, dict(drop_rate=0.2, drop_path_rate=0.2)),
     ("efficientnet_b0", 2, 64, 64, dict(sync_bn=True)),
     ("efficientnet_b0", 2, 64, 64, dict(gemm_impl="mma")),
-    ("efficientnet_b0", 2, 64, 64, dict(stem_impl="direct")),
     ("efficientnet_b0", 3, 64, 64, dict(drop_rate=0.2, drop_path_rate=0.2, sync_bn=True)),
     ("efficientnet_b4", 1, 76, 76, {}),
     ("efficientnet_b0", 4, 224, 224, {}),
+    ("efficientnet_deepfake_v4", 1, 96, 96, dict(in_chans=12)),
     ("tf_efficientnet_b0", 2, 66, 96, {}),
     ("tf_efficientnet_b0", 2, 64, 96, {}),
-    ("tf_efficientnet_b0", 2, 65, 97, dict(stem_impl="direct")),
+    ("tf_efficientnet_b0", 2, 66, 96, dict(drop_rate=0.2, drop_path_rate=0.2)),
     ("resnet18", 2, 64, 64, {}),
     ("resnet18", 2, 64, 64, dict(gemm_impl="mma")),
-    ("resnet18", 2, 64, 64, dict(stem_impl="direct")),
+    ("resnet18", 2, 64, 64, dict(in_chans=1)),
     ("resnet18", 2, 160, 224, dict(drop_block_rate=0.1)),
     ("resnet18", 2, 160, 160, dict(drop_rate=0.2, drop_path_rate=0.1, drop_block_rate=0.1)),
+    ("resnet34", 2, 64, 64, dict(global_pool="avgmax")),
     ("resnet50", 2, 160, 160, dict(drop_rate=0.2, drop_path_rate=0.1, drop_block_rate=0.1)),
     ("resnet50", 2, 160, 160, dict(drop_path_rate=0.1)),
     ("resnet50", 3, 96, 96, {}),
+    ("wide_resnet50_2", 2, 64, 64, {}),
+    ("resnet26d", 2, 72, 88, {}),
+    ("resnet50d", 2, 160, 160, dict(drop_rate=0.2, drop_path_rate=0.1, drop_block_rate=0.1)),
+    ("resnet50d", 2, 64, 64, dict(gemm_impl="mma")),
+    ("seresnet18", 2, 70, 72, {}),
+    ("seresnet50", 2, 64, 64, dict(drop_rate=0.2)),
+    ("seresnet50", 2, 64, 64, dict(gemm_impl="mma")),
+    ("xception", 2, 64, 80, {}),
+    ("xception", 2, 64, 80, dict(gemm_impl="mma")),
+    ("xception", 2, 64, 80, dict(global_pool="catavgmax")),
 ] + [(a, 2, 64, 64, dict(global_pool=g)) for a in ("efficientnet_b0", "resnet18") for g in ("max", "avgmax", "catavgmax")]
 
 
