@@ -15,9 +15,8 @@ import torch
 from deepfake_detection_b200.arch import get_spec, param_entries
 from deepfake_detection_b200.engine import Engine
 from deepfake_detection_b200.optim import ArenaOptimizer
-from oracle import model as OM
 from oracle import train as OT
-from oracle.weights import synth_batch, synth_state
+from oracle.weights import synth_batch, synth_state, tame_state
 
 
 def relerr(a, b, floor=0.0):
@@ -48,12 +47,8 @@ def run_parity(arch, batch, H, W, dtype="bf16", steps=2, gemm_impl="tc", opt_kin
     spec = get_spec(arch)
     sd0 = synth_state(spec, seed=7)
     if tame and spec.family == "resnet":
-        # the reference zero-initialises the last BN gamma of every residual block (resnet.py:417-420); the synthetic
-        # weights use gamma ~ 1 everywhere, which makes a ReLU network's gradients chaotic under 16-bit rounding.
-        # Damping the residual branches (both implementations see the same weights) keeps the comparison informative.
-        for b in spec.blocks:
-            k = b.name + (".bn2.weight" if b.kind == "basic" else ".bn3.weight")
-            sd0[k] = sd0[k] * 0.2
+        # damping the residual branches (both implementations see the same weights) keeps the comparison informative
+        tame_state(spec, sd0)
     eng = Engine(arch, batch, H, W, dtype=dtype, gemm_impl=gemm_impl)
     eng.load_state_dict(sd0)
     wd = 1e-4
@@ -131,3 +126,12 @@ def golden_compare(case, golden_dir, dtype="bf16", gemm_impl="tc"):
         ref_logits = torch.tensor(st["logits"])
         out.append(dict(loss_native=float(eng.loss), loss_ref=st["loss"], logits_rel=relerr(eng.logits, ref_logits)))
     return out
+
+
+def engine_masks(eng):
+    """the DropBlock, drop-path and dropout masks a native ResNet engine drew for its last training step, in the layout of
+    oracle.train.train_step's `drop_block`, `drop_masks` and `dropout_mask` (CPU)"""
+    db = {k: m.permute(0, 3, 1, 2).float().cpu() for k, (m, _) in eng.drop_block_masks.items()}
+    dp = {k: g[:, 0].cpu().clone() for k, g in eng.drop_masks.items()}
+    dm = eng.dropout_mask.cpu().clone() if eng.drop_rate > 0 else None
+    return db, dp, dm

@@ -1,6 +1,6 @@
 """Selectable global pooling (avg / max / avgmax / catavgmax) on the host side, without a GPU.
 
-The pool oracle (tests/gpool_oracle.py) against oracle.train at 'avg' and against the global-pool fixtures minted from the UNMODIFIED reference (tools/mint_gpool_goldens.py) at the
+The oracle's pool (oracle.model.global_pool) at 'avg' against its default call form and against the global-pool fixtures minted from the UNMODIFIED reference (tools/mint_gpool_goldens.py) at the
 tolerances of test_head_multiclass_cpu.py; the arch restatement against the reference's catavgmax state_dict names and
 shapes; create_model / get_spec carrying the pool type; the plans of both families."""
 import json
@@ -10,10 +10,9 @@ import pytest
 import torch
 
 from deepfake_detection_b200.arch import SUPPORTED_ARCHS, get_spec, param_entries, state_entries
+from oracle import model as OM
 from oracle import train as OT
 from oracle.weights import synth_batch, synth_state
-
-import gpool_oracle as GO
 
 from test_head_multiclass_cpu import RTOL, _check_summ
 
@@ -30,7 +29,7 @@ def test_oracle_global_pool_steps_match_reference(case, golden_dir):
     opt = OT.OptState(kind=rec["opt"], lr=rec["lr"], momentum=rec["momentum"], weight_decay=rec["weight_decay"], eps=1e-8)
     for i, st in enumerate(rec["steps"]):
         x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=1234 + i, soft=rec["soft"], num_classes=K)
-        out = GO.train_step(spec, sd, x, y, opt, smoothing=rec["smoothing"])
+        out = OT.train_step(spec, sd, x, y, opt, smoothing=rec["smoothing"])
         _check_summ(out["logits"], st["logits"], "logits step %d" % i, rtol=1e-3)
         assert float(out["loss"]) == pytest.approx(st["loss"], rel=1e-4)
         assert float(out["prec1"]) == pytest.approx(st["prec1"], abs=1e-3)
@@ -43,27 +42,29 @@ def test_oracle_global_pool_steps_match_reference(case, golden_dir):
         for k, s in st["buffers"].items():
             _check_summ(sd[k].float(), s, "buffer %s step %d" % (k, i), rt)
     x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=999, num_classes=K)
-    ev = GO.validate_step(spec, sd, x, y)
+    ev = OT.validate_step(spec, sd, x, y)
     _check_summ(ev["logits"], rec["eval"]["logits"], "eval logits", rtol=5e-3)
 
 
 @pytest.mark.parametrize("arch", ["efficientnet_b0", "resnet18"])
 def test_pool_oracle_at_avg_is_the_oracle(arch):
-    """at 'avg' the pool oracle's train step is oracle.train.train_step bit for bit (16-bit emulation and dropout included)"""
+    """at an explicit 'avg' pool and BatchNorm the oracle's train step is its default one bit for bit (16-bit emulation and
+    dropout included)"""
     torch.set_num_threads(8)
     spec = get_spec(arch, num_classes=3)
     x, y = synth_batch(2, 3, 64, 64, seed=5, num_classes=3)
     mask = (torch.rand(2, spec.num_features, generator=torch.Generator().manual_seed(1)) > 0.3).float() / 0.7 \
         if spec.family == "efficientnet" else None
     outs = []
-    for step in (OT.train_step, GO.train_step):
+    for sp, kw in ((spec, {}), (get_spec(arch, num_classes=3, global_pool="avg"), dict(bn=OM.BNState(training=True)))):
         sd = synth_state(spec, seed=7)
-        outs.append((step(spec, sd, x, y, OT.OptState(kind="sgd", lr=0.01), act_dtype=torch.bfloat16, dropout_mask=mask), sd))
+        outs.append((OT.train_step(sp, sd, x, y, OT.OptState(kind="sgd", lr=0.01), act_dtype=torch.bfloat16, dropout_mask=mask,
+                                   **kw), sd))
     (a, sa), (b, sb) = outs
     assert torch.equal(a["logits"], b["logits"]) and torch.equal(a["loss"], b["loss"])
     assert all(torch.equal(a["grads"][k], b["grads"][k]) for k in a["grads"])
     assert all(torch.equal(sa[k], sb[k]) for k in sa)
-    ev = [f(spec, sa, x, y, act_dtype=torch.bfloat16)["logits"] for f in (OT.validate_step, GO.validate_step)]
+    ev = [OT.validate_step(spec, sa, x, y, act_dtype=torch.bfloat16, **kw)["logits"] for kw in ({}, dict(bn_eps=1e-5))]
     assert torch.equal(ev[0], ev[1])
 
 
@@ -77,15 +78,15 @@ def test_catavgmax_state_entries_match_reference(arch, golden_dir):
 
 
 def test_oracle_global_pool_matches_torch_pooling():
-    """gpool_oracle.global_pool is SelectAdaptivePool2d's arithmetic (adaptive_avgmax_pool.py:24-48)"""
+    """oracle.model.global_pool is SelectAdaptivePool2d's arithmetic (adaptive_avgmax_pool.py:24-48)"""
     x = torch.randn(3, 16, 5, 7, dtype=torch.float64)
     avg, mx = torch.nn.functional.adaptive_avg_pool2d(x, 1).flatten(1), torch.nn.functional.adaptive_max_pool2d(x, 1).flatten(1)
-    assert torch.equal(GO.global_pool(x, "avg"), x.mean((2, 3)))
-    assert torch.equal(GO.global_pool(x, "max"), mx)
-    assert torch.equal(GO.global_pool(x, "avgmax"), 0.5 * (avg + mx))
-    assert torch.equal(GO.global_pool(x, "catavgmax"), torch.cat((avg, mx), 1))
+    assert torch.equal(OM.global_pool(x, "avg"), x.mean((2, 3)))
+    assert torch.equal(OM.global_pool(x, "max"), mx)
+    assert torch.equal(OM.global_pool(x, "avgmax"), 0.5 * (avg + mx))
+    assert torch.equal(OM.global_pool(x, "catavgmax"), torch.cat((avg, mx), 1))
     with pytest.raises(ValueError):
-        GO.global_pool(x, "avgmaxc")
+        OM.global_pool(x, "avgmaxc")
 
 
 @pytest.mark.parametrize("gp", ["avg", "max", "avgmax", "catavgmax"])

@@ -16,8 +16,6 @@ import torch
 
 from deepfake_detection_b200 import _lib
 
-import gpool_oracle as GO
-
 pytestmark = pytest.mark.gpu
 
 PT = _lib.POOL_TYPES
@@ -242,7 +240,7 @@ def test_trainer_graph_step_matches_oracle(arch, batch, res, dtype, gp):
         x, y = synth_batch(batch, 3, res, res, seed=1234 + i, num_classes=K)
         loss, correct = tr.train_step(x.cuda(), y.cuda())
         torch.cuda.synchronize()
-        o = GO.train_step(spec, sd, x, y, ost, smoothing=0.1, act_dtype=TDT[dtype])
+        o = OT.train_step(spec, sd, x, y, ost, smoothing=0.1, act_dtype=TDT[dtype])
         lo = float(o["loss"])
         assert abs(float(loss) - lo) < (3e-3 if dtype == "fp16" else 1e-2) * (1 + i) * max(1.0, lo), (i, float(loss), lo)
         assert _rel(tr.engine.logits, o["logits"]) < (2e-2 if dtype == "fp16" else 8e-2) * (1 + i), i
@@ -330,7 +328,7 @@ def test_catavgmax_dropout_matches_oracle():
     assert dmask.shape == (N, 2 * spec.num_features)
     assert abs(float((dmask > 0).float().mean()) - 0.65) < 0.02
     sd = {k: v.clone() for k, v in sd0.items()}
-    out = GO.train_step(spec, sd, x, y, OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4),
+    out = OT.train_step(spec, sd, x, y, OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4),
                         act_dtype=torch.float16, dropout_mask=dmask)
     assert abs(float(eng.loss) - float(out["loss"])) < 3e-3
     assert _rel(eng.logits, out["logits"]) < 2e-2
@@ -375,8 +373,8 @@ def test_catavgmax_model_protocol():
     v = validate(model, batches, torch.nn.CrossEntropyLoss(), args)
     sd = {k: t.clone() for k, t in sd0.items()}
     ost = OT.OptState(kind="sgd", lr=0.001, momentum=0.9, weight_decay=1e-4)
-    losses = [float(GO.train_step(spec, sd, x.cpu(), y.cpu(), ost, act_dtype=torch.float16)["loss"]) for x, y in batches]
-    vl = [float(GO.validate_step(spec, sd, x.cpu(), y.cpu(), act_dtype=torch.float16)["loss"]) for x, y in batches]
+    losses = [float(OT.train_step(spec, sd, x.cpu(), y.cpu(), ost, act_dtype=torch.float16)["loss"]) for x, y in batches]
+    vl = [float(OT.validate_step(spec, sd, x.cpu(), y.cpu(), act_dtype=torch.float16)["loss"]) for x, y in batches]
     assert abs(m["loss"] - sum(losses) / 2) < 2e-3 * sum(losses) / 2, (m, losses)
     assert abs(v["loss"] - sum(vl) / 2) < 5e-3 * sum(vl) / 2, (v, vl)
     ema = ModelEma(model, decay=0.9)

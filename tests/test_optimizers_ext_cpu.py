@@ -1,4 +1,4 @@
-"""radam / adadelta / rmsprop / novograd / nvnovograd without a GPU: the CPU restatement (tests/optim_ext_oracle.py) against
+"""radam / adadelta / rmsprop / novograd / nvnovograd without a GPU: the CPU restatement (oracle/train.py) against
 the fixtures minted from the unmodified reference (tools/mint_optimizer_goldens.py), the factory's names, groups and decay
 rules on the native optimizer, and the C-ABI launches of each kind's update phase on plan-only engines of every shipped
 configuration."""
@@ -9,7 +9,6 @@ from types import SimpleNamespace
 import pytest
 import torch
 
-import optim_ext_oracle as OX
 import plan_launches as PL
 import update_phase as UP
 from deepfake_detection_b200 import _lib
@@ -19,7 +18,7 @@ from oracle import train as OT
 from oracle.weights import synth_batch, synth_state
 
 RTOL = 2e-4
-KINDS = OX.KINDS
+KINDS = OT.EXT_KINDS
 STEP_KERNEL = {"radam": "dfd_radam_step", "adadelta": "dfd_adadelta_step", "rmsprop": "dfd_rmsprop_step",
                "novograd": "dfd_novograd_step", "nvnovograd": "dfd_nvnovograd_step"}
 
@@ -39,7 +38,7 @@ def _toy_grads(step, gen):
 def _run_oracle(r):
     kind = r["kind"]
     wd = r["weight_decay"] / r["lr"] if kind == "radam" else r["weight_decay"]
-    opt = OX.OptState(kind, lr=r["lr"], momentum=r["momentum"], weight_decay=wd, eps=r["eps"],
+    opt = OT.OptState(kind, lr=r["lr"], momentum=r["momentum"], weight_decay=wd, eps=r["eps"],
                       single_group=not r["filter_bias_and_bn"])
     params = _toy()
     gen = torch.Generator().manual_seed(11)
@@ -47,7 +46,7 @@ def _run_oracle(r):
         # group 0 = [bias] (no decay), group 1 = [w, k]; one group when the factory did not split
         by_name = {"bias": lrs[0], "w": lrs[-1], "k": lrs[-1]}
         opt.lr, opt.lr_nodecay = lrs[-1], lrs[0]
-        OX.optimizer_step(opt, params, _toy_grads(step, gen), lrs=by_name)
+        OT.optimizer_step(opt, params, _toy_grads(step, gen), lrs=by_name)
         yield step, params, opt
 
 
@@ -87,10 +86,10 @@ def test_oracle_train_steps_match_reference(case, golden_dir):
     spec = get_spec(rec["arch"], num_classes=rec["num_classes"])
     sd = synth_state(spec, seed=rec["weight_seed"])
     wd = rec["weight_decay"] / rec["lr"] if rec["opt"] == "radam" else rec["weight_decay"]
-    opt = OX.OptState(rec["opt"], lr=rec["lr"], momentum=rec["momentum"], weight_decay=wd, eps=1e-8)
+    opt = OT.OptState(rec["opt"], lr=rec["lr"], momentum=rec["momentum"], weight_decay=wd, eps=1e-8)
     for i, st in enumerate(rec["steps"]):
         x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=1234 + i, num_classes=rec["num_classes"])
-        out = OX.train_step(spec, sd, x, y, opt)
+        out = OT.train_step(spec, sd, x, y, opt)
         assert float(out["loss"]) == pytest.approx(st["loss"], rel=1e-4)
         rt = RTOL * (1 if i == 0 else 25)
         gfloor = 1e-5 * max(v["norm"] / max(out["grads"][k].numel(), 1) ** 0.5 for k, v in st["grads"].items())
@@ -252,11 +251,11 @@ def test_existing_kinds_launch_as_before(monkeypatch):
 
 
 def test_oracle_keeps_the_original_kinds():
-    """optim_ext_oracle.optimizer_step hands the four original kinds to oracle.train unchanged"""
+    """the four original kinds take a per-tensor lr as the new kinds do: the same lr for every tensor is the plain step"""
     params = _toy()
     ref = {k: v.clone() for k, v in params.items()}
     g = _toy_grads(1, torch.Generator().manual_seed(1))
-    OX.optimizer_step(OT.OptState(kind="adamw", lr=1e-2, weight_decay=1.0), params, g)
+    OT.optimizer_step(OT.OptState(kind="adamw", lr=1e-2, weight_decay=1.0), params, g, lrs={k: 1e-2 for k in params})
     OT.optimizer_step(OT.OptState(kind="adamw", lr=1e-2, weight_decay=1.0), ref, g)
     assert all(torch.equal(params[k], ref[k]) for k in params)
 

@@ -4,7 +4,7 @@
   wiring (tests/update_phase.py), in bf16 and in fp16 with loss scaling, over three update phases against an fp64
   restatement with first-order rounding-error bounds; the middle fp16 step overflows and must change nothing;
 - the per-tensor sums of squares against fp64, bit-identical across runs;
-- captured Trainer steps against tests/optim_ext_oracle.py and against the reference's step fixtures;
+- captured Trainer steps against oracle/train.py and against the reference's step fixtures;
 - one captured graph across a per-step lr schedule; state_dict round trips with torch's classes and between native
   optimizers; the runner.
 """
@@ -16,17 +16,17 @@ from types import SimpleNamespace
 import pytest
 import torch
 
-import optim_ext_oracle as OX
 import update_phase as UP
 from deepfake_detection_b200 import _lib
 from deepfake_detection_b200.arch import get_spec, param_entries
 from deepfake_detection_b200.engine import _ptr
+from oracle import train as OT
 from oracle.weights import synth_batch, synth_state
 
 pytestmark = pytest.mark.gpu
 
 TAGS = list(UP.GPU_BATCH)
-KINDS = OX.KINDS
+KINDS = OT.EXT_KINDS
 TDT = {"bf16": torch.bfloat16, "fp16": torch.float16}
 U = 2.0 ** -24
 
@@ -322,11 +322,11 @@ def test_captured_trainer_against_oracle(kind):
     tr = Trainer("efficientnet_b0", 16, 96, 96, dtype="fp16", opt=kind, lr=lr, weight_decay=1e-4, opt_eps=1e-3, use_graph=True)
     tr.load_state_dict(sd0)
     sd = {k: v.clone() for k, v in sd0.items()}
-    ost = OX.OptState(kind, lr=lr, weight_decay=1e-4 / lr if kind == "radam" else 1e-4, eps=1e-3)
+    ost = OT.OptState(kind, lr=lr, weight_decay=1e-4 / lr if kind == "radam" else 1e-4, eps=1e-3)
     for i in range(2):
         x, y = synth_batch(16, 3, 96, 96, seed=1234 + i)
         loss, _ = tr.train_step(x.cuda(), y.cuda())
-        o = OX.train_step(spec, sd, x, y, ost, act_dtype=torch.float16)
+        o = OT.train_step(spec, sd, x, y, ost, act_dtype=torch.float16)
         assert abs(float(loss) - float(o["loss"])) < 3e-3 * (1 + i) * max(1.0, float(o["loss"])), (i, float(loss))
     torch.cuda.synchronize()
     assert tr.n_captures == 1

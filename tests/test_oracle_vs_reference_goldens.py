@@ -72,6 +72,41 @@ def test_train_steps_match_reference(case, golden_dir):
     assert torch.allclose(ev["logits"], ref, rtol=5e-3, atol=5e-3 * float(ref.abs().max()))
 
 
+# one fixture per option the default EfficientNet / ResNet-18/50 cases above do not reach: a selectable global pool, TF "SAME"
+# padding with BatchNorm eps 1e-3, the ResNet-D stem and shortcut, the SE-ResNet blocks and stem pool, Xception
+FAMILY_CASES = ["step_resnet18_gp_avgmax", "step_efficientnet_b0_gp_max", "step_efficientnet_b0_k5_gp_catavgmax_ls",
+                "step_tf_efficientnet_b0_64x96", "step_resnet50d", "step_seresnet18_70x72", "step_xception_64x80"]
+
+
+@pytest.mark.parametrize("case", FAMILY_CASES)
+def test_generic_steps_match_family_fixtures(case, golden_dir):
+    """oracle.train.train_step / validate_step read every field of the spec they are given: each family's fixture through the
+    generic entry points, at the tolerances of that family's CPU test"""
+    rec = json.load(open(os.path.join(golden_dir, case + ".json")))
+    K = rec["num_classes"]
+    torch.set_num_threads(8)
+    spec = get_spec(rec["arch"], num_classes=K, global_pool=rec.get("global_pool", "avg"))
+    sd = synth_state(spec, seed=rec["weight_seed"])
+    opt = OT.OptState(kind=rec["opt"], lr=rec["lr"], momentum=rec["momentum"], weight_decay=rec["weight_decay"], eps=1e-8)
+    for i, st in enumerate(rec["steps"]):
+        x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=1234 + i, soft=rec["soft"], num_classes=K)
+        out = OT.train_step(spec, sd, x, y, opt, smoothing=rec["smoothing"])
+        _check_summ(out["logits"], st["logits"], "logits step %d" % i, rtol=1e-3)
+        assert float(out["loss"]) == pytest.approx(st["loss"], rel=1e-4)
+        assert float(out["prec1"]) == pytest.approx(st["prec1"], abs=1e-3)
+        rt = RTOL * (1 if i == 0 else 25)
+        gfloor = 1e-5 * max(v["norm"] / max(out["grads"][k].numel(), 1) ** 0.5 for k, v in st["grads"].items())
+        for k, s in st["grads"].items():
+            _check_summ(out["grads"][k], s, "grad %s step %d" % (k, i), rt, floor=gfloor)
+        for k, s in st["params"].items():
+            _check_summ(sd[k], s, "param %s step %d" % (k, i), rt)
+        for k, s in st["buffers"].items():
+            _check_summ(sd[k].float(), s, "buffer %s step %d" % (k, i), rt)
+    x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=999, num_classes=K)
+    ev = OT.validate_step(spec, sd, x, y)
+    _check_summ(ev["logits"], rec["eval"]["logits"], "eval logits", rtol=5e-3)
+
+
 def test_optimizers_match_reference(golden_dir):
     rec = json.load(open(os.path.join(golden_dir, "optimizers.json")))
     for name, r in rec.items():

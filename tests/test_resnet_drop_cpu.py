@@ -1,6 +1,6 @@
 """CPU: ResNet DropBlock / drop path / dropout.
 
-The drop oracle (tests/resnet_drop_oracle.py) is oracle.train bit for bit when no mask is given, reproduces the reference's
+The oracle's drop path (oracle.train with masks) is its plain step bit for bit when the masks are empty, reproduces the reference's
 drop_block_2d exactly (including the scrambled valid region of non-square maps and negative gamma), and is held to train
 steps minted from the unmodified reference with its recorded masks. The plan-only engines: all rates 0 is today's plan;
 rates > 0 add the mask generators and switch exactly the DropBlock sites and block tails to the masked kernels; the shapes on
@@ -16,10 +16,9 @@ import torch
 
 from deepfake_detection_b200.arch import get_spec, param_entries
 from deepfake_detection_b200.engine import Engine
+from oracle import formulas as OF
 from oracle import train as OT
 from oracle.weights import synth_batch, synth_state
-
-import resnet_drop_oracle as RO
 
 RATES = dict(drop_rate=0.2, drop_path_rate=0.1, drop_block_rate=0.2)
 NEW_OPS = {"dfd_drop_block_masks_train", "dfd_memset_async_train", "dfd_rng_masks_train", "dfd_rng_tick_train",
@@ -49,7 +48,7 @@ def test_no_mask_is_oracle_train_bit_for_bit(arch):
         a = {k: v.clone() for k, v in sd0.items()}
         b = {k: v.clone() for k, v in sd0.items()}
         oa = OT.train_step(spec, a, x, y, OT.OptState(kind="sgd", lr=0.01), act_dtype=adt)
-        ob = RO.train_step(spec, b, x, y, OT.OptState(kind="sgd", lr=0.01), act_dtype=adt)
+        ob = OT.train_step(spec, b, x, y, OT.OptState(kind="sgd", lr=0.01), act_dtype=adt, drop_block={}, drop_masks={})
         assert torch.equal(oa["logits"], ob["logits"]) and torch.equal(oa["loss"], ob["loss"])
         assert all(torch.equal(oa["grads"][n], ob["grads"][n]) for n in oa["grads"])
         assert all(torch.equal(a[n], b[n]) for n in a)
@@ -62,16 +61,16 @@ def test_drop_block_formulas_reproduced_exactly(golden_dir):
         H, W = c["H"], c["W"]
         shape = rec["shape"] + [H, W]
         x, u, out = _f32(c["x"]).view(shape), _f32(c["noise"]).view(shape), _f32(c["out"]).view(shape)
-        gamma, cb = RO.drop_block_gamma(H, W, c["drop_prob"], c["gamma_scale"], c["block_size"])
-        m = RO.block_from_seeds(RO.seeds_from_noise(u, gamma, cb), cb)
-        assert torch.equal(RO.drop_block_apply(x, m), out), (H, W, c["gamma_scale"])
+        gamma, cb = OF.drop_block_gamma(H, W, c["drop_prob"], c["gamma_scale"], c["block_size"])
+        m = OF.block_from_seeds(OF.seeds_from_noise(u, gamma, cb), cb)
+        assert torch.equal(OF.drop_block_apply(x, m), out), (H, W, c["gamma_scale"])
         n_neg += gamma < 0
         n_dropped += bool((m == 0).any())
         if gamma < 0:
             assert torch.equal(out, x * (m.numel() / (m.sum() + 1e-7)))       # nothing dropped
     assert n_neg == 2 and n_dropped >= 4          # 5 x 7 at both gamma scales
     # the non-square valid region is the reference's scrambled one, not the centred rectangle
-    v = RO.valid_block(10, 14, 7)[0, 0]
+    v = OF.valid_block(10, 14, 7)[0, 0]
     centred = torch.zeros(10, 14)
     centred[3:7, 3:11] = 1
     assert not torch.equal(v, centred) and int(v.sum()) == int(centred.sum())
@@ -101,11 +100,11 @@ def test_drop_oracle_matches_reference_steps(case, golden_dir):
         for name, d in st["drop_block"].items():
             H, W = d["shape"][-2:]
             gs = 0.25 if name.startswith("layer3") else 1.0
-            _, cb = RO.drop_block_gamma(H, W, rec["drop_block_rate"], gs)
-            db[name] = RO.block_from_seeds(_zeros_mask(d["shape"], d["zeros"]), cb)
+            _, cb = OF.drop_block_gamma(H, W, rec["drop_block_rate"], gs)
+            db[name] = OF.block_from_seeds(_zeros_mask(d["shape"], d["zeros"]), cb)
         dp = {k: torch.tensor(v) for k, v in st["drop_masks"].items()}
         dm = _zeros_mask(st["dropout_shape"], st["dropout_zeros"]) / (1.0 - rec["drop_rate"])
-        out = RO.train_step(spec, sd, x, y, ost, drop_block=db, drop_masks=dp, dropout_mask=dm)
+        out = OT.train_step(spec, sd, x, y, ost, drop_block=db, drop_masks=dp, dropout_mask=dm)
         assert abs(float(out["loss"]) - st["loss"]) < (1e-4 if i == 0 else 2e-2) * max(1.0, abs(st["loss"])), (i, float(out["loss"]))
         if i == 0:
             _check_summ(out["logits"], st["logits"], 1e-3, "logits")

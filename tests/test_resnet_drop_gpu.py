@@ -4,7 +4,7 @@ Masks: dfd_drop_block_masks against the reference expression recomputed in torch
 its kept count, the seed-drop rate inside the valid region, and fresh masks every step and every graph replay. Kernels: the
 masked BN + ReLU forward, block tail and the two backward reductions against fp64 torch on the same rounded operands, in
 bf16 and fp16, with bit-identical reruns. End to end: one training step of ResNet-18 / ResNet-50 with all three rates
-against tests/resnet_drop_oracle.py given the engine's masks (the statements and thresholds of
+against oracle/model.py given the engine's masks (the statements and thresholds of
 test_engine_gpu.py::test_resnet_train_step_parity), and the runner protocol with ModelEma."""
 from types import SimpleNamespace
 
@@ -13,8 +13,7 @@ import torch
 
 from deepfake_detection_b200 import _lib
 from deepfake_detection_b200.engine_resnet import drop_block_desc
-
-import resnet_drop_oracle as RO
+from oracle import formulas as OF
 
 pytestmark = pytest.mark.gpu
 
@@ -41,7 +40,7 @@ def _draw(shapes, step, noise=True):
     kept = torch.zeros(len(shapes), dtype=torch.int64, device="cuda")
     out, raw = [], b""
     for i, (N, H, W, C, rate, gs) in enumerate(shapes):
-        gamma, cb = RO.drop_block_gamma(H, W, rate, gs)
+        gamma, cb = OF.drop_block_gamma(H, W, rate, gs)
         m = torch.full((N, H, W, C), 7, dtype=torch.uint8, device="cuda")
         u = torch.full((N, H, W, C), -1.0, device="cuda") if noise else None
         raw += drop_block_desc(_P(m), _P(u), _P(kept) + 8 * i, gamma, N, H, W, C, cb, 100 + i)
@@ -64,12 +63,12 @@ def test_drop_block_masks_match_reference_expression():
     for (N, H, W, C, rate, gs), (m, u, gamma, cb), k, (m2, _, _, _) in zip(SITES, out, kept, out2):
         un = u.permute(0, 3, 1, 2).cpu()
         assert float(un.min()) >= 0.0 and float(un.max()) < 1.0
-        seeds = RO.seeds_from_noise(un, gamma, cb)
-        ref = RO.block_from_seeds(seeds, cb)
+        seeds = OF.seeds_from_noise(un, gamma, cb)
+        ref = OF.block_from_seeds(seeds, cb)
         got = m.permute(0, 3, 1, 2).cpu().float()
         assert torch.equal(got, ref), (H, W, C, gamma)
         assert int(k) == int(m.sum())
-        valid = RO.valid_block(H, W, cb).expand_as(seeds).bool()
+        valid = OF.valid_block(H, W, cb).expand_as(seeds).bool()
         dropped = seeds == 0
         assert not bool(dropped[~valid].any())
         n = int(valid.sum())
@@ -214,14 +213,14 @@ def test_train_step_with_drop_matches_oracle(arch, batch, res, dtype):
     opt = ArenaOptimizer(eng, opt="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4)
     x, y = synth_batch(batch, 3, res, res, seed=1234)
     EC.engine_step(eng, opt, x.cuda(), y.cuda())
-    db, dp, dm = RO.engine_masks(eng)
+    db, dp, dm = EC.engine_masks(eng)
     assert len(db) == (8 if arch == "resnet18" else 27) and len(dp) == len(spec.blocks)
     assert all(int(k) == int(m.sum()) for m, k in eng.drop_block_masks.values())
     pn = [n for n, _, _ in param_entries(spec)]
     rep = {}
     for key, adt in (("emul", TDT[dtype]), ("fp32", None)):
         sd = {k: v.clone() for k, v in sd0.items()}
-        out = RO.train_step(spec, sd, x, y, OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4), act_dtype=adt,
+        out = OT.train_step(spec, sd, x, y, OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4), act_dtype=adt,
                             drop_block=db, drop_masks=dp, dropout_mask=dm)
         tot = torch.cat([out["grads"][n].flatten() for n in pn])
         rep[key] = dict(logits=out["logits"], loss=float(out["loss"]), grads=tot, sd=sd)

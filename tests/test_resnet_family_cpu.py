@@ -1,5 +1,5 @@
 """Host logic of the dense ResNet family (resnet26/34/101/152, tv_resnet34/50, wide_resnet50_2/101_2, resnet26d, resnet50d),
-no GPU: the specs against the reference's state keys, the oracle (tests/resnet_family_oracle.py) against the reference's train
+no GPU: the specs against the reference's state keys, the oracle (oracle/model.py) against the reference's train
 steps, the model factory's registry, default_cfg and init, and the plans. Fixtures: tools/mint_resnet_family_goldens.py."""
 import hashlib
 import json
@@ -9,12 +9,11 @@ from collections import Counter
 import pytest
 import torch
 
-import resnet_family_oracle as RO
 from deepfake_detection_b200 import _lib
 from deepfake_detection_b200.arch import RESNET_ARCHS, SUPPORTED_ARCHS, get_spec, param_entries, state_entries
 from deepfake_detection_b200.engine import Engine
 from oracle import train as OT
-from oracle.weights import synth_batch, synth_state
+from oracle.weights import synth_batch, synth_state, tame_state
 from test_tf_efficientnet_cpu import RTOL, _check_summ
 
 STEP_CASES = ["step_resnet26d_72x88", "step_resnet50d", "step_resnet34", "step_wide_resnet50_2", "step_resnet101",
@@ -57,18 +56,18 @@ def test_specs_match_reference_state_keys(key, golden_dir):
 
 @pytest.mark.parametrize("case", STEP_CASES)
 def test_oracle_matches_reference_steps(case, golden_dir):
-    """tests/resnet_family_oracle.py against the reference's own train steps and eval, at the tolerances of
+    """oracle/model.py against the reference's own train steps and eval, at the tolerances of
     test_oracle_vs_reference_goldens.py / test_tf_efficientnet_cpu.py"""
     rec = json.load(open(os.path.join(golden_dir, case + ".json")))
     torch.set_num_threads(8)
     spec = get_spec(rec["arch"], num_classes=rec["num_classes"])
     sd = synth_state(spec, seed=rec["weight_seed"])
     if "tame" in rec:
-        sd = RO.tame_state(spec, sd, rec["tame"])
+        sd = tame_state(spec, sd, rec["tame"])
     opt = OT.OptState(kind=rec["opt"], lr=rec["lr"], momentum=rec["momentum"], weight_decay=rec["weight_decay"], eps=1e-8)
     for i, st in enumerate(rec["steps"]):
         x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=1234 + i)
-        out = RO.train_step(spec, sd, x, y, opt)
+        out = OT.train_step(spec, sd, x, y, opt)
         _check_summ(out["logits"], st["logits"], "logits step %d" % i, rtol=1e-3)
         assert float(out["loss"]) == pytest.approx(st["loss"], rel=1e-4)
         assert float(out["prec1"]) == pytest.approx(st["prec1"], abs=1e-3)
@@ -81,7 +80,7 @@ def test_oracle_matches_reference_steps(case, golden_dir):
         for k, s in st["buffers"].items():
             _check_summ(sd[k].float(), s, "buffer %s step %d" % (k, i), rt)
     x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=999)
-    ev = RO.validate_step(spec, sd, x, y)
+    ev = OT.validate_step(spec, sd, x, y)
     _check_summ(ev["logits"], rec["eval"]["logits"], "eval logits", rtol=5e-3)
 
 

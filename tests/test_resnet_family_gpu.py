@@ -2,7 +2,7 @@
 
   * dfd_avgpool2_fwd / dfd_avgpool2_bwd_add against fp64 F.avg_pool2d(2, 2, ceil_mode=True, count_include_pad=False) and its
     autograd, and bit for bit against a torch emulation of their one-rounding formulas, at even and odd extents, bf16 / fp16;
-  * whole train steps of resnet26d, resnet34, wide_resnet50_2 and resnet101 against the oracle (tests/resnet_family_oracle.py)
+  * whole train steps of resnet26d, resnet34, wide_resnet50_2 and resnet101 against the oracle (oracle/model.py)
     and the reference's step fixtures; resnet101 and resnet50d at batch 32, 224x224, from the reference init against the fp32
     oracle; the runner's train_epoch over create_model("resnet101"); resnet50d with DropBlock, drop path and dropout;
   * checkpoints round-trip bit for bit, and two resnet50d engines agree bit for bit.
@@ -144,24 +144,23 @@ def test_steps_match_oracle_and_reference(arch, batch, H, W, fixture, dtype, gol
     the emulation's own distance + a margin), every step's loss against the reference, and the step-0 logits against the
     reference's samples. resnet101 in bf16 is the one case where the emulation itself moves the logits by more than the
     emulation bound (7.4e-2): there that bound is 1.5 x the emulation's distance."""
-    import resnet_family_oracle as RO
     from deepfake_detection_b200.arch import param_entries
     from oracle import train as OT
-    from oracle.weights import synth_batch, synth_state
+    from oracle.weights import synth_batch, synth_state, tame_state
     from deepfake_detection_b200.arch import get_spec
     rec = json.load(open(os.path.join(golden_dir, fixture + ".json")))
     assert (rec["arch"], rec["batch"], rec["H"], rec["W"]) == (arch, batch, H, W)
     spec = get_spec(arch)
-    sd0 = RO.tame_state(spec, synth_state(spec, seed=rec["weight_seed"]), rec["tame"])
+    sd0 = tame_state(spec, synth_state(spec, seed=rec["weight_seed"]), rec["tame"])
     spec, sd0, tr, runs = _run_steps(arch, batch, H, W, dtype, len(rec["steps"]), sd0)
     sd = {k: v.clone() for k, v in sd0.items()}
     ost = OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4)
     e = tr.engine
     for i, (r, st) in enumerate(zip(runs, rec["steps"])):
         x, y = synth_batch(batch, 3, H, W, seed=1234 + i)
-        o = RO.train_step(spec, sd, x, y, ost, act_dtype=TDT[dtype])
+        o = OT.train_step(spec, sd, x, y, ost, act_dtype=TDT[dtype])
         if i == 0:
-            o32 = RO.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None)
+            o32 = OT.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None)
             yard_logits = _rel(o["logits"], o32["logits"])
             bound = max(2e-2 if dtype == "fp16" else 6e-2, 1.5 * yard_logits)
             assert _rel(r["logits"], o["logits"]) < bound, (_rel(r["logits"], o["logits"]), yard_logits)
@@ -186,7 +185,6 @@ _ORACLE = {}
 
 def _oracle_ref_init(arch, batch, res):
     """fp32 oracle step from the reference's own initialisers (cached: one CPU pass serves both dtypes)"""
-    import resnet_family_oracle as RO
     from deepfake_detection_b200.arch import get_spec, param_entries
     from deepfake_detection_b200.models import init_state_dict
     from oracle import train as OT
@@ -197,7 +195,7 @@ def _oracle_ref_init(arch, batch, res):
         spec = get_spec(arch)
         sd = {k: v.clone() for k, v in init_state_dict(spec, seed=11).items()}
         x, y = synth_batch(batch, 3, res, res, seed=1234)
-        out = RO.train_step(spec, sd, x, y, OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4))
+        out = OT.train_step(spec, sd, x, y, OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4))
         _ORACLE[key] = dict(spec=spec, sd=sd, x=x, y=y, logits=out["logits"], loss=float(out["loss"]),
                             pnames=[n for n, _, _ in param_entries(spec)])
     return _ORACLE[key]
@@ -239,7 +237,6 @@ def test_runner_train_epoch_resnet101_matches_oracle():
     """the runner's default model: train_epoch's loop body (train.py:610-649) over create_model("resnet101") and
     create_optimizer for two steps, against the oracle's two steps. Synthetic weights with the residual branches damped
     (engine_checks.run_parity(tame=True)); the weight updates are held to the yardstick of the oracle's own bf16 emulation."""
-    import resnet_family_oracle as RO
     from deepfake_detection_b200.arch import get_spec, param_entries
     from deepfake_detection_b200.models import create_model
     from deepfake_detection_b200.optim import create_optimizer
@@ -267,7 +264,7 @@ def test_runner_train_epoch_resnet101_matches_oracle():
     for key, adt in (("emul", torch.bfloat16), ("fp32", None)):
         sd = {k: v.clone() for k, v in sd0.items()}
         ost = OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4)
-        losses = [float(RO.train_step(spec, sd, x, y, ost, act_dtype=adt)["loss"]) for x, y in data]
+        losses = [float(OT.train_step(spec, sd, x, y, ost, act_dtype=adt)["loss"]) for x, y in data]
         res[key] = (sum(losses) / 2, torch.cat([(sd[n] - sd0[n]).flatten() for n in pn]))
     got = model.state_dict()
     dn = torch.cat([(got[n].cpu() - sd0[n]).flatten() for n in pn])
@@ -280,8 +277,7 @@ def test_runner_train_epoch_resnet101_matches_oracle():
 def test_resnet50d_with_drop_matches_oracle():
     """one Trainer step of resnet50d at 160x160 with all three rates, against the oracle fed the engine's masks (emulation and
     fp32), with tests/test_resnet_drop_gpu.py's statements"""
-    import resnet_drop_oracle as RD
-    import resnet_family_oracle as RO
+    from engine_checks import engine_masks
     from deepfake_detection_b200.arch import get_spec, param_entries
     from deepfake_detection_b200.trainer import Trainer
     from oracle import train as OT
@@ -298,14 +294,14 @@ def test_resnet50d_with_drop_matches_oracle():
     x, y = synth_batch(batch, 3, res, res, seed=1234)
     tr.train_step(x.cuda(), y.cuda())
     torch.cuda.synchronize()
-    db, dp, dm = RD.engine_masks(eng)
+    db, dp, dm = engine_masks(eng)
     assert len(db) == 27 and len(dp) == len(spec.blocks) and dm is not None
     assert any(float(m.sum()) < m.numel() for m in db.values())
     pn = [n for n, _, _ in param_entries(spec)]
     rep = {}
     for key, adt in (("emul", TDT[dtype]), ("fp32", None)):
         sd = {k: v.clone() for k, v in sd0.items()}
-        out = RO.train_step(spec, sd, x, y, None, act_dtype=adt, drop_block=db, drop_masks=dp, dropout_mask=dm)
+        out = OT.train_step(spec, sd, x, y, None, act_dtype=adt, drop_block=db, drop_masks=dp, dropout_mask=dm)
         rep[key] = dict(logits=out["logits"], loss=float(out["loss"]), grads=torch.cat([out["grads"][n].flatten() for n in pn]))
     gn = torch.cat([eng.grad_view(n).flatten().cpu() for n in pn])
     em, fp = rep["emul"], rep["fp32"]

@@ -1,4 +1,4 @@
-"""Host logic of the SE-ResNets, no GPU: the specs against the reference's state keys, the oracle (tests/senet_oracle.py) against
+"""Host logic of the SE-ResNets, no GPU: the specs against the reference's state keys, the oracle (oracle/model.py) against
 the reference's train steps, the model factory (default_cfg, init, the keyword arguments the reference refuses or drops) and the
 plans. Fixtures: tools/mint_senet_goldens.py."""
 import json
@@ -9,13 +9,12 @@ from collections import Counter
 import pytest
 import torch
 
-import senet_oracle as SO
 from deepfake_detection_b200 import _lib
 from deepfake_detection_b200.arch import (RESNET_ARCHS, SENET_ARCHS, SUPPORTED_ARCHS, get_spec, param_entries, state_entries,
                                           stem_pool_out)
 from deepfake_detection_b200.engine import Engine
 from oracle import train as OT
-from oracle.weights import synth_batch, synth_state
+from oracle.weights import synth_batch, synth_state, tame_state
 from test_resnet_family_cpu import _digest
 from test_tf_efficientnet_cpu import RTOL, _check_summ
 
@@ -64,18 +63,18 @@ def test_se_widths_and_strides():
 
 @pytest.mark.parametrize("case", STEP_CASES)
 def test_oracle_matches_reference_steps(case, golden_dir):
-    """tests/senet_oracle.py against the reference's own train steps and eval, at the ResNet family's fp32 tolerances"""
+    """oracle/model.py against the reference's own train steps and eval, at the ResNet family's fp32 tolerances"""
     rec = json.load(open(os.path.join(golden_dir, case + ".json")))
     assert rec["drop_rate"] == 0.0
     torch.set_num_threads(8)
     spec = get_spec(rec["arch"], num_classes=rec["num_classes"])
     sd = synth_state(spec, seed=rec["weight_seed"])
     if "tame" in rec:
-        sd = SO.tame_state(spec, sd, rec["tame"])
+        sd = tame_state(spec, sd, rec["tame"])
     opt = OT.OptState(kind=rec["opt"], lr=rec["lr"], momentum=rec["momentum"], weight_decay=rec["weight_decay"], eps=1e-8)
     for i, st in enumerate(rec["steps"]):
         x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=1234 + i)
-        out = SO.train_step(spec, sd, x, y, opt)
+        out = OT.train_step(spec, sd, x, y, opt)
         _check_summ(out["logits"], st["logits"], "logits step %d" % i, rtol=1e-3)
         assert float(out["loss"]) == pytest.approx(st["loss"], rel=1e-4)
         assert float(out["prec1"]) == pytest.approx(st["prec1"], abs=1e-3)
@@ -88,7 +87,7 @@ def test_oracle_matches_reference_steps(case, golden_dir):
         for k, s in st["buffers"].items():
             _check_summ(sd[k].float(), s, "buffer %s step %d" % (k, i), rt)
     x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=999)
-    ev = SO.validate_step(spec, sd, x, y)
+    ev = OT.validate_step(spec, sd, x, y)
     _check_summ(ev["logits"], rec["eval"]["logits"], "eval logits", rtol=5e-3)
 
 

@@ -4,7 +4,7 @@
     extents with forced ties; dfd_pool_se_relu against the SEModule formula in fp64 at every (C, Cse, HW) of seresnet18 / 50,
     batch 1 (chunked) and 64; dfd_relu_se_bwd_reduce + dfd_act_bwd + the BatchNorm backward + dfd_se_fc_wgrad against fp64
     autograd of relu(se(bn(y)) + res); bf16 and fp16;
-  * whole train steps against the oracle (tests/senet_oracle.py) and the reference's tamed step fixtures; seresnet50 at batch
+  * whole train steps against the oracle (oracle/model.py) and the reference's tamed step fixtures; seresnet50 at batch
     32, 224x224, from the reference init against the fp32 oracle; fp16 eval at batch 1; max / avgmax pooling; the default
     dropout; checkpoints and two engines bit for bit; the runner's train_epoch with an EMA update.
 No test here reads the reference tree: the fixtures under tests/golden/ came from tools/mint_senet_goldens.py.
@@ -205,23 +205,22 @@ STEP_CASES = [("seresnet18", 8, 70, 72, "step_seresnet18_tame_70x72"), ("seresne
 @pytest.mark.parametrize("arch,batch,H,W,fixture", STEP_CASES, ids=[c[0] for c in STEP_CASES])
 def test_steps_match_oracle_and_reference(arch, batch, H, W, fixture, dtype, golden_dir):
     """tests/test_resnet_family_gpu.py::test_steps_match_oracle_and_reference's statements over the tamed SE-ResNet fixtures"""
-    import senet_oracle as SO
     from deepfake_detection_b200.arch import get_spec, param_entries
     from oracle import train as OT
-    from oracle.weights import synth_batch, synth_state
+    from oracle.weights import synth_batch, synth_state, tame_state
     rec = json.load(open(os.path.join(golden_dir, fixture + ".json")))
     assert (rec["arch"], rec["batch"], rec["H"], rec["W"]) == (arch, batch, H, W)
     spec = get_spec(arch)
-    sd0 = SO.tame_state(spec, synth_state(spec, seed=rec["weight_seed"]), rec["tame"])
+    sd0 = tame_state(spec, synth_state(spec, seed=rec["weight_seed"]), rec["tame"])
     tr, runs = _run_steps(arch, batch, H, W, dtype, len(rec["steps"]), sd0)
     sd = {k: v.clone() for k, v in sd0.items()}
     ost = OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4)
     e = tr.engine
     for i, (r, st) in enumerate(zip(runs, rec["steps"])):
         x, y = synth_batch(batch, 3, H, W, seed=1234 + i)
-        o = SO.train_step(spec, sd, x, y, ost, act_dtype=TDT[dtype])
+        o = OT.train_step(spec, sd, x, y, ost, act_dtype=TDT[dtype])
         if i == 0:
-            o32 = SO.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None)
+            o32 = OT.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None)
             yard_logits = _rel(o["logits"], o32["logits"])
             bound = max(2e-2 if dtype == "fp16" else 6e-2, 1.5 * yard_logits)
             assert _rel(r["logits"], o["logits"]) < bound, (_rel(r["logits"], o["logits"]), yard_logits)
@@ -245,7 +244,6 @@ def test_seresnet50_batch32_224_reference_init(dtype, record_property):
     """seresnet50 at batch 32, 224x224, from the reference's initialisers: loss and updated weights within 1e-2 of the fp32
     oracle, or - where the oracle's own 16-bit emulation is already further than that from fp32 - within 1.5 x that distance
     (yard) + 1e-2. Which statement holds is recorded."""
-    import senet_oracle as SO
     from deepfake_detection_b200.arch import get_spec, param_entries
     from deepfake_detection_b200.models import init_state_dict
     from deepfake_detection_b200.trainer import Trainer
@@ -259,7 +257,7 @@ def test_seresnet50_batch32_224_reference_init(dtype, record_property):
     ref = {}
     for key, adt in (("fp32", None), ("emul", TDT[dtype])):
         sd = {k: v.clone() for k, v in w0.items()}
-        out = SO.train_step(spec, sd, x, y, OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4), act_dtype=adt)
+        out = OT.train_step(spec, sd, x, y, OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4), act_dtype=adt)
         ref[key] = dict(loss=float(out["loss"]), sd=sd)
     tr = Trainer("seresnet50", 32, 224, 224, dtype=dtype, opt="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4, use_graph=False)
     eng = tr.engine
@@ -287,7 +285,7 @@ def test_seresnet50_batch32_224_reference_init(dtype, record_property):
 
 def test_eval_batch1_fp16():
     """the test_img path: eval at batch 1 in fp16 (chunked SE pools) from the reference's initialisers"""
-    import senet_oracle as SO
+    from oracle import train as OT
     from deepfake_detection_b200.arch import get_spec
     from deepfake_detection_b200.models import create_model, init_state_dict
     from oracle.weights import synth_batch
@@ -300,8 +298,8 @@ def test_eval_batch1_fp16():
     with torch.no_grad():
         got = m(x.cuda()).cpu()
         again = m(x.cuda()).cpu()
-    ref = SO.validate_step(spec, sd, x, y)["logits"]
-    emu = SO.validate_step(spec, sd, x, y, act_dtype=torch.float16)["logits"]
+    ref = OT.validate_step(spec, sd, x, y)["logits"]
+    emu = OT.validate_step(spec, sd, x, y, act_dtype=torch.float16)["logits"]
     assert torch.equal(got, again)
     assert _rel(got, emu) < 2e-2 and _rel(got, ref) < 1.5 * _rel(emu, ref) + 2e-2, (_rel(got, emu), _rel(got, ref), _rel(emu, ref))
 
@@ -309,12 +307,12 @@ def test_eval_batch1_fp16():
 @pytest.mark.parametrize("gp", ["max", "avgmax"])
 def test_global_pool_step(gp):
     """--gp max / avgmax: one step of the tamed seresnet18 against the oracle's emulation and fp32"""
-    import senet_oracle as SO
+    from oracle import train as OT
     from deepfake_detection_b200.arch import get_spec, param_entries
     from deepfake_detection_b200.trainer import Trainer
-    from oracle.weights import synth_batch, synth_state
+    from oracle.weights import synth_batch, synth_state, tame_state
     spec = get_spec("seresnet18", global_pool=gp)
-    sd0 = SO.tame_state(spec, synth_state(spec, seed=7))
+    sd0 = tame_state(spec, synth_state(spec, seed=7))
     tr = Trainer("seresnet18", 8, 96, 96, dtype="bf16", opt="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4, global_pool=gp)
     tr.engine.load_state_dict(sd0)
     x, y = synth_batch(8, 3, 96, 96, seed=1234)
@@ -322,8 +320,8 @@ def test_global_pool_step(gp):
     torch.cuda.synchronize()
     e = tr.engine
     pn = [n for n, _, _ in param_entries(spec)]
-    em = SO.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None, act_dtype=torch.bfloat16)
-    fp = SO.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None)
+    em = OT.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None, act_dtype=torch.bfloat16)
+    fp = OT.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None)
     yard_l = _rel(em["logits"], fp["logits"])
     assert _rel(e.logits, fp["logits"]) < 1.5 * yard_l + 1e-2, (_rel(e.logits, fp["logits"]), yard_l)
     gn = torch.cat([e.grad_view(n).flatten().cpu() for n in pn])
@@ -334,12 +332,12 @@ def test_global_pool_step(gp):
 def test_default_dropout_matches_oracle():
     """create_model("seresnet50") trains with SENet's default drop_rate 0.2: the engine draws the mask on the pooled vector, and
     the step matches the oracle fed that mask"""
-    import senet_oracle as SO
+    from oracle import train as OT
     from deepfake_detection_b200.arch import get_spec, param_entries
     from deepfake_detection_b200.models import create_model
-    from oracle.weights import synth_batch, synth_state
+    from oracle.weights import synth_batch, synth_state, tame_state
     spec = get_spec("seresnet50")
-    sd0 = SO.tame_state(spec, synth_state(spec, seed=7))
+    sd0 = tame_state(spec, synth_state(spec, seed=7))
     model = create_model("seresnet50", num_classes=2)
     assert model.drop_rate == 0.2
     model.load_state_dict(sd0)
@@ -353,8 +351,8 @@ def test_default_dropout_matches_oracle():
     keep = mask != 0
     assert 0 < int((~keep).sum()) < mask.numel() and torch.allclose(mask[keep], torch.full_like(mask[keep], 1 / 0.8))
     pn = [n for n, _, _ in param_entries(spec)]
-    em = SO.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None, act_dtype=torch.bfloat16, dropout_mask=mask)
-    fp = SO.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None, dropout_mask=mask)
+    em = OT.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None, act_dtype=torch.bfloat16, dropout_mask=mask)
+    fp = OT.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None, dropout_mask=mask)
     assert _rel(out.detach(), fp["logits"]) < 1.5 * _rel(em["logits"], fp["logits"]) + 1e-2
     gn = torch.cat([e.grad_view(n).flatten().cpu() for n in pn])
     gf, ge = (torch.cat([o["grads"][n].flatten() for n in pn]) for o in (fp, em))
@@ -401,14 +399,13 @@ def test_two_engines_agree_bit_for_bit(arch, batch):
 def test_runner_train_epoch_with_ema():
     """train_epoch's loop body over create_model("seresnet50", drop_rate=0.0) for two steps, against the oracle's two steps
     (tamed synthetic weights); then one EMA update"""
-    import senet_oracle as SO
     from deepfake_detection_b200.arch import get_spec, param_entries
     from deepfake_detection_b200.ema import ModelEma
     from deepfake_detection_b200.models import create_model
     from deepfake_detection_b200.optim import create_optimizer
     from deepfake_detection_b200.runners.train import train_epoch
     from oracle import train as OT
-    from oracle.weights import synth_batch, synth_state
+    from oracle.weights import synth_batch, synth_state, tame_state
 
     class _Loader(list):
         mixup_enabled = False
@@ -417,7 +414,7 @@ def test_runner_train_epoch_with_ema():
                            mixup_off_epoch=0, num_classes=2, smoothing=0.0, distributed=False, world_size=1, local_rank=0,
                            log_interval=1, save_images=False, recovery_interval=0, tta=0, model="seresnet50")
     spec = get_spec("seresnet50")
-    sd0 = SO.tame_state(spec, synth_state(spec, seed=7))
+    sd0 = tame_state(spec, synth_state(spec, seed=7))
     model = create_model("seresnet50", num_classes=2, drop_rate=0.0)
     model.load_state_dict(sd0)
     opt = create_optimizer(args, model)
@@ -430,7 +427,7 @@ def test_runner_train_epoch_with_ema():
     for key, adt in (("emul", torch.bfloat16), ("fp32", None)):
         sd = {k: v.clone() for k, v in sd0.items()}
         ost = OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4)
-        losses = [float(SO.train_step(spec, sd, x, y, ost, act_dtype=adt)["loss"]) for x, y in data]
+        losses = [float(OT.train_step(spec, sd, x, y, ost, act_dtype=adt)["loss"]) for x, y in data]
         res[key] = (sum(losses) / 2, torch.cat([(sd[n] - sd0[n]).flatten() for n in pn]))
     got = model.state_dict()
     dn = torch.cat([(got[n].cpu() - sd0[n]).flatten() for n in pn])

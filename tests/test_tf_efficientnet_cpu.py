@@ -9,7 +9,6 @@ import pytest
 import torch
 
 import tf_same_cases as TC
-import tf_same_oracle as TO
 from deepfake_detection_b200 import _lib
 from deepfake_detection_b200.arch import SUPPORTED_ARCHS, TF_ARCHS, conv_pads, get_spec, param_entries, state_entries
 from deepfake_detection_b200.engine import Engine, base_name
@@ -95,7 +94,7 @@ def test_issue_pad_table_at_default_resolutions():
 
 @pytest.mark.parametrize("case", ["step_tf_efficientnet_b0_64x96", "step_tf_efficientnet_b0_66x96"])
 def test_oracle_matches_reference_steps(case, golden_dir):
-    """tests/tf_same_oracle.py against the reference's own tf_efficientnet_b0 train steps, at the tolerances of
+    """oracle/model.py against the reference's own tf_efficientnet_b0 train steps, at the tolerances of
     test_oracle_vs_reference_goldens.py / test_head_multiclass_cpu.py"""
     rec = json.load(open(os.path.join(golden_dir, case + ".json")))
     torch.set_num_threads(8)
@@ -104,7 +103,7 @@ def test_oracle_matches_reference_steps(case, golden_dir):
     opt = OT.OptState(kind=rec["opt"], lr=rec["lr"], momentum=rec["momentum"], weight_decay=rec["weight_decay"], eps=1e-8)
     for i, st in enumerate(rec["steps"]):
         x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=1234 + i)
-        out = TO.train_step(spec, sd, x, y, opt)
+        out = OT.train_step(spec, sd, x, y, opt)
         _check_summ(out["logits"], st["logits"], "logits step %d" % i, rtol=1e-3)
         assert float(out["loss"]) == pytest.approx(st["loss"], rel=1e-4)
         assert float(out["prec1"]) == pytest.approx(st["prec1"], abs=1e-3)
@@ -117,7 +116,7 @@ def test_oracle_matches_reference_steps(case, golden_dir):
         for k, s in st["buffers"].items():
             _check_summ(sd[k].float(), s, "buffer %s step %d" % (k, i), rt)
     x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=999)
-    ev = TO.validate_step(spec, sd, x, y)
+    ev = OT.validate_step(spec, sd, x, y)
     _check_summ(ev["logits"], rec["eval"]["logits"], "eval logits", rtol=5e-3)
 
 
@@ -125,7 +124,7 @@ def test_oracle_eval_logits_match_reference(golden_dir):
     rec = json.load(open(os.path.join(golden_dir, "tf_eval_b0_224.json")))
     spec = get_spec(rec["arch"])
     x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=rec["input_seed"])
-    ev = TO.validate_step(spec, synth_state(spec, seed=rec["weight_seed"]), x, y)
+    ev = OT.validate_step(spec, synth_state(spec, seed=rec["weight_seed"]), x, y)
     ref = torch.tensor(rec["logits"])
     assert torch.allclose(ev["logits"], ref, rtol=1e-4, atol=1e-5), (ev["logits"], ref)
 

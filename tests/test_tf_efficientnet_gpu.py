@@ -4,7 +4,7 @@
     batch) and the non-square cases, in bf16 and fp16, against fp64 torch (tests/tf_same_checks.py); at symmetric pads the
     new entry points equal the old ones bit for bit;
   * graph-captured tf_efficientnet_b0 Trainer steps (bf16; fp16 with dynamic loss scaling) against the oracle
-    (tests/tf_same_oracle.py) and the reference's step fixtures, identical bits over two runs; one tf_efficientnet_b4 step at
+    (oracle/model.py) and the reference's step fixtures, identical bits over two runs; one tf_efficientnet_b4 step at
     380² against the oracle;
   * the reference's eval logits of tf_efficientnet_b0 at 224², and the runner's train_epoch / validate on a tf model.
 No test here reads the reference tree: the fixtures under tests/golden/ came from tools/mint_tf_goldens.py.
@@ -97,7 +97,6 @@ def _run_steps(arch, batch, H, W, dtype, steps):
 @pytest.mark.parametrize("dtype", ["bf16", "fp16"])
 @pytest.mark.parametrize("H,W", [(64, 96), (66, 96)])
 def test_tf_b0_captured_steps_match_oracle_and_reference(H, W, dtype, golden_dir):
-    import tf_same_oracle as TO
     from deepfake_detection_b200.arch import param_entries
     from oracle import train as OT
     from oracle.weights import synth_batch
@@ -113,7 +112,7 @@ def test_tf_b0_captured_steps_match_oracle_and_reference(H, W, dtype, golden_dir
     emul_loss = []
     for i, r in enumerate(runs):
         x, y = synth_batch(batch, 3, H, W, seed=1234 + i)
-        o = TO.train_step(spec, sd, x, y, ost, act_dtype=_dt(dtype))
+        o = OT.train_step(spec, sd, x, y, ost, act_dtype=_dt(dtype))
         emul_loss.append(float(o["loss"]))
         # tests/test_engine_gpu.py's step tolerances for B0 (fp16 per step; bf16 as its emulation bound). Batch 4 is a chaotic
         # regime for bf16 storage after the first update (the oracle's own bf16 emulation moves the step-1 logits by tens of
@@ -126,7 +125,7 @@ def test_tf_b0_captured_steps_match_oracle_and_reference(H, W, dtype, golden_dir
             # gradients against the fp32 oracle, relative to the yardstick of tests/test_engine_gpu.py: how far the oracle's own
             # 16-bit emulation lands from fp32 (batch 4 at 64x96 normalises the last stages over few values per channel, so
             # 16-bit rounding alone moves the gradients by tens of percent, oracle included)
-            o32 = TO.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None)
+            o32 = OT.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None)
             names = [n for n, _, _ in param_entries(spec)]
             gn = torch.cat([r["grads"][e.p_off[n][0]:e.p_off[n][0] + e.p_off[n][2]] for n in names]) / r["scale"]
             go, g32 = (torch.cat([oo["grads"][n].flatten() for n in names]) for oo in (o, o32))
@@ -147,12 +146,11 @@ def test_tf_b0_captured_steps_match_oracle_and_reference(H, W, dtype, golden_dir
 
 def test_tf_b4_step_at_380_matches_oracle():
     """reduced batch (2): one fp16 step of the full-resolution B4 plan against the oracle"""
-    import tf_same_oracle as TO
     from oracle import train as OT
     from oracle.weights import synth_batch
     spec, sd0, tr, runs = _run_steps("tf_efficientnet_b4", 2, 380, 380, "fp16", 1)
     x, y = synth_batch(2, 3, 380, 380, seed=1234)
-    o = TO.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, OT.OptState(kind="sgd", lr=0.01, momentum=0.9,
+    o = OT.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, OT.OptState(kind="sgd", lr=0.01, momentum=0.9,
                                                                                         weight_decay=1e-4), act_dtype=torch.float16)
     assert _relerr(runs[0]["logits"], o["logits"]) < 2e-2
     assert abs(runs[0]["loss"] - float(o["loss"])) < 5e-3

@@ -1,4 +1,4 @@
-"""Host logic of Xception, no GPU: the spec against the reference's state keys, the oracle (tests/xception_oracle.py) against
+"""Host logic of Xception, no GPU: the spec against the reference's state keys, the oracle (oracle/model.py) against
 the reference's train steps, the model factory (default_cfg, init, the keyword arguments the reference refuses or drops) and
 the plans. Fixtures: tools/mint_xception_goldens.py."""
 import json
@@ -9,12 +9,11 @@ from collections import Counter
 import pytest
 import torch
 
-import xception_oracle as XO
 from deepfake_detection_b200 import _lib
 from deepfake_detection_b200.arch import SUPPORTED_ARCHS, XCEPTION_ARCHS, get_spec, param_entries, state_entries, xception_extents
 from deepfake_detection_b200.engine import Engine
 from oracle import train as OT
-from oracle.weights import synth_batch, synth_state
+from oracle.weights import synth_batch, synth_state, tame_state
 from test_resnet_family_cpu import _digest
 from test_tf_efficientnet_cpu import RTOL, _check_summ
 
@@ -43,17 +42,17 @@ def test_spec_matches_reference_state_keys(key, golden_dir):
 
 @pytest.mark.parametrize("case", STEP_CASES)
 def test_oracle_matches_reference_steps(case, golden_dir):
-    """tests/xception_oracle.py against the reference's own train steps and eval, at the ResNet family's fp32 tolerances"""
+    """oracle/model.py against the reference's own train steps and eval, at the ResNet family's fp32 tolerances"""
     rec = json.load(open(os.path.join(golden_dir, case + ".json")))
     torch.set_num_threads(8)
     spec = get_spec(rec["arch"], num_classes=rec["num_classes"])
     sd = synth_state(spec, seed=rec["weight_seed"])
     if "tame" in rec:
-        sd = XO.tame_state(spec, sd, rec["tame"])
+        sd = tame_state(spec, sd, rec["tame"])
     opt = OT.OptState(kind=rec["opt"], lr=rec["lr"], momentum=rec["momentum"], weight_decay=rec["weight_decay"], eps=1e-8)
     for i, st in enumerate(rec["steps"]):
         x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=1234 + i)
-        out = XO.train_step(spec, sd, x, y, opt)
+        out = OT.train_step(spec, sd, x, y, opt)
         _check_summ(out["logits"], st["logits"], "logits step %d" % i, rtol=1e-3)
         assert float(out["loss"]) == pytest.approx(st["loss"], rel=1e-4)
         assert float(out["prec1"]) == pytest.approx(st["prec1"], abs=1e-3)
@@ -66,7 +65,7 @@ def test_oracle_matches_reference_steps(case, golden_dir):
         for k, s in st["buffers"].items():
             _check_summ(sd[k].float(), s, "buffer %s step %d" % (k, i), rt)
     x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=999)
-    ev = XO.validate_step(spec, sd, x, y)
+    ev = OT.validate_step(spec, sd, x, y)
     _check_summ(ev["logits"], rec["eval"]["logits"], "eval logits", rtol=5e-3)
 
 

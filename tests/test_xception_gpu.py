@@ -3,7 +3,7 @@
   * the depthwise forward with a ReLU input (after a BN or alone) and the fused depthwise backward in its two ReLU modes
     against fp64 torch at Xception's shapes; the strided block tail (dfd_bn_maxpool_add) and its backward
     (dfd_maxpool_bn_bwd_reduce) against F.max_pool2d and its indices, with negative inputs and forced ties;
-  * whole train steps against the oracle (tests/xception_oracle.py) and the reference's fixture; batch 32 at 299x299 from the
+  * whole train steps against the oracle (oracle/model.py) and the reference's fixture; batch 32 at 299x299 from the
     reference init against the fp32 oracle; eval at batch 1 in fp16 (the test_img path);
   * drop_rate changes no bit; checkpoints round-trip bit for bit and two engines agree bit for bit; the runner's train_epoch
     with SGD and RMSpropTF and an EMA update.
@@ -209,23 +209,22 @@ def test_steps_match_oracle_and_reference(dtype, golden_dir):
     """the tamed fixture (batch 8, 64x80) with tests/test_resnet_family_gpu.py's statements: step 0 logits and loss against the
     oracle's 16-bit emulation, logits and gradients against the fp32 oracle within 1.5 x the emulation's own distance + a
     margin, every step's loss against the reference, the step-0 logits against the reference's samples"""
-    import xception_oracle as XO
     from deepfake_detection_b200.arch import get_spec, param_entries
     from oracle import train as OT
-    from oracle.weights import synth_batch, synth_state
+    from oracle.weights import synth_batch, synth_state, tame_state
     rec = json.load(open(os.path.join(golden_dir, "step_xception_tame_64x80.json")))
     batch, H, W = rec["batch"], rec["H"], rec["W"]
     spec = get_spec("xception")
-    sd0 = XO.tame_state(spec, synth_state(spec, seed=rec["weight_seed"]), rec["tame"])
+    sd0 = tame_state(spec, synth_state(spec, seed=rec["weight_seed"]), rec["tame"])
     tr, runs = _trainer_steps(batch, H, W, dtype, len(rec["steps"]), sd0)
     e = tr.engine
     sd = {k: v.clone() for k, v in sd0.items()}
     ost = OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4)
     for i, (r, st) in enumerate(zip(runs, rec["steps"])):
         x, y = synth_batch(batch, 3, H, W, seed=1234 + i)
-        o = XO.train_step(spec, sd, x, y, ost, act_dtype=TDT[dtype])
+        o = OT.train_step(spec, sd, x, y, ost, act_dtype=TDT[dtype])
         if i == 0:
-            o32 = XO.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None)
+            o32 = OT.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None)
             yard_logits = _rel(o["logits"], o32["logits"])
             assert _rel(r["logits"], o["logits"]) < max(2e-2 if dtype == "fp16" else 6e-2, 1.5 * yard_logits)
             assert abs(r["loss"] - float(o["loss"])) < 5e-3, (r["loss"], float(o["loss"]))
@@ -245,7 +244,6 @@ def test_steps_match_oracle_and_reference(dtype, golden_dir):
 @pytest.mark.parametrize("dtype", ["bf16", "fp16"])
 def test_batch32_299_reference_init(dtype):
     """loss and updated weights within 1e-2 of the fp32 oracle from the reference's initialisers (batch 32, 299x299)"""
-    import xception_oracle as XO
     from deepfake_detection_b200.arch import get_spec, param_entries
     from deepfake_detection_b200.models import init_state_dict
     from deepfake_detection_b200.trainer import Trainer
@@ -257,7 +255,7 @@ def test_batch32_299_reference_init(dtype):
     if key not in globals():
         sd = {k: v.clone() for k, v in init_state_dict(spec, seed=11).items()}
         x, y = synth_batch(32, 3, 299, 299, seed=1234)
-        out = XO.train_step(spec, sd, x, y, OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4))
+        out = OT.train_step(spec, sd, x, y, OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4))
         globals()[key] = dict(sd=sd, x=x, y=y, logits=out["logits"], loss=float(out["loss"]))
     o = globals()[key]
     pn = [n for n, _, _ in param_entries(spec)]
@@ -287,7 +285,7 @@ def test_batch32_299_reference_init(dtype):
 def test_eval_batch1_fp16_299():
     """the test_img path: eval at batch 1 in fp16 from the reference's initialisers, against the fp32 oracle and its fp16
     emulation (the synthetic weights of oracle/weights.py grow the activations beyond the fp16 range at 299x299)"""
-    import xception_oracle as XO
+    from oracle import train as OT
     from deepfake_detection_b200.arch import get_spec
     from deepfake_detection_b200.models import create_model, init_state_dict
     from oracle.weights import synth_batch
@@ -300,8 +298,8 @@ def test_eval_batch1_fp16_299():
     with torch.no_grad():
         got = m(x.cuda()).cpu()
         again = m(x.cuda()).cpu()
-    ref = XO.validate_step(spec, sd, x, y)["logits"]
-    emu = XO.validate_step(spec, sd, x, y, act_dtype=torch.float16)["logits"]
+    ref = OT.validate_step(spec, sd, x, y)["logits"]
+    emu = OT.validate_step(spec, sd, x, y, act_dtype=torch.float16)["logits"]
     assert torch.equal(got, again)
     assert _rel(got, emu) < 2e-2 and _rel(got, ref) < 1.5 * _rel(emu, ref) + 2e-2, (_rel(got, emu), _rel(got, ref), _rel(emu, ref))
 
@@ -354,14 +352,13 @@ def test_checkpoint_round_trip_is_bit_exact():
 def test_runner_train_epoch_with_ema(opt_name):
     """train_epoch's loop body over create_model("xception") for two steps, against the oracle's two steps (tamed synthetic
     weights); then one EMA update"""
-    import xception_oracle as XO
     from deepfake_detection_b200.arch import get_spec, param_entries
     from deepfake_detection_b200.ema import ModelEma
     from deepfake_detection_b200.models import create_model
     from deepfake_detection_b200.optim import create_optimizer
     from deepfake_detection_b200.runners.train import train_epoch
     from oracle import train as OT
-    from oracle.weights import synth_batch, synth_state
+    from oracle.weights import synth_batch, synth_state, tame_state
 
     class _Loader(list):
         mixup_enabled = False
@@ -372,7 +369,7 @@ def test_runner_train_epoch_with_ema(opt_name):
                            world_size=1, local_rank=0, log_interval=1, save_images=False, recovery_interval=0, tta=0,
                            model="xception")
     spec = get_spec("xception")
-    sd0 = XO.tame_state(spec, synth_state(spec, seed=7))
+    sd0 = tame_state(spec, synth_state(spec, seed=7))
     model = create_model("xception", num_classes=2)
     model.load_state_dict(sd0)
     opt = create_optimizer(args, model)
@@ -385,7 +382,7 @@ def test_runner_train_epoch_with_ema(opt_name):
     for key, adt in (("emul", torch.bfloat16), ("fp32", None)):
         sd = {k: v.clone() for k, v in sd0.items()}
         ost = OT.OptState(kind=opt_name, lr=lr, momentum=0.9, weight_decay=1e-4, eps=args.opt_eps)
-        losses = [float(XO.train_step(spec, sd, x, y, ost, act_dtype=adt)["loss"]) for x, y in data]
+        losses = [float(OT.train_step(spec, sd, x, y, ost, act_dtype=adt)["loss"]) for x, y in data]
         res[key] = (sum(losses) / 2, torch.cat([(sd[n] - sd0[n]).flatten() for n in pn]))
     got = model.state_dict()
     dn = torch.cat([(got[n].cpu() - sd0[n]).flatten() for n in pn])

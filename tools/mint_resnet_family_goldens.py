@@ -18,7 +18,7 @@ step_resnet101.json
         one step + eval at batch 2, 64x64.
 step_resnet26d_tame_104x88.json, step_resnet34_tame_96.json, step_wide_resnet50_2_tame_96.json, step_resnet101_tame_96.json
         the same at batch 8 with the last BatchNorm gamma of every residual branch scaled by 0.2
-        (tests/resnet_family_oracle.py `tame_state`, recorded as "tame"): resnet26d at 104x88 (pools 26x22 -> 13x11,
+        (oracle/weights.py `tame_state`, recorded as "tame"): resnet26d at 104x88 (pools 26x22 -> 13x11,
         13x11 -> 7x6 and 7x6 -> 4x3), the others at 96x96, resnet101 one step. The un-tamed steps above amplify 16-bit
         rounding into changes of order one; these are the steps a 16-bit path is compared with.
 """
@@ -31,7 +31,6 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 from deepfake_detection_b200.arch import RESNET_ARCHS  # noqa: E402
 from oracle import ref_shims  # noqa: E402
@@ -53,7 +52,7 @@ def mint_state_keys():
 def mint_tamed(arch, batch, H, W, n_steps, tag):
     """tools/mint_multiclass_goldens.py `mint_step_k` with the residual branches of the synthetic weights tamed"""
     import mint_multiclass_goldens as MM
-    from resnet_family_oracle import TAME, tame_state
+    from oracle.weights import TAME, tame_state
     orig = MM.synth_state
     MM.synth_state = lambda spec, seed=0: tame_state(spec, orig(spec, seed=seed))
     try:

@@ -15,7 +15,7 @@ step_seresnet50_64x64.json
 step_seresnet101.json
         one step + eval of seresnet101 at batch 2, 64x64.
 step_seresnet18_tame_70x72.json, step_seresnet50_tame_64x64.json, step_seresnet101_tame_64x64.json
-        the same at batch 8 with the last BatchNorm gamma of every residual branch scaled by 0.2 (tests/senet_oracle.py
+        the same at batch 8 with the last BatchNorm gamma of every residual branch scaled by 0.2 (oracle/weights.py
         `tame_state`, recorded as "tame"): the un-tamed steps amplify 16-bit rounding into changes of order one; these are the
         steps a 16-bit path is compared with.
 Every model is built with drop_rate=0.0: SENet's default of 0.2 would draw dropout masks from torch's generator, which no other
@@ -31,7 +31,6 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 from deepfake_detection_b200.arch import SENET_ARCHS  # noqa: E402
 from oracle import ref_shims  # noqa: E402
@@ -55,7 +54,7 @@ def mint_step(arch, batch, H, W, n_steps, tag, tame=False):
     of the synthetic weights tamed"""
     import dfd.timm.models as RM
     import mint_multiclass_goldens as MM
-    from senet_oracle import TAME, tame_state
+    from oracle.weights import TAME, tame_state
     orig_create, orig_synth = RM.create_model, MM.synth_state
     RM.create_model = partial(orig_create, drop_rate=0.0)
     if tame:

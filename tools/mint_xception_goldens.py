@@ -13,7 +13,7 @@ step_xception_299.json
         one step + eval at batch 2, 299x299 (the model's own geometry).
 step_xception_tame_64x80.json
         two steps + eval at batch 8, 64x80, with the last BatchNorm gamma of every block's `rep` scaled by 0.2
-        (tests/xception_oracle.py `tame_state`, recorded as "tame"): the un-tamed steps amplify 16-bit rounding into changes of
+        (oracle/weights.py `tame_state`, recorded as "tame"): the un-tamed steps amplify 16-bit rounding into changes of
         order one; this is the step a 16-bit path is compared with.
 """
 import json
@@ -25,7 +25,6 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 from oracle import ref_shims  # noqa: E402
 from oracle.mint_goldens import GOLDEN  # noqa: E402
@@ -43,7 +42,7 @@ def mint_state_keys():
 
 def mint_tamed(batch, H, W, n_steps, tag):
     import mint_multiclass_goldens as MM
-    from xception_oracle import TAME, tame_state
+    from oracle.weights import TAME, tame_state
     orig = MM.synth_state
     MM.synth_state = lambda spec, seed=0: tame_state(spec, orig(spec, seed=seed))
     try:
