@@ -8,13 +8,10 @@ import torch
 import torch.nn.functional as F
 
 from deepfake_detection_b200 import _lib
-from gpu_checks import DT, P, _bn_params, maxerr_scaled, nchw, nhwc, relerr, st, stat_buf
+from gpu_checks import (DT, P, TINY16, U_OUT, ULP_IN, _bn_params, _u32, dw_dgrad_bound, dw_input_grad64, maxerr_scaled,
+                        maxpool_bwd_bound, nchw, nhwc, ratio_pair, relerr, st, stat_buf, sum_bound)
 
 ACT_NONE, ACT_RELU = 0, 2
-# half an ulp of the 16-bit output (relative), the largest relative ulp of a 16-bit input, the smallest positive 16-bit value
-U_OUT = {torch.bfloat16: 2.0 ** -8, torch.float16: 2.0 ** -11}
-ULP_IN = {torch.bfloat16: 2.0 ** -7, torch.float16: 2.0 ** -10}
-TINY16 = {torch.bfloat16: 2.0 ** -133, torch.float16: 2.0 ** -24}
 
 
 def _nan(*shape, dtype=torch.float32):
@@ -23,12 +20,6 @@ def _nan(*shape, dtype=torch.float32):
 
 def _bits_equal(a, b):
     return bool(torch.equal(a.view(torch.int16), b.view(torch.int16))) if a.element_size() == 2 else bool(torch.equal(a, b))
-
-
-def _u32(y, scale, shift):
-    """fmaf(y, scale, shift) as the kernels form it: the product of a 16-bit and an fp32 value is exact in fp64, the sum is
-    rounded to fp32 (the fp64 rounding in between changes the result only at an exact fp32 tie)"""
-    return (y.double() * scale.double() + shift.double()).float()
 
 
 # ---- depthwise convolution with a ReLU input (Xception's separable convolutions) ---------------------------------------
@@ -99,6 +90,10 @@ def check_dwconv_relu(N, H, W, C, k, s, dtype=torch.bfloat16, bn=True, add=False
     base = addt.double() if add else torch.zeros_like(ga)
     gref = torch.where(mask, ga + base, base)
     res["dgrad_rel"] = relerr(gx.double(), gref)
+    # element-wise (gpu_checks.dw_dgrad_bound, MODES 2 / 3): gy is staged as stored, the mask is exact
+    ga64, mag64 = dw_input_grad64(gy, w, H, W, k, s, (1, 1, 1, 1))
+    res["dgrad_ulp"], res["dgrad_ulp_bf16trip"] = dw_dgrad_bound(gx, ga64, mag64, k, dtype, add=addt, mask=mask)
+    del ga64, mag64
     # the mask, exactly: off it gx is the added gradient (or zero) bit for bit; on it (without `add`, which can absorb a
     # small dgrad in the rounding) gx is not zero where the dgrad is not
     off = ~mask & (gx.double() != base)
@@ -147,6 +142,9 @@ def check_bn_maxpool(N, H, W, C, dtype=torch.bfloat16, seed=0):
     pooled, ind = F.max_pool2d(u, 3, 2, 1, return_indices=True)
     ref = nhwc(pooled.detach().double()) + ys.double() * scale_s.double() + shift_s.double()
     res = dict(nan=int(torch.isnan(out.float()).sum()), out_max=maxerr_scaled(out, ref), noidx_mismatch=int(not _bits_equal(out, out2)))
+    # bn_act.cu:1251-1259: the maximum of the fp32 u's (exact, the reference's values), + fmaf(ys, scale_s, shift_s), one store
+    sc_mag = nhwc(pooled.detach().double()).abs() + (ys.double() * scale_s.double()).abs() + shift_s.double().abs()
+    res["out_ulp"], res["out_ulp_bf16trip"] = ratio_pair(out, ref, sum_bound(ref, sc_mag, 2, dtype))
     iy, ix = nhwc(ind // W), nhwc(ind % W)
     oy = torch.arange(Ho, device="cuda").view(1, Ho, 1, 1)
     ox = torch.arange(Wo, device="cuda").view(1, 1, Wo, 1)
@@ -173,6 +171,7 @@ def check_bn_maxpool(N, H, W, C, dtype=torch.bfloat16, seed=0):
     gref = nhwc(u.grad.double())
     gxd = gx.double()
     xhat = (y.double() - mean.double()) * rstd.double()
+    res["bwd_ulp"], res["bwd_ulp_bf16trip"] = maxpool_bwd_bound(gx, nhwc(u.detach()), gy, lambda t: F.max_pool2d(t, 3, 2, 1), dtype)
     res.update(nan_b=int(torch.isnan(gx.float()).sum()), bwd_max=maxerr_scaled(gx, gref),
                s1_rel=relerr(s1.sum(0), gxd.sum((0, 1, 2))), s2_rel=relerr(s2.sum(0), (gxd * xhat).sum((0, 1, 2))))
     return res
@@ -199,7 +198,8 @@ def check_maxpool_ceil(N, H, W, C, dtype=torch.bfloat16, seed=0):
     oy = torch.arange(Ho, device="cuda").view(1, Ho, 1, 1)
     ox = torch.arange(Wo, device="cuda").view(1, 1, Wo, 1)
     flat = (2 * oy + idx.long() // 3) * W + 2 * ox + idx.long() % 3
-    return dict(fwd_mismatch=int((y.float() != nhwc(ref.detach())).sum()), idx_mismatch=int((flat != nhwc(ind)).sum()),
+    bwd_ulp = maxpool_bwd_bound(gx, x, gy, lambda t: F.max_pool2d(t, 3, 2, ceil_mode=True), dtype)
+    return dict(bwd_ulp=bwd_ulp[0], bwd_ulp_bf16trip=bwd_ulp[1],fwd_mismatch=int((y.float() != nhwc(ref.detach())).sum()), idx_mismatch=int((flat != nhwc(ind)).sum()),
                 clipped=int((H - 3) % 2 == 1) + int((W - 3) % 2 == 1), bwd_max=maxerr_scaled(gx, nhwc(xr.grad.double())),
                 nan=int(torch.isnan(y.float()).sum()), nan_b=int(torch.isnan(gx.float()).sum()))
 
@@ -335,8 +335,16 @@ def check_avgpool2(N, H, W, C, add=True, dtype=torch.bfloat16, seed=0):
     ref = F.avg_pool2d(xr, 2, 2, ceil_mode=True, count_include_pad=False)
     ref.backward(nchw(dy.double()))
     gref = nhwc(xr.grad) + (addt.double() if add else 0.0)
-    return dict(fwd_max=maxerr_scaled(y, nhwc(ref.detach())), bwd_max=maxerr_scaled(dx, gref),
-                nan=int(torch.isnan(y.float()).sum()), nan_b=int(torch.isnan(dx.float()).sum()))
+    res = dict(fwd_max=maxerr_scaled(y, nhwc(ref.detach())), bwd_max=maxerr_scaled(dx, gref),
+               nan=int(torch.isnan(y.float()).sum()), nan_b=int(torch.isnan(dx.float()).sum()))
+    # bn_act.cu:1159-1179: <= 4 terms summed in fp32, times 1 / count (1, 2 or 4: exact); bn_act.cu:1206: one fmaf
+    with torch.no_grad():
+        fref = nhwc(ref.detach())
+        fmag = nhwc(F.avg_pool2d(xr.detach().abs(), 2, 2, ceil_mode=True, count_include_pad=False))
+        res["fwd_ulp"], res["fwd_ulp_bf16trip"] = ratio_pair(y, fref, sum_bound(fref, fmag, 4, dtype))
+        bmag = nhwc(xr.grad).abs() + (addt.double().abs() if add else 0.0)
+        res["bwd_ulp"], res["bwd_ulp_bf16trip"] = ratio_pair(dx, gref, sum_bound(gref, bmag, 1, dtype))
+    return res
 
 
 # ---- dense convolutions through im2col ---------------------------------------------------------------------------------------
@@ -373,4 +381,13 @@ def check_im2col(N, H, W, C, k, s, pad, add=False, dtype=torch.bfloat16, seed=0)
         gref[n0:n1] = F.fold(dc.double(), (H, W), k, padding=pad, stride=s)
     gref = nhwc(gref) + (addt.double() if add else 0.0)
     res.update(col2im_max=maxerr_scaled(dx, gref), nan_b=int(torch.isnan(dx.float()).sum()))
+    # conv_dense.cu:50-71: add, then every overlapping column term (ceil(k/s)^2 at most) summed in fp32, one store
+    gmag = torch.zeros(N, C, H, W, device="cuda", dtype=torch.float64)
+    for n0 in range(0, N, per):
+        n1 = min(N, n0 + per)
+        dc = dcols[n0 * Ho * Wo:n1 * Ho * Wo].view(n1 - n0, Ho * Wo, k * k, C).permute(0, 3, 2, 1).reshape(n1 - n0, C * k * k, Ho * Wo)
+        gmag[n0:n1] = F.fold(dc.double().abs(), (H, W), k, padding=pad, stride=s)
+    gmag = nhwc(gmag) + (addt.double().abs() if add else 0.0)
+    n = -(-k // s) ** 2 + 1
+    res["col2im_ulp"], res["col2im_ulp_bf16trip"] = ratio_pair(dx, gref, sum_bound(gref, gmag, n, dtype))
     return res

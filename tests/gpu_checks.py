@@ -37,6 +37,184 @@ def maxerr_scaled(a, b):
     return float(((a - b).abs() / (b.abs() + scale)).max())
 
 
+# ---- element-wise error bounds ---------------------------------------------------------------------------------------------
+# A 16-bit output is held to |out - ref| <= bound element by element, the bound a sum of named terms, each traced to a step of
+# the kernel's arithmetic. The reference rounds where the kernel rounds (16-bit staged operands, the fp32 fmaf of u), so the
+# terms cover only what the kernel does in fp32 and its final store. The helpers work on CPU and GPU tensors alike.
+#
+# half an ulp of the 16-bit output (relative), the largest relative ulp of a 16-bit input, the smallest positive 16-bit value
+U_OUT = {torch.bfloat16: 2.0 ** -8, torch.float16: 2.0 ** -11}
+ULP_IN = {torch.bfloat16: 2.0 ** -7, torch.float16: 2.0 ** -10}
+TINY16 = {torch.bfloat16: 2.0 ** -133, torch.float16: 2.0 ** -24}
+# sigmoid_fast (common.cuh:97) = fmaf(tanh.approx(x / 2), 0.5, 0.5): tanh.approx.f32 has at most 2^-10.987 relative error
+# (PTX ISA) and |tanh| <= 1, halved by the fmaf, plus the fmaf's own fp32 rounding (2^-24, as s <= 1): absolute on s
+E_TANH = 2.0 ** -10.987
+E_SIG = 0.5 * E_TANH + 2.0 ** -24
+# the scaled bound of the fp16 tensor-core contractions (the fp16 GEMM's, tests/test_plan_launches_gpu.OUT_FP16_GEMM)
+OUT_FP16_TC = 2.0 ** -9
+
+
+def ulp_ratio(out, ref, bound):
+    """max |out - ref| / bound (<= 1: every element within its bound)"""
+    return float(((out.double() - ref.double()).abs() / (bound.double() + 1e-300)).max())
+
+
+def bf16_trip(out):
+    """the output rounded through bf16 and back: what a kernel that rounds through bf16 somewhere would store"""
+    return out.to(torch.bfloat16).to(out.dtype)
+
+
+def out_term(ref, dtype):
+    """the kernel's one rounding of its fp32 result to the 16-bit output: half an ulp, or half the subnormal spacing"""
+    return U_OUT[dtype] * ref.double().abs() + TINY16[dtype] / 2
+
+
+def in_term(mag, dtype):
+    """an operand rounded to 16 bits at a point where the reference cannot round it identically: one ulp of |operand| * |weight|"""
+    return ULP_IN[dtype] * mag
+
+
+def acc_term(mag, n=16):
+    """an fp32 evaluation of a short sum or chain of n operations (taps, pool windows, col2im overlaps, the fmaf's of a row
+    kernel): at most n roundings of 2^-24 of the partial sums, each <= mag = the same sum of absolute values; 2^-20 for n <= 16"""
+    return max(n, 16) * 2.0 ** -24 * mag
+
+
+def swish64(u):
+    return u * torch.sigmoid(u)
+
+
+def swish_grad64(u):
+    s = torch.sigmoid(u)
+    return s * (1 + u * (1 - s))
+
+
+def swish_fwd_term(u, mult):
+    """act_fwd<SWISH>(u) = u * sigmoid_fast(u) (common.cuh:102): |u| E_SIG from the sigmoid, 2^-24 |swish| from the product;
+    times mult = |what the activation is multiplied by| (gate, weight)"""
+    return (u.abs() * E_SIG + 2.0 ** -24 * swish64(u).abs()) * mult
+
+
+def swish_grad_err(u):
+    """|act_bwd<SWISH>(u) - swish'(u)|: d(s) = fmaf(s, fmaf(-u, s, u), s) = s + u s - u s^2 (common.cuh:110) with s off by
+    delta, |delta| <= E_SIG: d(s + delta) - d(s) = delta (1 + u (1 - 2 s)) - u delta^2; the two fmaf's round to fp32 at
+    2^-24 (|s u (1 - s)| + |d|) <= 2^-23 (s + |s u (1 - s)|)"""
+    s = torch.sigmoid(u)
+    return (1 + u * (1 - 2 * s)).abs() * E_SIG + u.abs() * E_SIG ** 2 + 2.0 ** -23 * (s + (s * u * (1 - s)).abs())
+
+
+def swish_bwd_term(u, mult):
+    """a gradient of magnitude mult times act_bwd<SWISH>(u)"""
+    return swish_grad_err(u) * mult
+
+
+def elem_bound(ref, dtype, *terms):
+    """out_term + the error of the fp32 value before the store (1 + U_OUT: the store's rounding is relative to that value)"""
+    b = out_term(ref, dtype)
+    for t in terms:
+        b = b + (1 + U_OUT[dtype]) * t
+    return b
+
+
+def ratio_pair(out, ref, bound):
+    """(ratio of the output, ratio of the output rounded through bf16) on the same reference and bound"""
+    return ulp_ratio(out, ref, bound), ulp_ratio(bf16_trip(out), ref, bound)
+
+
+def _scaled_pair(out, ref, to_nchw=True):
+    """maxerr_scaled of a 16-bit NHWC output (to_nchw: against an NCHW reference) against an fp64 reference, and of the output
+    rounded through bf16"""
+    if to_nchw:
+        out = nchw(out)
+    return maxerr_scaled(out.double(), ref), maxerr_scaled(bf16_trip(out).double(), ref)
+
+
+def maxpool_bwd_bound(gx, x, gy, pool, dtype):
+    """a max-pool's gathered gradient (dfd_maxpool_bwd, dfd_maxpool_ceil_bwd, dfd_maxpool_bn_bwd_reduce; conv_dense.cu:271-293,
+    bn_act.cu:1296-1314): the fp32 sum of the <= 4 window gradients routed to a pixel, rounded once. Reference: fp64 autograd
+    of `pool` on the values the kernel compared (NHWC x; same windows, same first-maximum rule), and the same routing of |gy|
+    for the sum's magnitude. Returns (ratio, ratio of the output rounded through bf16)."""
+    xr = nchw(x.double()).requires_grad_(True)
+    y = pool(xr)
+    ref, = torch.autograd.grad(y, xr, nchw(gy.double()), retain_graph=True)
+    mag, = torch.autograd.grad(y, xr, nchw(gy.double()).abs())
+    ref, mag = nhwc(ref), nhwc(mag)
+    return ratio_pair(gx, ref, sum_bound(ref, mag, 4, dtype))
+
+
+def bn_act_bound(u, act, gt, r, res_mode, dtype):
+    """(reference, bound) of dfd_bn_act (bn_act.cu:233-246): act(u) [* gate] [+ res] [relu], every step in fp32 (relu is
+    1-Lipschitz), one 16-bit store. u: the fp32 fmaf(y, scale, shift) in fp64; gt: the gate broadcast (or 1); r: the residual
+    or None. Terms: the fp32 steps over |act(u) gate| + |res|, and for Swish the tanh.approx term on |u gate|."""
+    a = _act_ref(u, act)[0] * gt
+    ref, mag = a, a.abs()
+    if r is not None:
+        ref, mag = ref + r.double(), mag + r.double().abs()
+    if res_mode == 2:
+        ref = ref.clamp_min(0)
+    terms = [acc_term(mag, 4)] + ([swish_fwd_term(u, gt.abs())] if act == 1 else [])
+    return ref, elem_bound(ref, dtype, *terms)
+
+
+def act_bwd_bound(u, act, gin, gmag, dtype):
+    """(reference, bound) of dfd_act_bwd (bn_act.cu:879-884): gin = fmaf(da, gate, dpool * inv_hw) in fp32 (gmag = |da gate| +
+    |dpool| / hw), times act_bwd(u) (Swish: the tanh.approx term of swish_grad_err on |gin|), one 16-bit store"""
+    dact = _act_ref(u, act)[1]
+    ref = gin * dact
+    gacc = acc_term(gmag, 4)
+    derr = swish_grad_err(u) if act == 1 else torch.zeros_like(u)
+    terms = [gacc * (dact.abs() + derr)] + ([swish_bwd_term(u, gmag + gacc)] if act == 1 else [])
+    return ref, elem_bound(ref, dtype, *terms)
+
+
+def sum_bound(ref, mag, n, dtype):
+    """a short fp32 sum of n stored terms (pool windows, col2im overlaps, an added gradient) rounded once to 16 bits"""
+    return elem_bound(ref, dtype, acc_term(mag, n))
+
+
+def _u32(y, scale, shift):
+    """fmaf(y, scale, shift) as the kernels form it: the product of a 16-bit and an fp32 value is exact in fp64, the sum is
+    rounded to fp32 (the fp64 rounding in between changes the result only at an exact fp32 tie)"""
+    return (y.double() * scale.double() + shift.double()).float()
+
+
+def staged_dy(gy, yout, cA, cB, cC, dtype):
+    """the gradient tile the depthwise backward stages (dwconv.cu stage_grad_tile): round16(fmaf(cA, gy, fmaf(cB, yout, cC))),
+    in fp64 (exact products, each fmaf rounded to fp32 as the kernel rounds it)"""
+    inner = (cB.double() * yout.double() + cC.double()).float()
+    return (cA.double() * gy.double() + inner.double()).float().to(dtype).double()
+
+
+def dw_input_grad64(dy, w, H, W, k, s, pads):
+    """the depthwise input gradient in fp64 and the same sum over |w| |dy| (NHWC): dy [N, Ho, Wo, C], w [C, k*k] or
+    [C, 1, k, k], pads (top, bottom, left, right) of the forward"""
+    N, C = dy.shape[0], dy.shape[3]
+    pt, pb, pl, pr = pads
+    shape = (N, C, H + pt + pb, W + pl + pr)
+    w64, d64 = w.double().reshape(C, 1, k, k), nchw(dy.double())
+    ga = torch.nn.grad.conv2d_input(shape, w64, d64, stride=s, groups=C)[:, :, pt:pt + H, pl:pl + W]
+    mag = torch.nn.grad.conv2d_input(shape, w64.abs(), d64.abs(), stride=s, groups=C)[:, :, pt:pt + H, pl:pl + W]
+    return nhwc(ga), nhwc(mag)
+
+
+def dw_dgrad_bound(gx, ga, mag, k, dtype, u=None, add=None, mask=None):
+    """element-wise bound of a depthwise input gradient (dwconv.cu dwconv_bwd_kernel / dwconv_dgrad_kernel): the fp32 sum of
+    k*k taps of the staged dy (acc_term over mag), then
+      u given (MODE 1): gu = round16(acc * act_bwd<SWISH>(u)) - the tanh.approx term on |acc| and the product's rounding;
+      mask given (MODES 2, 3): round16(acc * mask (+ add));  else (MODE 0): round16(acc (+ add)).
+    Returns (ratio, ratio of the output rounded through bf16)."""
+    if u is not None:
+        d, err = swish_grad64(u), swish_grad_err(u)
+        ref = ga * d
+        acc = acc_term(mag, k * k + 1)
+        bound = elem_bound(ref, dtype, acc * (d.abs() + err), swish_bwd_term(u, ga.abs() + acc))
+    else:
+        m = mask.double() if mask is not None else 1.0
+        ref = ga * m + (add.double() if add is not None else 0.0)
+        bound = elem_bound(ref, dtype, acc_term(mag * m + (add.double().abs() if add is not None else 0.0), k * k + 1))
+    return ratio_pair(gx, ref, bound)
+
+
 def slots():
     return _lib.lib().stat_slots
 
@@ -173,7 +351,7 @@ def check_dwconv(N, H, W, C, k, s, dtype=torch.bfloat16, affine=True, seed=0, fw
     #   |out - ref| <= u_out |ref| + (ulp_in + 2^-20) sum_taps |w a| + (1 + ulp_in) 2^-11 sum_taps |w u|
     # The scaled 2^-7 (|ref| + rms) bound does not follow from this arithmetic and fails once cancelling sums are sampled 10^8
     # times; a wrong tap, channel or tile is off by a whole |w a| term and fails this one.
-    u_out, ulp_in = (2.0 ** -8, 2.0 ** -7) if dtype == torch.bfloat16 else (2.0 ** -11, 2.0 ** -10)
+    u_out, ulp_in = U_OUT[dtype], ULP_IN[dtype]
     with torch.no_grad():
         mag = F.conv2d(a_q.detach().abs(), w.abs(), stride=s, padding=pad, groups=C)
         bound = u_out * ref.detach().abs() + (ulp_in + 2.0 ** -20) * mag
@@ -181,6 +359,12 @@ def check_dwconv(N, H, W, C, k, s, dtype=torch.bfloat16, affine=True, seed=0, fw
             bound += (1 + ulp_in) * 2.0 ** -11 * F.conv2d(u.detach().abs(), w.abs(), stride=s, padding=pad, groups=C)
         res["fwd_ulp"] = float(((nchw(out.float()) - ref.detach()).abs() / (bound + 1e-30)).max())
         del mag, bound
+        if not affine:      # a raw input is read as stored: no staging rounding, only the taps' fp32 sum and the store (fp64)
+            x64, w64 = nchw(x.double()), w.double()
+            ref64 = F.conv2d(x64, w64, stride=s, padding=pad, groups=C)
+            mag64 = F.conv2d(x64.abs(), w64.abs(), stride=s, padding=pad, groups=C)
+            res["fwd_ulp"], res["fwd_ulp_bf16trip"] = ratio_pair(nchw(out), ref64, elem_bound(ref64, dtype, acc_term(mag64, k * k)))
+            del x64, ref64, mag64
     of = out.double()
     res["sum_rel"] = relerr(s1.sum(0), of.sum((0, 1, 2)))
     res["sq_rel"] = relerr(s2.sum(0), (of * of).sum((0, 1, 2)))
@@ -191,6 +375,8 @@ def check_dwconv(N, H, W, C, k, s, dtype=torch.bfloat16, affine=True, seed=0, fw
     cC = 0.01 * torch.randn(C, device="cuda", generator=g)
     dy = (cA * gy.float() + cB * out.float() + cC).to(dtype).float()
     ref.backward(nchw(dy))
+    # the input gradient's element-wise bound (dgrad_ulp <= 1) in fp64 on the dy tile exactly as the kernel stages it
+    ga64, mag64 = dw_input_grad64(staged_dy(gy, out, cA, cB, cC, dtype), w, H, W, k, s, (pad, pad, pad, pad))
     dW = torch.zeros_like(w)
     _lib.call("dfd_dwconv_wgrad", P(x), P(scale) if affine else None, P(shift) if affine else None, P(gy), P(out), P(cA), P(cB),
               P(cC), P(dW), N, H, W, C, k, s, DT[dtype], st())
@@ -208,6 +394,7 @@ def check_dwconv(N, H, W, C, k, s, dtype=torch.bfloat16, affine=True, seed=0, fw
         gu_ref = xr.grad / scale.view(1, C, 1, 1)
         res["dgrad_max"] = maxerr_scaled(nchw(gx.float()), gu_ref)
         res["dgrad_rel"] = relerr(nchw(gx.float()), gu_ref)
+        res["dgrad_ulp"], res["dgrad_ulp_bf16trip"] = dw_dgrad_bound(gx, ga64, mag64, k, dtype, u=_u32(x, scale, shift).double())
         gxd = gx.double()
         xhat = (x.double() - mean.double()) * rstd.double()
         res["bs1_rel"] = relerr(b1.sum(0), gxd.sum((0, 1, 2)))
@@ -239,6 +426,7 @@ def check_dwconv(N, H, W, C, k, s, dtype=torch.bfloat16, affine=True, seed=0, fw
         ref_gx = xr.grad + nchw(addt.float()) if add else xr.grad
         res["dgrad_max"] = maxerr_scaled(nchw(gx.float()), ref_gx)
         res["dgrad_rel"] = relerr(nchw(gx.float()), ref_gx)
+        res["dgrad_ulp"], res["dgrad_ulp_bf16trip"] = dw_dgrad_bound(gx, ga64, mag64, k, dtype, add=addt)
         # fused pass, mode 0 (input consumed as is, residual gradient added when given)
         gx2 = torch.full((N, H, W, C), float("nan"), device="cuda", dtype=dtype)
         dW2 = torch.zeros_like(w)
@@ -484,14 +672,11 @@ def check_row_kernel(kernel, N, HW, C, args, ptrs, dtype=torch.bfloat16, seed=0)
         _lib.call(kernel, P(y), P(scale) if has(1) else None, P(shift) if has(2) else None, P(gate) if has(3) else None,
                   P(r), P(out), N, HW, C, act, res_mode, d, st())
         torch.cuda.synchronize()
-        ref = _act_ref(u_of(has(1)), act)[0]
-        if has(3):
-            ref = ref * gate.double().unsqueeze(1)
-        if res_mode:
-            ref = ref + r.double()
-        if res_mode == 2:
-            ref = ref.clamp_min(0)
+        u = u_of(has(1))
+        gt = gate.double().unsqueeze(1) if has(3) else torch.ones((), dtype=torch.float64, device="cuda")
+        ref, bound = bn_act_bound(u, act, gt, r if res_mode else None, res_mode, dtype)
         res.update(out_max=maxerr_scaled(out.float(), ref), nan=int(torch.isnan(out.float()).sum()))
+        res["out_ulp"], res["out_ulp_bf16trip"] = ratio_pair(out, ref, bound)
     elif kernel == "dfd_act_bwd":
         act = args[0]
         da = (torch.randn(N, HW, C, device="cuda", generator=g) * 0.1).to(dtype) if has(0) else None
@@ -506,8 +691,10 @@ def check_row_kernel(kernel, N, HW, C, args, ptrs, dtype=torch.bfloat16, seed=0)
             gin = da.double() * (gate.double().unsqueeze(1) if has(6) else 1.0)
         if has(7):
             gin = gin + dpool.double().unsqueeze(1) / HW
-        ref = gin * _act_ref(u_of(True), act)[1]
+        gmag = gin.abs() if not has(7) else (gin - dpool.double().unsqueeze(1) / HW).abs() + dpool.double().abs().unsqueeze(1) / HW
+        ref, bound = act_bwd_bound(u_of(True), act, gin, gmag, dtype)
         res.update(out_max=maxerr_scaled(gu.float(), ref), nan=int(torch.isnan(gu.float()).sum()))
+        res["out_ulp"], res["out_ulp_bf16trip"] = ratio_pair(gu, ref, bound)
         if has(9):      # the BatchNorm backward sums of the STORED gradient
             r1, r2 = sums(gu.double())
             res.update(s1_rel=relerr(s1.sum(0), r1), s2_rel=relerr(s2.sum(0), r2))
@@ -540,6 +727,9 @@ def check_row_kernel(kernel, N, HW, C, args, ptrs, dtype=torch.bfloat16, seed=0)
         gm = gr.double() * ((out.double() > 0).double() if has(2) else 1.0)
         ref = cA.double() * gm + cB.double() * yd + cC.double()
         res.update(out_max=maxerr_scaled(dy.float(), ref), nan=int(torch.isnan(dy.float()).sum()))
+        # bn_bwd_apply_kernel (bn_act.cu:606): two fp32 fmaf's, one 16-bit store
+        mag = (cA.double() * gm).abs() + (cB.double() * yd).abs() + cC.double().abs()
+        res["out_ulp"], res["out_ulp_bf16trip"] = ratio_pair(dy, ref, elem_bound(ref, dtype, acc_term(mag, 2)))
     elif kernel == "dfd_se_bwd_reduce":
         da = (torch.randn(N, HW, C, device="cuda", generator=g) * 0.1).to(dtype)
         draw = torch.full((N, C), float("nan"), device="cuda")
@@ -916,7 +1106,8 @@ def check_conv_implicit(N, H, W, Cin, Cout, k=3, dtype=torch.bfloat16, seed=0, s
     wr = w.double().clone().requires_grad_(True)
     ref = F.conv2d(xr, wr, stride=stride, padding=pad)
     yf = y.float()
-    res = dict(fwd_max=maxerr_scaled(nchw(yf), ref.detach()), nan=int(torch.isnan(yf).sum()))
+    res = dict(fwd_max=maxerr_scaled(nchw(yf), ref.detach()), nan=int(torch.isnan(yf).sum()),
+               fwd_max_bf16trip=maxerr_scaled(nchw(bf16_trip(y).float()), ref.detach()))
     # the statistics-free launch (the eval form, and the stride-1 input gradient) stores the same bits
     y_ns = torch.full_like(y, float("nan"))
     _lib.call("dfd_conv_tc", P(x), P(wp), P(y_ns), N, H, W, Cin, Cout, k, stride, d, None, None, None, st())
@@ -942,6 +1133,7 @@ def check_conv_implicit(N, H, W, Cin, Cout, k=3, dtype=torch.bfloat16, seed=0, s
         _lib.call("dfd_conv_dgrad_s2_tc", P(dy), P(wpD), P(dx), N, H, W, Cin, Cout, d, st())
         torch.cuda.synchronize()
         res["dgrad_rel"] = relerr(nchw(dx.float()), xr.grad)
+        res["dgrad_max"], res["dgrad_max_bf16trip"] = _scaled_pair(dx, xr.grad)
         res["nan_b"] = int(torch.isnan(dx.float()).sum())
         # against the GEMM + col2im formulation (same products, different summation order inside a pixel: not bit-identical)
         dcols = torch.zeros(N * Ho * Wo, k * k * Cin, device="cuda", dtype=dtype)
@@ -950,11 +1142,13 @@ def check_conv_implicit(N, H, W, Cin, Cout, k=3, dtype=torch.bfloat16, seed=0, s
         _lib.call("dfd_col2im", P(dcols), None, P(dx2), N, H, W, Cin, k, 2, pad, d, st())
         torch.cuda.synchronize()
         res["dgrad_vs_col2im"] = relerr(dx.float(), dx2.float())
+        res["col2im_dgrad_max"], res["col2im_dgrad_max_bf16trip"] = _scaled_pair(dx2, xr.grad)
     if stride == 1:
         dx = torch.full((N, H, W, Cin), float("nan"), device="cuda", dtype=dtype)
         _lib.call("dfd_conv_tc", P(dy), P(wpD), P(dx), N, H, W, Cout, Cin, k, 1, d, None, None, None, st())
         torch.cuda.synchronize()
         res["dgrad_rel"] = relerr(nchw(dx.float()), xr.grad)
+        res["dgrad_max"], res["dgrad_max_bf16trip"] = _scaled_pair(dx, xr.grad)
         res["nan_b"] = int(torch.isnan(dx.float()).sum())
     # weight gradient (implicit too): packed [Cout][kh][kw][Cin] fp32 -> OIHW; atomic flush and workspace partials + ordered reduce
     Kw = k * k * Cin
@@ -996,8 +1190,11 @@ def check_conv1x1_dgrad_add(N, H, W, Cin, Cout, stride, dtype=torch.bfloat16, se
     exact = (dy.float().reshape(-1, Cout) @ w.float()).reshape(N, Ho, Wo, Cin)
     full = main.float().clone()
     full[:, ::stride, ::stride, :] += exact
+    full64 = main.double()          # fp64: the scaled bound of the tensor-core contractions
+    full64[:, ::stride, ::stride, :] += (dy.double().reshape(-1, Cout) @ w.double()).reshape(N, Ho, Wo, Cin)
+    out_max, out_max_trip = _scaled_pair(got, full64, to_nchw=False)
     return dict(mismatch=int((got.view(torch.int16) != ref.view(torch.int16)).sum()), rel=relerr(got.float(), full),
-                nan=int(torch.isnan(got.float()).sum()))
+                nan=int(torch.isnan(got.float()).sum()), out_max=out_max, out_max_bf16trip=out_max_trip)
 
 
 def check_relu_bn_bwd_reduce(N, HW, C, dtype=torch.bfloat16, seed=0, two=False):
@@ -1046,6 +1243,8 @@ def check_maxpool_relu_pool(N, H, W, C, dtype=torch.bfloat16, seed=0):
     bro = torch.zeros(N, Ho * Wo, C, device="cuda", dtype=dtype)
     _lib.call("dfd_pool_bwd", P(dp), P(bro), N, Ho * Wo, C, d, st())
     torch.cuda.synchronize()
-    return dict(fwd_exact=int((nchw(out.float()) != ref.detach()).sum()), bwd_rel=relerr(nchw(gx.float()), xr.grad),
+    bwd_ulp = maxpool_bwd_bound(gx, x, gy, lambda t: F.max_pool2d(t, 3, 2, 1), dtype)
+    return dict(bwd_ulp=bwd_ulp[0], bwd_ulp_bf16trip=bwd_ulp[1],
+                fwd_exact=int((nchw(out.float()) != ref.detach()).sum()), bwd_rel=relerr(nchw(gx.float()), xr.grad),
                 relu_mismatch=int((gm.float() != gy.float() * (out.float() > 0)).sum()),
                 pool_bwd_rel=relerr(bro.float(), (dp / (Ho * Wo)).to(dtype).float().unsqueeze(1).expand(N, Ho * Wo, C)))

@@ -11,6 +11,9 @@ plans launch have their own checkers in tests/family_checks.py and tests/tf_same
     full ones, and every output of two launches of a fixed-slot or order-deterministic reduction;
   * RED for fp32 reductions of 16-bit data (pools, dL/dgate), 1e-5 for BatchNorm-backward sums of the stored gradient (as
     test_bn_chain), F32 * 5 for the fp32 SE chains and weight gradients, and the depthwise bounds of _check_dwconv.
+In fp16 the 16-bit outputs are held to fp16 precision besides: the element-wise bounds of tests/gpu_checks.py (`*_ulp` <= 1)
+for the depthwise input gradients, the max-pool tails and gathered gradients, the average pool and col2im, each with the
+self-check that the same output rounded through bf16 violates it (test_plan_launches_gpu.fp16_ulp).
 Every output starts as NaN (an accumulated one from a known base).
 """
 import pytest
@@ -24,6 +27,7 @@ pytestmark = pytest.mark.gpu
 
 OUT16, RED, F32 = TPL.OUT16, TPL.RED, TPL.F32
 TDT = TPL.TDT
+fp16_ulp = TPL.fp16_ulp
 
 
 def _fc():
@@ -40,6 +44,8 @@ def _check_dwconv_relu(kw, dt):
     else:
         assert r["dgrad_rel"] < 8e-3 and r["wgrad_rel"] < RED, str(r)
     assert r["det_bitwise"] and r["det_vs_atomic"] < 1e-5 and r["det_gx_diff"] == 0.0, str(r)
+    if dt == "fp16":
+        fp16_ulp(r, "dgrad_ulp")
     if kw["bn"]:
         assert r["s1_rel"] < 1e-5 and r["s2_rel"] < 1e-5, str(r)
     if "ws_bytes" in kw:
@@ -51,12 +57,17 @@ def _check_bn_maxpool(kw, dt):
     assert r["nan"] == 0 and r["nan_b"] == 0 and r["out_max"] < OUT16 and r["noidx_mismatch"] == 0, str(r)
     assert r["idx_mismatch"] == 0 and r["tied_windows"] > 0, str(r)
     assert r["bwd_max"] < OUT16 and r["s1_rel"] < 1e-5 and r["s2_rel"] < 1e-5, str(r)
+    if dt == "fp16":
+        fp16_ulp(r, "out_ulp")
+        fp16_ulp(r, "bwd_ulp")
 
 
 def _check_maxpool_ceil(kw, dt):
     r = _fc().check_maxpool_ceil(kw["N"], kw["H"], kw["W"], kw["C"], dtype=TDT[dt])
     assert r["nan"] == 0 and r["nan_b"] == 0 and r["fwd_mismatch"] == 0 and r["idx_mismatch"] == 0, str(r)
     assert r["bwd_max"] < OUT16, str(r)
+    if dt == "fp16":
+        fp16_ulp(r, "bwd_ulp")
 
 
 def _check_pool_se_relu(kw, dt):
@@ -78,11 +89,16 @@ def _check_se_fc_wgrad(kw, dt):
 def _check_avgpool2(kw, dt):
     r = _fc().check_avgpool2(kw["N"], kw["H"], kw["W"], kw["C"], add=kw["add"], dtype=TDT[dt])
     assert r["nan"] == 0 and r["nan_b"] == 0 and r["fwd_max"] < OUT16 and r["bwd_max"] < OUT16, str(r)
+    if dt == "fp16":
+        fp16_ulp(r, "fwd_ulp")
+        fp16_ulp(r, "bwd_ulp")
 
 
 def _check_im2col(kw, dt):
     r = _fc().check_im2col(kw["N"], kw["H"], kw["W"], kw["C"], kw["k"], kw["s"], kw["pad"], add=kw["add"], dtype=TDT[dt])
     assert r["nan"] == 0 and r["cols_mismatch"] == 0 and r["nan_b"] == 0 and r["col2im_max"] < OUT16, str(r)
+    if dt == "fp16":
+        fp16_ulp(r, "col2im_ulp")
 
 
 def _check_dw_pad(kw, dt):
@@ -94,6 +110,8 @@ def _check_dw_pad(kw, dt):
     assert r["sum_rel"] < RED and r["sq_rel"] < RED and r["bwd_bitwise"], str(r)
     assert r.get("sym_fwd_mismatch", 0) == 0 and r.get("sym_bwd_mismatch", 0) == 0, str(r)
     assert r["dgrad_rel"] < (4e-3 if dt == "fp16" else 8e-3) and r["wgrad_rel"] < RED, str(r)
+    if dt == "fp16":
+        fp16_ulp(r, "dgrad_ulp")
     assert r["bs1_rel"] < RED and r["bs2_rel"] < RED, str(r)
     if "ws_bytes" in kw:
         assert r["ws_bytes"] == kw["ws_bytes"], (r["ws_bytes"], kw["ws_bytes"])

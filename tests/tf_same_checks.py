@@ -7,7 +7,7 @@ import torch
 import torch.nn.functional as F
 
 from deepfake_detection_b200 import _lib
-from gpu_checks import DT, P, nchw, relerr, st, stat_buf
+from gpu_checks import DT, P, U_OUT, ULP_IN, _u32, dw_dgrad_bound, dw_input_grad64, nchw, relerr, st, stat_buf, staged_dy
 
 
 def _same_pads(extent, k, s):
@@ -66,7 +66,7 @@ def check_dw_pad(N, H, W, C, k, s, pt, pl, dtype=torch.bfloat16, seed=0, bwd=Tru
     ref = F.conv2d(F.pad(a_q, padding), wr, stride=s, groups=C)
     # bound of gpu_checks.check_dwconv (there in fp32, here fp64): output half-ulp, the staged input's rounding and the
     # tanh.approx sigmoid (2^-11 absolute), fp32 accumulation of <= 25 taps
-    u_out, ulp_in = (2.0 ** -8, 2.0 ** -7) if dtype == torch.bfloat16 else (2.0 ** -11, 2.0 ** -10)
+    u_out, ulp_in = U_OUT[dtype], ULP_IN[dtype]
     with torch.no_grad():
         mag = F.conv2d(F.pad(a_q.abs(), padding), w.double().abs(), stride=s, groups=C)
         bound = u_out * ref.abs() + (ulp_in + 2.0 ** -20) * mag
@@ -114,6 +114,10 @@ def check_dw_pad(N, H, W, C, k, s, pt, pl, dtype=torch.bfloat16, seed=0, bwd=Tru
     # xr.grad = scale * (dgrad * swish'(u)); the kernel stores gu = dgrad * swish'(u), rounded to the 16-bit type
     gu_ref = xr.grad / scale.double().view(1, C, 1, 1)
     res["dgrad_rel"] = relerr(nchw(gx.double()), gu_ref)
+    # element-wise (gpu_checks.dw_dgrad_bound, MODE 1) on the dy tile exactly as the kernel stages it
+    ga64, mag64 = dw_input_grad64(staged_dy(gy, out, cA, cB, cC, dtype), w, H, W, k, s, (pt, pa, pl, qa))
+    res["dgrad_ulp"], res["dgrad_ulp_bf16trip"] = dw_dgrad_bound(gx, ga64, mag64, k, dtype, u=_u32(x, scale, shift).double())
+    del ga64, mag64
     res["wgrad_rel"] = relerr(dW.double(), wr.grad)
     gxd = gx.double()
     xhat = (x.double() - mean.double()) * rstd.double()
