@@ -98,6 +98,16 @@ SIGNATURES = {
     "dfd_maxpool_bwd": "ppp" "iiii" "i" "p",
     "dfd_maxpool_ceil_fwd": "ppp" "iiii" "i" "p",
     "dfd_maxpool_ceil_bwd": "ppp" "iiii" "i" "p",
+    "dfd_conv3x3_narrow_tc": "ppp" "iiiiii" "i" "pp" "i" "p",
+    "dfd_conv3x3_narrow_dgrad_tc": "ppp" "iiiii" "i" "p",
+    "dfd_bn_finalize_ld": "ppd" "ppppp" "ffiii" "ppppp",
+    "dfd_bn_relu_ld": "pi" "ppp" "li" "i" "p",
+    "dfd_copy_ld": "pi" "pi" "p" "li" "i" "pp" "i" "p",
+    "dfd_relu_bn_bwd_reduce_ld": "pppi" "pp" "li" "i" "ppp",
+    "dfd_relu_bn_bwd_apply_add_ld": "pppi" "ppp" "pi" "li" "i" "p",
+    "dfd_bn_relu_avgpool2": "pppp" "iiii" "i" "p",
+    "dfd_bn_relu_avgpool2_bwd_reduce": "pppppp" "iiii" "i" "ppp",
+    "dfd_bn_relu_avgpool2_bwd_apply": "ppppppp" "p" "iiii" "i" "p",
     "dfd_relu_bwd": "ppp" "li" "p",
     "dfd_pool_bwd": "pp" "ili" "i" "p",
     "dfd_gpool_bwd": "ppp" "ili" "ii" "p",

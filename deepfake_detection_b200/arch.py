@@ -21,6 +21,8 @@ BASELINE.json names; it builds no modules and owns no tensors.
   * SE-ResNets (seresnet18/34/50/101/152): dfd/timm/models/senet.py (SEModule :67-86, SEResNetBottleneck :141-163 with the
     stride on conv1, SEResNetBlock :190-223, SENet :226-396: layer0 7x7 s2 -> BN -> ReLU -> MaxPool2d(3, 2, ceil_mode=True),
     1x1 downsample, `last_linear`; entrypoints :399-461)
+  * DenseNet-121/161/169/201: dfd/timm/models/densenet.py (_DenseLayer :37-56, _DenseBlock :59-65, _Transition :62-70,
+    DenseNet :73-140, entrypoints :161-215)
 """
 import math
 import re
@@ -309,6 +311,67 @@ def xception_extents(H, W):
 
 
 # ----------------------------------------------------------------------------------------------
+# DenseNet
+# ----------------------------------------------------------------------------------------------
+
+@dataclass
+class DenseNetSpec:
+    """DenseNet-BC (densenet.py:73-140): stem conv0 7x7 s2 -> norm0 -> relu -> max-pool 3x3 s2 p1, dense blocks of layers
+    (norm1, relu, 1x1 conv1 to bn_size * k, norm2, relu, 3x3 conv2 to k, concatenated), transitions (norm, relu, 1x1 conv
+    halving the width, 2x2 average pool) between them, norm5 and the classifier."""
+    arch: str
+    in_chans: int
+    growth: int
+    init_features: int
+    block_config: Tuple[int, ...]
+    num_classes: int
+    input_size: Tuple[int, int, int] = (3, 224, 224)
+    bn_size: int = 4
+    family: str = "densenet"
+    global_pool: str = "avg"
+
+    @property
+    def block_widths(self):
+        """[(input width C0, final width)] of every dense block"""
+        out, c = [], self.init_features
+        for n in self.block_config:
+            out.append((c, c + n * self.growth))
+            c = (c + n * self.growth) // 2
+        return out
+
+    @property
+    def num_features(self):
+        return self.block_widths[-1][1]
+
+    @property
+    def pooled_features(self):
+        return self.num_features * pool_feat_mult(self.global_pool)
+
+
+# arch -> (growth k, init features, block config), densenet.py:161-215
+_DENSENET_DEFS = {
+    "densenet121": (32, 64, (6, 12, 24, 16)),
+    "densenet169": (32, 64, (6, 12, 32, 32)),
+    "densenet201": (32, 64, (6, 12, 48, 32)),
+    "densenet161": (48, 96, (6, 12, 36, 24)),
+}
+DENSENET_ARCHS = tuple(_DENSENET_DEFS)
+
+
+def densenet_extents(H, W):
+    """feature-map extents of a DenseNet at input H x W: [(h, w)] of the stem conv, then of every dense block (the stem
+    pool 3x3 s2 p1, then a floor-mode 2x2 average pool per transition)"""
+    h, w = conv_out(H, 7, 2, 3), conv_out(W, 7, 2, 3)
+    out = [(h, w)]
+    h, w = conv_out(h, 3, 2, 1), conv_out(w, 3, 2, 1)
+    out.append((h, w))
+    for _ in range(3):
+        h, w = h // 2, w // 2
+        out.append((h, w))
+    return out
+
+
+# ----------------------------------------------------------------------------------------------
 # registry of the variants on the hot path
 # ----------------------------------------------------------------------------------------------
 
@@ -356,6 +419,10 @@ def _base_spec(arch, num_classes, in_chans):
         return _xception_spec(arch, in_chans, num_classes)
     if arch in SENET_ARCHS:
         return _senet_spec(arch, in_chans, num_classes)
+    if arch in DENSENET_ARCHS:
+        k, c0, cfg = _DENSENET_DEFS[arch]
+        return DenseNetSpec(arch=arch, in_chans=in_chans, growth=k, init_features=c0, block_config=cfg,
+                            num_classes=num_classes)
     raise ValueError("arch %r is not on the native hot path (see SURVEY.md section 8)" % (arch,))
 
 
@@ -470,6 +537,25 @@ def state_entries(spec):
                 out += _bn_entries(p + ".bn2", b.cout)
         out.append(("conv_head.weight", (spec.num_features, spec.head_in, 1, 1), "conv_w"))
         out += _bn_entries("bn2", spec.num_features)
+        out.append(("classifier.weight", (spec.num_classes, spec.pooled_features), "fc_w"))
+        out.append(("classifier.bias", (spec.num_classes,), "fc_b"))
+    elif spec.family == "densenet":
+        c0, k = spec.init_features, spec.growth
+        out.append(("features.conv0.weight", (c0, spec.in_chans, 7, 7), "conv_w"))
+        out += _bn_entries("features.norm0", c0)
+        for b, (cin, cend) in enumerate(spec.block_widths):
+            for l in range(spec.block_config[b]):
+                p = "features.denseblock%d.denselayer%d" % (b + 1, l + 1)
+                c = cin + l * k
+                out += _bn_entries(p + ".norm1", c)
+                out.append((p + ".conv1.weight", (spec.bn_size * k, c, 1, 1), "conv_w"))
+                out += _bn_entries(p + ".norm2", spec.bn_size * k)
+                out.append((p + ".conv2.weight", (k, spec.bn_size * k, 3, 3), "conv_w"))
+            if b + 1 < len(spec.block_config):
+                p = "features.transition%d" % (b + 1)
+                out += _bn_entries(p + ".norm", cend)
+                out.append((p + ".conv.weight", (cend // 2, cend, 1, 1), "conv_w"))
+        out += _bn_entries("features.norm5", spec.num_features)
         out.append(("classifier.weight", (spec.num_classes, spec.pooled_features), "fc_w"))
         out.append(("classifier.bias", (spec.num_classes,), "fc_b"))
     elif spec.family == "xception":

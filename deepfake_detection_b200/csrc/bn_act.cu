@@ -153,7 +153,7 @@ __global__ void bn_finalize_kernel(const double* __restrict__ dsum, const double
                                    float* __restrict__ running_mean, float* __restrict__ running_var,
                                    long long* __restrict__ nbt, float momentum, float eps, int training, int C,
                                    float* __restrict__ scale, float* __restrict__ shift,
-                                   float* __restrict__ mean_out, float* __restrict__ rstd_out) {
+                                   float* __restrict__ mean_out, float* __restrict__ rstd_out, int ld) {
     int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c == 0 && training && nbt) *nbt += 1;
     if (c >= C) return;
@@ -161,8 +161,8 @@ __global__ void bn_finalize_kernel(const double* __restrict__ dsum, const double
     if (training) {
         // reciprocals come from the host: fp64 divisions are long dependent sequences on this part and these one-block
         // kernels sit on the critical path of every layer
-        double m = stat_total(dsum, C, c) * inv_count;
-        double v = stat_total(dsq, C, c) * inv_count - m * m;
+        double m = stat_total(dsum, ld, c) * inv_count;
+        double v = stat_total(dsq, ld, c) * inv_count - m * m;
         if (v < 0) v = 0;
         mean = (float)m;
         var = (float)v;
@@ -1326,6 +1326,204 @@ __global__ void maxpool_bn_bwd_reduce_kernel(const T* __restrict__ gy, const uns
     reduce_rows_and_emit(sm, a2, [&](int c, float v) { atomicAdd(p2 + c, (double)v); });
 }
 
+// ---------------------------------------------------------------------------------------------
+// DenseNet (densenet.py): channel slices of a dense block's concatenated NHWC buffer, whose rows hold `ld` channels. A thread
+// owns one 8-channel vector of the C channels a kernel touches (row geometry over the M = N*H*W rows, or per image for the
+// pools); channels outside them are neither read nor written.
+// ---------------------------------------------------------------------------------------------
+
+// norm1 + relu1 over the channel prefix [0, C): out[m, c] = round16(relu(x[m * ldx + c] * scale[c] + shift[c])), out contiguous
+template <typename T>
+__global__ void bn_relu_ld_kernel(const T* __restrict__ x, int ldx, const float* __restrict__ scale,
+                                  const float* __restrict__ shift, T* __restrict__ out, long long M, int rows_per_block) {
+    const int C = blockDim.x * 8, c0 = threadIdx.x * 8;
+    float sc[8], sh[8];
+    ldg_f8(scale + c0, sc);
+    ldg_f8(shift + c0, sh);
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    const long long r1 = min(r0 + rows_per_block, M);
+    for (long long r = r0 + threadIdx.y; r < r1; r += blockDim.y) {
+        float f[8];
+        unpack8<T>(ldg16(x + (size_t)r * ldx + c0), f);
+#pragma unroll
+        for (int i = 0; i < 8; i++) f[i] = fmaxf(fmaf(f[i], sc[i], sh[i]), 0.f);
+        stg16(out + (size_t)r * C + c0, pack8<T>(f));
+    }
+}
+
+// dst[m * ldd + c] = round16(src[m * lds + c] * mask[m * C + c]) (mask == NULL: a copy), plus the batch statistics of the
+// stored values into [DFD_STAT_SLOTS][stat_ld] (dsum == NULL: none)
+template <typename T>
+__global__ void copy_ld_kernel(const T* __restrict__ src, int lds, T* __restrict__ dst, int ldd, const float* __restrict__ mask,
+                               long long M, int rows_per_block, double* __restrict__ dsum, double* __restrict__ dsq, int stat_ld) {
+    extern __shared__ float sm[];
+    const int C = blockDim.x * 8, c0 = threadIdx.x * 8;
+    float s[8], q[8];
+#pragma unroll
+    for (int i = 0; i < 8; i++) { s[i] = 0.f; q[i] = 0.f; }
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    const long long r1 = min(r0 + rows_per_block, M);
+    for (long long r = r0 + threadIdx.y; r < r1; r += blockDim.y) {
+        uint4 v = ldg16(src + (size_t)r * lds + c0);
+        if (mask || dsum) {
+            float f[8];
+            unpack8<T>(v, f);
+            if (mask) {
+                float mk[8];
+                ldg_f8(mask + (size_t)r * C + c0, mk);
+#pragma unroll
+                for (int i = 0; i < 8; i++) f[i] = round_t<T>(f[i] * mk[i]);
+                v = pack8<T>(f);
+            }
+#pragma unroll
+            for (int i = 0; i < 8; i++) { s[i] += f[i]; q[i] = fmaf(f[i], f[i], q[i]); }
+        }
+        stg16(dst + (size_t)r * ldd + c0, v);
+    }
+    if (dsum) {
+        double* ps = stat_slot(dsum, stat_ld);
+        double* pq = stat_slot(dsq, stat_ld);
+        reduce_rows_and_emit(sm, s, [&](int c, float v) { atomicAdd(ps + c, (double)v); });
+        reduce_rows_and_emit(sm, q, [&](int c, float v) { atomicAdd(pq + c, (double)v); });
+    }
+}
+
+// backward of norm1 + relu1 over the prefix, a = the stored relu output (the ReLU mask is a > 0), g = dL/da (contiguous):
+//   APPLY == false: s1[c] += sum g * [a > 0], s2[c] += sum g * [a > 0] * (x - mean) * rstd
+//   APPLY == true : dx[m * ldd + c] = round16(dx + cA * g * [a > 0] + cB * x + cC)   (the prefix gradient ADDS the norm1 path)
+template <typename T, bool APPLY>
+__global__ void relu_bn_bwd_ld_kernel(const T* __restrict__ g, const T* __restrict__ a, const T* __restrict__ x, int ldx,
+                                      const float* __restrict__ p0, const float* __restrict__ p1, const float* __restrict__ p2,
+                                      T* dx, int ldd, long long M, int rows_per_block, double* __restrict__ s1,
+                                      double* __restrict__ s2) {
+    extern __shared__ float sm[];
+    const int C = blockDim.x * 8, c0 = threadIdx.x * 8;
+    float A[8], B[8], Cc[8], a1[8], a2[8];
+    ldg_f8(p0 + c0, A);                 // APPLY: cA, cB, cC; reduce: mean, rstd
+    ldg_f8(p1 + c0, B);
+    ldg_f8(APPLY ? p2 + c0 : nullptr, Cc);
+#pragma unroll
+    for (int i = 0; i < 8; i++) { a1[i] = 0.f; a2[i] = 0.f; }
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    const long long r1 = min(r0 + rows_per_block, M);
+    for (long long r = r0 + threadIdx.y; r < r1; r += blockDim.y) {
+        float gg[8], aa[8], xx[8];
+        unpack8<T>(ldg16(g + (size_t)r * C + c0), gg);
+        unpack8<T>(ldg16(a + (size_t)r * C + c0), aa);
+        unpack8<T>(ldg16(x + (size_t)r * ldx + c0), xx);
+#pragma unroll
+        for (int i = 0; i < 8; i++) gg[i] = aa[i] > 0.f ? gg[i] : 0.f;
+        if (APPLY) {
+            float d[8];
+            T* dp = dx + (size_t)r * ldd + c0;
+            unpack8<T>(*reinterpret_cast<const uint4*>(dp), d);
+#pragma unroll
+            for (int i = 0; i < 8; i++) d[i] += fmaf(A[i], gg[i], fmaf(B[i], xx[i], Cc[i]));
+            stg16(dp, pack8<T>(d));
+        } else {
+#pragma unroll
+            for (int i = 0; i < 8; i++) { a1[i] += gg[i]; a2[i] = fmaf(gg[i], (xx[i] - A[i]) * B[i], a2[i]); }
+        }
+    }
+    if (!APPLY) {
+        double* q1 = stat_slot(s1, C);
+        double* q2 = stat_slot(s2, C);
+        reduce_rows_and_emit(sm, a1, [&](int c, float v) { atomicAdd(q1 + c, (double)v); });
+        reduce_rows_and_emit(sm, a2, [&](int c, float v) { atomicAdd(q2 + c, (double)v); });
+    }
+}
+
+// DenseNet transition (densenet.py:62-70): norm, relu, then nn.AvgPool2d(2, 2) - floor mode, so an odd last row / column is
+// dropped - applied BEFORE the 1x1 conv (both are linear and the conv has no bias, so the order does not change the result and
+// the GEMM runs on a quarter of the pixels): y = round16(((r00 + r01) + r10) + r11) * 0.25), r = relu(scale * x + shift) in
+// fp32. Rows are output pixels; x is [N, H, W, C], y [N, H/2, W/2, C].
+template <typename T>
+__global__ void bn_relu_avgpool2_kernel(const T* __restrict__ x, const float* __restrict__ scale, const float* __restrict__ shift,
+                                        T* __restrict__ y, int H, int W, int Wo, long long hwo, int rows_per_block) {
+    const int C = blockDim.x * 8, c0 = threadIdx.x * 8;
+    float sc[8], sh[8];
+    ldg_f8(scale + c0, sc);
+    ldg_f8(shift + c0, sh);
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    const long long r1 = min(r0 + rows_per_block, hwo);
+    const T* img = x + (size_t)blockIdx.y * H * W * C + c0;
+    T* out = y + (size_t)blockIdx.y * hwo * C + c0;
+    for (long long r = r0 + threadIdx.y; r < r1; r += blockDim.y) {
+        const int oy = (int)(r / Wo), ox = (int)(r - (long long)oy * Wo);
+        const T* p = img + ((size_t)(2 * oy) * W + 2 * ox) * C;
+        uint4 raw[4] = {ldg16(p), ldg16(p + C), ldg16(p + (size_t)W * C), ldg16(p + (size_t)W * C + C)};
+        float acc[8];
+#pragma unroll
+        for (int t = 0; t < 4; t++) {
+            float f[8];
+            unpack8<T>(raw[t], f);
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                const float v = fmaxf(fmaf(f[i], sc[i], sh[i]), 0.f);
+                acc[i] = t == 0 ? v : acc[i] + v;
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < 8; i++) acc[i] *= 0.25f;
+        stg16(out + (size_t)r * C, pack8<T>(acc));
+    }
+}
+
+// backward of bn_relu_avgpool2_kernel; rows are INPUT pixels. gu = gp[y/2, x/2] * 0.25 * [scale * x + shift > 0] (0 in a
+// dropped last row / column):
+//   APPLY == false: s1[c] += sum gu, s2[c] += sum gu * (x - mean) * rstd
+//   APPLY == true : dx = round16(cA * gu + cB * x + cC) for every pixel (the dropped ones keep the BatchNorm terms)
+template <typename T, bool APPLY>
+__global__ void bn_relu_avgpool2_bwd_kernel(const T* __restrict__ gp, const T* __restrict__ x, const float* __restrict__ scale,
+                                            const float* __restrict__ shift, const float* __restrict__ p0,
+                                            const float* __restrict__ p1, const float* __restrict__ p2, T* __restrict__ dx,
+                                            int H, int W, int Ho, int Wo, int rows_per_block, double* __restrict__ s1,
+                                            double* __restrict__ s2) {
+    extern __shared__ float sm[];
+    const int C = blockDim.x * 8, c0 = threadIdx.x * 8;
+    const long long hw = (long long)H * W;
+    float sc[8], sh[8], A[8], B[8], Cc[8], a1[8], a2[8];
+    ldg_f8(scale + c0, sc);
+    ldg_f8(shift + c0, sh);
+    ldg_f8(p0 + c0, A);                 // APPLY: cA, cB, cC; reduce: mean, rstd
+    ldg_f8(p1 + c0, B);
+    ldg_f8(APPLY ? p2 + c0 : nullptr, Cc);
+#pragma unroll
+    for (int i = 0; i < 8; i++) { a1[i] = 0.f; a2[i] = 0.f; }
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    const long long r1 = min(r0 + rows_per_block, hw);
+    const size_t img = (size_t)blockIdx.y * hw * C + c0;
+    const T* g = gp + (size_t)blockIdx.y * Ho * Wo * C + c0;
+    for (long long r = r0 + threadIdx.y; r < r1; r += blockDim.y) {
+        const int iy = (int)(r / W), ix = (int)(r - (long long)iy * W);
+        const int oy = iy >> 1, ox = ix >> 1;
+        float xx[8], gg[8];
+        unpack8<T>(ldg16(x + img + (size_t)r * C), xx);
+        if (oy < Ho && ox < Wo) {
+            unpack8<T>(ldg16(g + ((size_t)oy * Wo + ox) * C), gg);
+#pragma unroll
+            for (int i = 0; i < 8; i++) gg[i] = fmaf(xx[i], sc[i], sh[i]) > 0.f ? gg[i] * 0.25f : 0.f;
+        } else {
+#pragma unroll
+            for (int i = 0; i < 8; i++) gg[i] = 0.f;
+        }
+        if (APPLY) {
+#pragma unroll
+            for (int i = 0; i < 8; i++) gg[i] = fmaf(A[i], gg[i], fmaf(B[i], xx[i], Cc[i]));
+            stg16(dx + img + (size_t)r * C, pack8<T>(gg));
+        } else {
+#pragma unroll
+            for (int i = 0; i < 8; i++) { a1[i] += gg[i]; a2[i] = fmaf(gg[i], (xx[i] - A[i]) * B[i], a2[i]); }
+        }
+    }
+    if (!APPLY) {
+        double* q1 = stat_slot(s1, C);
+        double* q2 = stat_slot(s2, C);
+        reduce_rows_and_emit(sm, a1, [&](int c, float v) { atomicAdd(q1 + c, (double)v); });
+        reduce_rows_and_emit(sm, a2, [&](int c, float v) { atomicAdd(q2 + c, (double)v); });
+    }
+}
+
 }  // namespace
 
 // =============================================================================================
@@ -1353,7 +1551,18 @@ int dfd_bn_finalize(const double* dsum, const double* dsq, double count, const f
     if (C <= 0) return dfd_set_error(DFD_ERR_ARG, "dfd_bn_finalize: C");
     bn_finalize_kernel<<<cdiv(C, 128), 128, 0, (cudaStream_t)stream>>>(dsum, dsq, 1.0 / count, count > 1 ? count / (count - 1) : 1.0, gamma, beta, running_mean,
                                                                          running_var, nbt, momentum, eps, training, C,
-                                                                         scale, shift, mean, rstd);
+                                                                         scale, shift, mean, rstd, C);
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+int dfd_bn_finalize_ld(const double* dsum, const double* dsq, double count, const float* gamma, const float* beta,
+                       float* running_mean, float* running_var, long long* nbt, float momentum, float eps,
+                       int training, int C, int ld, float* scale, float* shift, float* mean, float* rstd, void* stream) {
+    if (C <= 0 || ld < C) return dfd_set_error(DFD_ERR_ARG, "dfd_bn_finalize_ld: 0 < C <= ld");
+    bn_finalize_kernel<<<cdiv(C, 128), 128, 0, (cudaStream_t)stream>>>(dsum, dsq, 1.0 / count, count > 1 ? count / (count - 1) : 1.0, gamma, beta, running_mean,
+                                                                         running_var, nbt, momentum, eps, training, C,
+                                                                         scale, shift, mean, rstd, ld);
     DFD_LAUNCH_CHECK();
     return DFD_OK;
 }
@@ -1803,6 +2012,91 @@ int dfd_maxpool_bn_bwd_reduce(const void* gy, const void* idx, const void* y, co
     RowGeom g = make_geom(C, (long long)H * W, N);
     DISPATCH_T(dt, (maxpool_bn_bwd_reduce_kernel<T><<<g.grid, g.block, reduce_smem(g), (cudaStream_t)stream>>>((const T*)gy,
         (const unsigned char*)idx, (const T*)y, mean, rstd, (T*)gx, H, W, Ho, Wo, g.rows_per_block, s1, s2)));
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+// ---- DenseNet: see the kernels above ----
+static bool ld_ok(const void* p, int ld, int C) { return ld >= C && ld % 8 == 0 && ((uintptr_t)p & 15) == 0; }
+
+int dfd_bn_relu_ld(const void* x, int ldx, const float* scale, const float* shift, void* out, long long M, int C, int dt,
+                   void* stream) {
+    if (C % 8 || C <= 0 || M <= 0 || !ld_ok(x, ldx, C)) return dfd_set_error(DFD_ERR_ARG, "dfd_bn_relu_ld: C%8, ldx%8 >= C, sizes");
+    RowGeom g = make_geom(C, M, 1);
+    cudaStream_t st = (cudaStream_t)stream;
+    DISPATCH_T(dt, (bn_relu_ld_kernel<T><<<g.grid, g.block, 0, st>>>((const T*)x, ldx, scale, shift, (T*)out, M, g.rows_per_block)));
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+int dfd_copy_ld(const void* src, int lds, void* dst, int ldd, const float* mask, long long M, int C, int dt, double* dsum,
+                double* dsq, int stat_ld, void* stream) {
+    if (C % 8 || C <= 0 || M <= 0 || !ld_ok(src, lds, C) || !ld_ok(dst, ldd, C) || (dsum && stat_ld < C))
+        return dfd_set_error(DFD_ERR_ARG, "dfd_copy_ld: C%8, lds / ldd %8 >= C, stat_ld >= C, sizes");
+    RowGeom g = make_geom(C, M, 1);
+    cudaStream_t st = (cudaStream_t)stream;
+    DISPATCH_T(dt, (copy_ld_kernel<T><<<g.grid, g.block, reduce_smem(g), st>>>((const T*)src, lds, (T*)dst, ldd, mask, M,
+                                                                               g.rows_per_block, dsum, dsq, stat_ld)));
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+int dfd_relu_bn_bwd_reduce_ld(const void* g_, const void* a, const void* x, int ldx, const float* mean, const float* rstd,
+                              long long M, int C, int dt, double* s1, double* s2, void* stream) {
+    if (C % 8 || C <= 0 || M <= 0 || !ld_ok(x, ldx, C)) return dfd_set_error(DFD_ERR_ARG, "dfd_relu_bn_bwd_reduce_ld: C%8, ldx, sizes");
+    RowGeom g = make_geom(C, M, 1);
+    cudaStream_t st = (cudaStream_t)stream;
+    DISPATCH_T(dt, (relu_bn_bwd_ld_kernel<T, false><<<g.grid, g.block, reduce_smem(g), st>>>(
+                       (const T*)g_, (const T*)a, (const T*)x, ldx, mean, rstd, nullptr, nullptr, 0, M, g.rows_per_block, s1, s2)));
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+int dfd_relu_bn_bwd_apply_add_ld(const void* g_, const void* a, const void* x, int ldx, const float* cA, const float* cB,
+                                 const float* cC, void* dx, int ldd, long long M, int C, int dt, void* stream) {
+    if (C % 8 || C <= 0 || M <= 0 || !ld_ok(x, ldx, C) || !ld_ok(dx, ldd, C))
+        return dfd_set_error(DFD_ERR_ARG, "dfd_relu_bn_bwd_apply_add_ld: C%8, ldx / ldd, sizes");
+    RowGeom g = make_geom(C, M, 1);
+    cudaStream_t st = (cudaStream_t)stream;
+    DISPATCH_T(dt, (relu_bn_bwd_ld_kernel<T, true><<<g.grid, g.block, 0, st>>>(
+                       (const T*)g_, (const T*)a, (const T*)x, ldx, cA, cB, cC, (T*)dx, ldd, M, g.rows_per_block, nullptr, nullptr)));
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+int dfd_bn_relu_avgpool2(const void* x, const float* scale, const float* shift, void* y, int N, int H, int W, int C, int dt,
+                         void* stream) {
+    if (C % 8 || C <= 0 || N <= 0 || H < 2 || W < 2) return dfd_set_error(DFD_ERR_ARG, "dfd_bn_relu_avgpool2: C%8, H, W >= 2");
+    const int Wo = W / 2;
+    const long long hwo = (long long)(H / 2) * Wo;
+    RowGeom g = make_geom(C, hwo, N);
+    cudaStream_t st = (cudaStream_t)stream;
+    DISPATCH_T(dt, (bn_relu_avgpool2_kernel<T><<<g.grid, g.block, 0, st>>>((const T*)x, scale, shift, (T*)y, H, W, Wo, hwo,
+                                                                             g.rows_per_block)));
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+int dfd_bn_relu_avgpool2_bwd_reduce(const void* gp, const void* x, const float* scale, const float* shift, const float* mean,
+                                    const float* rstd, int N, int H, int W, int C, int dt, double* s1, double* s2, void* stream) {
+    if (C % 8 || C <= 0 || N <= 0 || H < 2 || W < 2) return dfd_set_error(DFD_ERR_ARG, "dfd_bn_relu_avgpool2_bwd_reduce: C%8, H, W >= 2");
+    RowGeom g = make_geom(C, (long long)H * W, N);
+    cudaStream_t st = (cudaStream_t)stream;
+    DISPATCH_T(dt, (bn_relu_avgpool2_bwd_kernel<T, false><<<g.grid, g.block, reduce_smem(g), st>>>(
+                       (const T*)gp, (const T*)x, scale, shift, mean, rstd, nullptr, nullptr, H, W, H / 2, W / 2, g.rows_per_block,
+                       s1, s2)));
+    DFD_LAUNCH_CHECK();
+    return DFD_OK;
+}
+
+int dfd_bn_relu_avgpool2_bwd_apply(const void* gp, const void* x, const float* scale, const float* shift, const float* cA,
+                                   const float* cB, const float* cC, void* dx, int N, int H, int W, int C, int dt, void* stream) {
+    if (C % 8 || C <= 0 || N <= 0 || H < 2 || W < 2) return dfd_set_error(DFD_ERR_ARG, "dfd_bn_relu_avgpool2_bwd_apply: C%8, H, W >= 2");
+    RowGeom g = make_geom(C, (long long)H * W, N);
+    cudaStream_t st = (cudaStream_t)stream;
+    DISPATCH_T(dt, (bn_relu_avgpool2_bwd_kernel<T, true><<<g.grid, g.block, 0, st>>>(
+                       (const T*)gp, (const T*)x, scale, shift, cA, cB, cC, (T*)dx, H, W, H / 2, W / 2, g.rows_per_block,
+                       nullptr, nullptr)));
     DFD_LAUNCH_CHECK();
     return DFD_OK;
 }

@@ -191,9 +191,56 @@ __device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t adesc, uint6
     }
 }
 
+// D[64 x 32] (+)= A[64 x 16] * B[16 x 32]: the narrow tiles of the DenseNet 3x3 convolutions (growth 32 / 48)
+template <typename T, int TA, int TB>
+__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    if constexpr (std::is_same<T, bf16>::value) {
+        asm volatile(
+            "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {"
+            "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15"
+            "}, %16, %17, p, 1, 1, %19, %20;\n}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
+    }
+    else {
+        asm volatile(
+            "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {"
+            "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15"
+            "}, %16, %17, p, 1, 1, %19, %20;\n}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
+    }
+}
+// D[64 x 48] (+)= A[64 x 16] * B[16 x 48]: the narrow tiles of the DenseNet 3x3 convolutions (growth 32 / 48)
+template <typename T, int TA, int TB>
+__device__ __forceinline__ void wgmma_n48(float (&d)[24], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    if constexpr (std::is_same<T, bf16>::value) {
+        asm volatile(
+            "{\n.reg .pred p;\nsetp.ne.b32 p, %26, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {"
+            "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23"
+            "}, %24, %25, p, 1, 1, %27, %28;\n}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+            : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
+    }
+    else {
+        asm volatile(
+            "{\n.reg .pred p;\nsetp.ne.b32 p, %26, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {"
+            "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23"
+            "}, %24, %25, p, 1, 1, %27, %28;\n}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+            : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
+    }
+}
+
 template <typename T, int BN, int TA, int TB>
 __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-    if constexpr (BN == 64) wgmma_n64<T, TA, TB>(d, adesc, bdesc, accumulate);
+    if constexpr (BN == 32) wgmma_n32<T, TA, TB>(d, adesc, bdesc, accumulate);
+    else if constexpr (BN == 48) wgmma_n48<T, TA, TB>(d, adesc, bdesc, accumulate);
+    else if constexpr (BN == 64) wgmma_n64<T, TA, TB>(d, adesc, bdesc, accumulate);
     else wgmma_n128<T, TA, TB>(d, adesc, bdesc, accumulate);
 }
 
@@ -247,9 +294,12 @@ struct TcParams {
     int dbg;              // debug switches (DFD_DBG env): 1 = skip TMA store, 2 = skip stats pass, 8 = A from L2
 };
 
-// BN = the MMA's N (64 or 128): the B tile holds block_n <= BN real rows; the MMA also reads the rows above them, whose
-// products land in accumulator columns that are never stored.
-template <typename T, int BN>
+// BN = the MMA's N (32, 48, 64 or 128): the B tile holds block_n <= BN real rows; the MMA also reads the rows above them,
+// whose products land in accumulator columns that are never stored.
+// KTAP (convolution mode only; 0 = 64-channel k-blocks): a k-block is ONE tap of a KTAP-channel input (32 or 48). The A box
+// is still 64 channels wide - TMA fills the channels past KTAP with zeros - but only KTAP / 16 MMAs are issued per k-block,
+// and the B box starts at column tap * KTAP of the [rows][taps * KTAP] packed weight (its columns past KTAP are not read).
+template <typename T, int BN, int KTAP = 0>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const __grid_constant__ CUtensorMap tmap_c, const TcParams p) {
@@ -299,6 +349,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                     int bk = kb * BLOCK_K;
                     if (p.conv) {
                         const int tap = kb / p.cv_cpb, cb = kb - tap * p.cv_cpb;
+                        if constexpr (KTAP != 0) bk = tap * KTAP;
                         int ax, ay;
                         if (p.cv_ntaps) {
                             ax = cx0 + p.cv_tox[tap]; ay = cy0 + p.cv_toy[tap];
@@ -358,7 +409,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                 const uint32_t a_addr = smem_addr(smem_a + (size_t)stage * a_bytes) + wg * 64 * 128;
                 const uint32_t b_addr = smem_addr(smem_b + (size_t)stage * b_stride);
                 const int krem = p.K - kb * BLOCK_K;
-                const int nk = krem >= BLOCK_K ? BLOCK_K / MMA_K : (krem + MMA_K - 1) / MMA_K;
+                const int nk = KTAP != 0 ? KTAP / MMA_K : krem >= BLOCK_K ? BLOCK_K / MMA_K : (krem + MMA_K - 1) / MMA_K;
                 fence_acc(acc);
                 wgmma_fence();
                 for (int k = 0; k < nk; k++)
@@ -375,7 +426,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
             fence_acc(acc);
             if ((et & 127) == 0) mbar_arrive(empty_bar + prev_stage);
 #pragma unroll
-            for (int s = 0; s < BN / SLAB; s++) {
+            for (int s = 0; s < (BN + SLAB - 1) / SLAB; s++) {
                 if (s >= nslabs) break;
                 uint8_t* cbuf = smem_c + (size_t)(slab_count & 1) * (BLOCK_M * SLAB * 2);
                 const int ncols = min(SLAB, p.block_n - s * SLAB);
@@ -383,7 +434,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                 epi_barrier();
 #pragma unroll
                 for (int j = 0; j < SLAB / 8; j++) {
-                    if (j * 8 < ncols) {
+                    if (s * SLAB + j * 8 < BN && j * 8 < ncols) {
                         const int i = (s * (SLAB / 8) + j) * 4;
                         // logical 16-byte chunk j of a 128-byte row sits at chunk j ^ (row & 7) (r0 and r0 + 8 share row & 7)
                         const uint32_t off = ((j ^ (r0 & 7)) << 4) + cq * 2;
@@ -667,12 +718,12 @@ static int make_map_nhwc(CUtensorMap* m, const void* base, int N, int H, int W, 
     return DFD_OK;
 }
 
-template <typename T, int BN>
+template <typename T, int BN, int KTAP = 0>
 static void launch_tc_kernel(int grid, size_t smem, cudaStream_t st, const CUtensorMap& ma, const CUtensorMap& mb,
                              const CUtensorMap& mc, const TcParams& p) {
     static bool attr = false;
-    if (!attr) { cudaFuncSetAttribute(gemm_tc_kernel<T, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BUDGET); attr = true; }
-    gemm_tc_kernel<T, BN><<<grid, NUM_THREADS, smem, st>>>(ma, mb, mc, p);
+    if (!attr) { cudaFuncSetAttribute(gemm_tc_kernel<T, BN, KTAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BUDGET); attr = true; }
+    gemm_tc_kernel<T, BN, KTAP><<<grid, NUM_THREADS, smem, st>>>(ma, mb, mc, p);
 }
 
 template <typename T, int BN>
@@ -683,9 +734,12 @@ static void launch_wgrad_kernel(dim3 grid, size_t smem, cudaStream_t st, const C
     wgrad_tc_kernel<T, BN><<<grid, WG_THREADS, smem, st>>>(mg, mx, dW, p);
 }
 
-// pipeline depth, shared memory and grid of gemm_tc_kernel for the tile shape in p, then the launch
-static int run_tc(TcParams& p, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mc, void* stream, const char* what) {
-    const int bn = p.block_n <= 64 ? 64 : 128;
+// pipeline depth, shared memory and grid of gemm_tc_kernel for the tile shape in p, then the launch. narrow = the MMA N
+// follows block_n down to 32 / 48 (the DenseNet entry points; the others keep 64-wide MMAs at block_n <= 64); ktap: see
+// gemm_tc_kernel
+static int run_tc(TcParams& p, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mc, void* stream, const char* what,
+                  bool narrow = false, int ktap = 0) {
+    const int bn = narrow && p.block_n <= 32 ? 32 : narrow && p.block_n <= 48 ? 48 : p.block_n <= 64 ? 64 : 128;
     p.dbg = 0;
     { const char* e = getenv("DFD_DBG"); if (e) p.dbg = atoi(e); }
     const int stage_bytes = BLOCK_M * BLOCK_K * 2 + bn * BLOCK_K * 2;
@@ -701,11 +755,23 @@ static int run_tc(TcParams& p, const CUtensorMap& ma, const CUtensorMap& mb, con
     int grid = p.num_m_tiles * p.num_n_tiles;
     if (grid > sms) grid = sms;
     cudaStream_t st = (cudaStream_t)stream;
-    if (p.is_bf16) {
-        if (bn == 64) launch_tc_kernel<bf16, 64>(grid, smem, st, ma, mb, mc, p);
+    if (ktap == 32 && bn == 128) {
+        if (p.is_bf16) launch_tc_kernel<bf16, 128, 32>(grid, smem, st, ma, mb, mc, p);
+        else launch_tc_kernel<__half, 128, 32>(grid, smem, st, ma, mb, mc, p);
+    } else if (ktap == 48 && bn == 128) {
+        if (p.is_bf16) launch_tc_kernel<bf16, 128, 48>(grid, smem, st, ma, mb, mc, p);
+        else launch_tc_kernel<__half, 128, 48>(grid, smem, st, ma, mb, mc, p);
+    } else if (ktap) {
+        return dfd_set_error(DFD_ERR_UNSUPPORTED, what);
+    } else if (p.is_bf16) {
+        if (bn == 32) launch_tc_kernel<bf16, 32>(grid, smem, st, ma, mb, mc, p);
+        else if (bn == 48) launch_tc_kernel<bf16, 48>(grid, smem, st, ma, mb, mc, p);
+        else if (bn == 64) launch_tc_kernel<bf16, 64>(grid, smem, st, ma, mb, mc, p);
         else launch_tc_kernel<bf16, 128>(grid, smem, st, ma, mb, mc, p);
     } else {
-        if (bn == 64) launch_tc_kernel<__half, 64>(grid, smem, st, ma, mb, mc, p);
+        if (bn == 32) launch_tc_kernel<__half, 32>(grid, smem, st, ma, mb, mc, p);
+        else if (bn == 48) launch_tc_kernel<__half, 48>(grid, smem, st, ma, mb, mc, p);
+        else if (bn == 64) launch_tc_kernel<__half, 64>(grid, smem, st, ma, mb, mc, p);
         else launch_tc_kernel<__half, 128>(grid, smem, st, ma, mb, mc, p);
     }
     DFD_LAUNCH_CHECK();
@@ -717,7 +783,8 @@ static int run_tc(TcParams& p, const CUtensorMap& ma, const CUtensorMap& mb, con
 struct ConvTaps { int n, ox[9], oy[9], kidx[9]; };
 static int launch_conv_tc(const void* x, const void* wpk, void* y, int N, int Hin, int Win, int Cin, int Cout, int k, int S,
                           int dt, double* dsum, double* dsq, const void* fin, void* stream, const ConvTaps* taps = nullptr,
-                          int outH = 0, int outW = 0, const PixelView* out_view = nullptr, int wcols = 0, int accum = 0) {
+                          int outH = 0, int outW = 0, const PixelView* out_view = nullptr, int wcols = 0, int accum = 0,
+                          int ktap = 0, int ldy = 0, int stat_ld = 0) {
     TcParams p;
     p.fin = (const BnFinDesc*)fin;
     p.conv = 1;
@@ -739,10 +806,10 @@ static int launch_conv_tc(const void* x, const void* wpk, void* y, int N, int Hi
     p.cv_TW = TW; p.cv_TH = TH; p.cv_TN = TN; p.cv_rows = TW * TH * TN;
     p.cv_tiles_x = (W + TW - 1) / TW; p.cv_tiles_y = (H + TH - 1) / TH;
     p.cv_W = W; p.cv_H = H; p.cv_N = N;
-    p.cv_k = k; p.cv_pad = (k - 1) / 2; p.cv_cpb = Cin / BLOCK_K;
+    p.cv_k = k; p.cv_pad = (k - 1) / 2; p.cv_cpb = ktap ? 1 : Cin / BLOCK_K;
     const int K = taps ? wcols : k * k * Cin;          // columns of the packed weight matrix
     p.M = N * H * W; p.N = Cout; p.K = K;
-    p.stat_n = Cout;
+    p.stat_n = stat_ld ? stat_ld : Cout;
     p.is_bf16 = dt == DFD_DT_BF16;
     p.block_n = Cout <= MAX_BLOCK_N ? ((Cout + 15) / 16) * 16 : MAX_BLOCK_N;
     p.num_m_tiles = p.cv_tiles_x * p.cv_tiles_y * ((N + TN - 1) / TN);
@@ -753,8 +820,10 @@ static int launch_conv_tc(const void* x, const void* wpk, void* y, int N, int Hi
     int rc;
     if ((rc = make_map_nhwc(&ma, x, N, Hin, Win, Cin, TW, TH, TN, p.is_bf16, S))) return rc;
     if ((rc = make_map(&mb, wpk, Cout, K, p.block_n, p.is_bf16))) return rc;
-    if ((rc = make_map_nhwc(&mc, y, N, H, W, Cout, TW, TH, TN, p.is_bf16, 1, out_view))) return rc;
-    return run_tc(p, ma, mb, mc, stream, "dfd_conv_tc: smem");
+    // ldy: the output is the channel slice [0, Cout) of a tensor with ldy channels per pixel (the store clips at Cout)
+    PixelView slice = {(long long)ldy * 2, (long long)W * ldy * 2, (long long)H * W * ldy * 2};
+    if ((rc = make_map_nhwc(&mc, y, N, H, W, Cout, TW, TH, TN, p.is_bf16, 1, ldy ? &slice : out_view))) return rc;
+    return run_tc(p, ma, mb, mc, stream, "dfd_conv_tc: smem", ldy != 0 || ktap != 0, ktap);
 }
 
 // C[M,N] = A[M,K] * B[N,K]^T; statistics of output column c go to channel c % stat_n
@@ -835,6 +904,33 @@ int dfd_conv_tc(const void* x, const void* wpk, void* y, int N, int H, int W, in
         return dfd_set_error(DFD_ERR_ARG, "dfd_conv_tc: Cin % 64, Cout % 64, k in {1,3,5,7}, stride in {1,2}");
     if (dt != DFD_DT_BF16 && dt != DFD_DT_FP16) return dfd_set_error(DFD_ERR_ARG, "dfd_conv_tc: dtype");
     return launch_conv_tc(x, wpk, y, N, H, W, Cin, Cout, k, stride, dt, dsum, dsq, fin, stream);
+}
+
+// DenseNet's 3x3 convolution (densenet.py:44-45: bn_size * k -> k channels, stride 1, padding 1) for growth k = Cout in
+// {32, 48}: the implicit GEMM above with 32- / 48-wide MMAs, whose output is the channel slice at y of a tensor with ldy
+// channels per pixel (the dense block's concatenated buffer). The store goes through a tensor map over that slice alone,
+// so no channel outside it is ever written. dsum / dsq: [DFD_STAT_SLOTS][stat_ld] statistics, offset to the slice's first
+// channel (NULL: none).
+int dfd_conv3x3_narrow_tc(const void* x, const void* wpk, void* y, int N, int H, int W, int Cin, int Cout, int ldy, int dt,
+                          double* dsum, double* dsq, int stat_ld, void* stream) {
+    if (N <= 0 || H <= 0 || W <= 0 || Cin <= 0 || (Cin % 64) || (Cout != 32 && Cout != 48) || ldy < Cout || (ldy % 8) ||
+        ((uintptr_t)y & 15) || (dsum && stat_ld < Cout))
+        return dfd_set_error(DFD_ERR_ARG, "dfd_conv3x3_narrow_tc: Cin % 64, Cout in {32, 48}, ldy % 8 >= Cout, y 16-byte aligned");
+    if (dt != DFD_DT_BF16 && dt != DFD_DT_FP16) return dfd_set_error(DFD_ERR_ARG, "dfd_conv3x3_narrow_tc: dtype");
+    return launch_conv_tc(x, wpk, y, N, H, W, Cin, Cout, 3, 1, dt, dsum, dsq, nullptr, stream, nullptr, 0, 0, nullptr, 0, 0, 0,
+                          ldy, stat_ld ? stat_ld : Cout);
+}
+
+// Input gradient of dfd_conv3x3_narrow_tc: dx[N,H,W,Cin] = conv3x3(dy[N,H,W,Cout], tap-flipped wpkD [Cin][kh'][kw'][Cout]),
+// dy contiguous with Cout in {32, 48} channels. Each k-block is one tap of Cout channels (KTAP): no padding of K, so no MMA
+// multiplies a padded zero.
+int dfd_conv3x3_narrow_dgrad_tc(const void* dy, const void* wpkD, void* dx, int N, int H, int W, int Cin, int Cout, int dt,
+                                void* stream) {
+    if (N <= 0 || H <= 0 || W <= 0 || Cin < 128 || (Cin % 64) || (Cout != 32 && Cout != 48))
+        return dfd_set_error(DFD_ERR_ARG, "dfd_conv3x3_narrow_dgrad_tc: Cin % 64 >= 128, Cout in {32, 48}");
+    if (dt != DFD_DT_BF16 && dt != DFD_DT_FP16) return dfd_set_error(DFD_ERR_ARG, "dfd_conv3x3_narrow_dgrad_tc: dtype");
+    return launch_conv_tc(dy, wpkD, dx, N, H, W, Cout, Cin, 3, 1, dt, nullptr, nullptr, nullptr, stream, nullptr, 0, 0, nullptr, 0,
+                          0, Cout);
 }
 
 // Input gradient of a 3x3, stride-2, padding-1 convolution as FOUR implicit GEMMs, one per parity class (py, px) of the input

@@ -7,7 +7,7 @@ This is the host side of the hot path (dfd/runners/train.py:610-649): given an a
   * builds, once, the ordered list of C-ABI calls ("plan") for forward, backward and the optimizer, and
   * replays the plan on the caller's current CUDA stream (optionally captured into a CUDA graph).
 
-The family's plan builder (engine_efficientnet, engine_resnet, engine_xception) lays out the activations
+The family's plan builder (engine_efficientnet, engine_resnet, engine_xception, engine_densenet) lays out the activations
 and lists the ops; the conventions every plan shares (BatchNorm statistics, finalisation and backward apply, the mask
 generators, the deterministic weight-gradient reduce, the stem as im2col + GEMM, the pooled classifier head, the packed k x k
 weights, validation against the ABI table) are the plan helpers of this class.
@@ -63,7 +63,8 @@ class Engine:
                                    "there is no CPU path")
         self.L = _lib.lib()
         self.spec = spec = get_spec(arch, num_classes=num_classes, in_chans=in_chans, global_pool=global_pool)
-        self.cls_name = "classifier" if spec.family == "efficientnet" else (spec.cls_name if spec.family == "resnet" else "fc")
+        self.cls_name = "classifier" if spec.family in ("efficientnet", "densenet") else (
+            spec.cls_name if spec.family == "resnet" else "fc")
         self.device = torch.device(device if device is not None else "cuda:%d" % torch.cuda.current_device())
         self.N = int(batch)
         self.H = int(height or spec.input_size[1])
@@ -87,10 +88,11 @@ class Engine:
             if dist.is_available() and dist.is_initialized():
                 self.sync_world = dist.get_world_size()
             self.sync_bn = self.sync_world > 1
-        if self.sync_bn and spec.family in ("resnet", "xception"):
+        if self.sync_bn and spec.family in ("resnet", "xception", "densenet"):
             raise _lib.NativeError("sync_bn over %d ranks: the %s plan has no synchronised BatchNorm (only the "
                                    "EfficientNet plan all-reduces its batch statistics)"
-                                   % (self.sync_world, "ResNet" if spec.family == "resnet" else "Xception"))
+                                   % (self.sync_world, {"resnet": "ResNet", "xception": "Xception",
+                                                        "densenet": "DenseNet"}[spec.family]))
         self.bn_momentum = float(bn_momentum)
         self.bn_eps = float(bn_eps)
         # "tc": wgmma GEMMs and implicit convolutions; "mma": the mma.sync cross-check path (GEMMs over im2col columns)
@@ -421,12 +423,15 @@ class Engine:
         wname, Cout, _, taps, Kp = self._stem
         return ("dfd_unpad_grad", (_ptr(self.stem_gpad), self._g32(wname), Cout, taps, Kp))
 
-    def _alloc_bn(self, bn_specs):
-        """per-BN pointers into the parameter / running-stat arenas + the per-step statistic and coefficient arenas"""
+    def _alloc_bn(self, bn_specs, extra_stats=0):
+        """per-BN pointers into the parameter / running-stat arenas + the per-step statistic and coefficient arenas.
+        extra_stats: fp64 values appended to the statistics arena (zeroed with it every step) for statistics that several
+        BatchNorms share; they start at element 4 * S * tot_c + 8, returned"""
         dev, S = self.device, self.L.stat_slots
         tot_c = sum((c + 3) // 4 * 4 for _, c in bn_specs)
         self.bnstate = torch.zeros(7 * tot_c, dtype=torch.float32, device=dev)      # scale shift mean rstd cA cB cC
-        self.stats = torch.zeros(4 * S * tot_c + 8, dtype=torch.float64, device=dev)  # fsum fsq bs1 bs2 (+ loss/correct)
+        # fsum fsq bs1 bs2 (+ loss/correct)
+        self.stats = torch.zeros(4 * S * tot_c + 8 + extra_stats, dtype=torch.float64, device=dev)
         self.bns = {}
         co = 0
         for name, c in bn_specs:
@@ -449,16 +454,18 @@ class Engine:
             co += (c + 3) // 4 * 4
             self.bns[name] = bn
         self.scalars = torch.zeros(4, dtype=torch.float32, device=dev)     # loss_acc, correct_acc, (spare)
+        return 4 * S * tot_c + 8
 
 
     def _build(self):
+        from .engine_densenet import build_densenet
         from .engine_efficientnet import build_efficientnet
         from .engine_resnet import build_resnet
         from .engine_xception import build_xception
         self._keep, self.acts = [], {}
         self._masks = []            # dfd_rng_masks table: (tensor, rows, width, keep_prob), see _mask_head
         self.x_in = torch.zeros(self.N, self.spec.in_chans, self.H, self.W, dtype=self.tdtype, device=self.device)
-        {"resnet": build_resnet, "xception": build_xception}.get(self.spec.family, build_efficientnet)(self)
+        {"resnet": build_resnet, "xception": build_xception, "densenet": build_densenet}.get(self.spec.family, build_efficientnet)(self)
 
     # ---- plan helpers shared by the family builders ---------------------------------------------------------------------
     # pointers to a parameter's fp32 value and gradient, its 16-bit copy and the transposed 16-bit copy of a 1x1 weight
@@ -624,7 +631,7 @@ class Engine:
             if training:
                 args[2] = args[2] * self.sync_world          # global element count behind the summed statistics
             name = "dfd_bn_finalize"
-        if name == "dfd_bn_finalize":
+        if name in ("dfd_bn_finalize", "dfd_bn_finalize_ld"):
             args = tuple((1 if training else 0) if a == "TRAINING" else a for a in args)
             if not training:
                 args = (None, None) + args[2:]

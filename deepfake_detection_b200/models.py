@@ -18,7 +18,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .arch import RESNET_ARCHS, SENET_ARCHS, SUPPORTED_ARCHS, TF_ARCHS, TF_POOL_CROP, XCEPTION_ARCHS, get_spec, state_entries
+from .arch import DENSENET_ARCHS, RESNET_ARCHS, SENET_ARCHS, SUPPORTED_ARCHS, TF_ARCHS, TF_POOL_CROP, XCEPTION_ARCHS, get_spec, state_entries
 from .engine import Engine
 
 _DEFAULT_CFG = dict(num_classes=1000, pool_size=(7, 7), crop_pct=0.875, interpolation="bicubic",
@@ -77,13 +77,15 @@ def init_state_dict(spec, seed=None):
     Xception: xception.py:171-177 (every nn.Conv2d, depthwise included, kaiming_normal fan_out = out_channels * k * k - torch
     does not divide by the groups - BN 1 / 0, nn.Linear's default init for fc);
     SE-ResNet: senet.py:59-64,344-345 (every nn.Conv2d, the SE FCs included, kaiming_normal fan_out, BN 1 / 0 with no zero-init
-    of the last gamma; the SE biases keep nn.Conv2d's default U(+-1/sqrt(fan_in)) and last_linear nn.Linear's default)."""
+    of the last gamma; the SE biases keep nn.Conv2d's default U(+-1/sqrt(fan_in)) and last_linear nn.Linear's default);
+    DenseNet: densenet.py has no init loop, so PyTorch's defaults hold: nn.Conv2d U(+-1/sqrt(fan_in)), BN 1 / 0, nn.Linear's
+    default for the classifier."""
     import math
     g = torch.Generator(device="cpu").manual_seed((torch.initial_seed() if seed is None else seed) % (2 ** 31))
     sd = OrderedDict()
     resnet = spec.family == "resnet"
     senet = resnet and spec.naming == "senet"
-    fan_in_fc = spec.family in ("resnet", "xception")
+    fan_in_fc = spec.family in ("resnet", "xception", "densenet")
     last_bn = set()
     if resnet and not senet:
         for b in spec.blocks:
@@ -98,6 +100,10 @@ def init_state_dict(spec, seed=None):
             continue
         if senet and role == "se_b":
             r = 1.0 / math.sqrt(sd[name[: -len("bias")] + "weight"].shape[1])     # fan_in of the 1x1 FC
+            sd[name] = (torch.rand(shape, generator=g) * 2 - 1) * r
+            continue
+        if role == "conv_w" and spec.family == "densenet":
+            r = 1.0 / math.sqrt(shape[1] * shape[2] * shape[3])
             sd[name] = (torch.rand(shape, generator=g) * 2 - 1) * r
             continue
         if role in ("conv_w", "dw_w", "se_w"):
@@ -159,6 +165,8 @@ class NativeModel(nn.Module):
             self.default_cfg.update(interpolation="bicubic" if arch in _RESNET_BICUBIC else "bilinear")
         if arch in XCEPTION_ARCHS:
             self.default_cfg.update(_XCEPTION_CFG)
+        if arch in DENSENET_ARCHS:  # densenet.py:20-26
+            self.default_cfg.update(first_conv="features.conv0", classifier="classifier")
         self._engines = OrderedDict()
         self._primary = None
         self._pending_state = None
@@ -292,12 +300,12 @@ def create_model(model_name, pretrained=False, num_classes=1000, in_chans=3, che
     """dfd/timm/models/factory.py:8-64 for the architectures on the native hot path."""
     if pretrained:
         raise _lib.NativeError("pretrained weights need network access; load a checkpoint instead")
-    if model_name not in SUPPORTED_ARCHS + TF_ARCHS + RESNET_ARCHS + XCEPTION_ARCHS + SENET_ARCHS:
+    if model_name not in SUPPORTED_ARCHS + TF_ARCHS + RESNET_ARCHS + XCEPTION_ARCHS + SENET_ARCHS + DENSENET_ARCHS:
         raise RuntimeError("Unknown model (%s)" % model_name)       # factory.py:56
-    if model_name in XCEPTION_ARCHS + SENET_ARCHS:
+    if model_name in XCEPTION_ARCHS + SENET_ARCHS + DENSENET_ARCHS:
         # factory.py:31-45: the BatchNorm arguments are dropped for every model that is not an EfficientNet, and
-        # drop_block_rate / drop_path_rate when they are None; anything else reaches Xception.__init__ / SENet.__init__, which
-        # refuse it
+        # drop_block_rate / drop_path_rate when they are None; anything else reaches Xception.__init__ / SENet.__init__ /
+        # DenseNet.__init__, which refuse it
         for k in ("bn_tf", "bn_momentum", "bn_eps"):
             kwargs.pop(k, None)
         dc = kwargs.pop("drop_connect_rate", None)

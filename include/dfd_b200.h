@@ -422,6 +422,47 @@ int dfd_update_loss_scale(int* flag, float* scale, int* good_steps, int interval
 /* table: device array of { const void* src; void* dst; int O; int I; } — dst[I,O] = transpose(src[O,I]) */
 int dfd_transpose_weights(const void* table, int count, int dt, void* stream);
 
+/* ---- DenseNet (densenet.py): narrow 3x3 convolutions and channel slices of a dense block's concatenated NHWC buffer ------
+ * A dense block keeps ONE buffer whose rows hold ld channels; layer l writes its k new channels at [C0 + l*k, C0 + (l+1)*k).
+ * Its batch statistics live in one [DFD_STAT_SLOTS][ld] pair per block, each channel reduced once, when it is produced. */
+/* conv2 of a dense layer (densenet.py:44-45): 3x3, stride 1, padding 1, Cin % 64 == 0 -> Cout in {32, 48} channels, the
+ * wgmma implicit GEMM of dfd_conv_tc with 32- / 48-wide tiles. y points at the output slice's first channel in a tensor of
+ * ldy channels per pixel (16-byte aligned, ldy % 8 == 0); no channel outside [0, Cout) of it is written. dsum / dsq: the
+ * [DFD_STAT_SLOTS][stat_ld] statistics offset to the same channel (NULL: none). */
+int dfd_conv3x3_narrow_tc(const void* x, const void* wpk, void* y, int N, int H, int W, int Cin, int Cout, int ldy, int dt,
+                          double* dsum, double* dsq, int stat_ld, void* stream);
+/* its input gradient: dx [N,H,W,Cin] = conv3x3(dy [N,H,W,Cout] contiguous, wpkD = the tap-flipped [Cin][kh'][kw'][Cout]);
+ * one k-block per tap of Cout channels (no zero padding of K); Cin % 64 == 0, Cin >= 128 */
+int dfd_conv3x3_narrow_dgrad_tc(const void* dy, const void* wpkD, void* dx, int N, int H, int W, int Cin, int Cout, int dt,
+                                void* stream);
+/* dfd_bn_finalize over channels [0, C) of statistics laid out [DFD_STAT_SLOTS][ld] (a prefix of a dense block's statistics) */
+int dfd_bn_finalize_ld(const double* dsum, const double* dsq, double count, const float* gamma, const float* beta,
+                       float* running_mean, float* running_var, long long* num_batches_tracked, float momentum,
+                       float eps, int training, int C, int ld, float* scale, float* shift, float* mean, float* rstd,
+                       void* stream);
+/* norm1 + relu1 over a prefix: out [M, C] = relu(scale * x[m * ldx + c] + shift) */
+int dfd_bn_relu_ld(const void* x, int ldx, const float* scale, const float* shift, void* out, long long M, int C, int dt,
+                   void* stream);
+/* dst[m * ldd + c] = src[m * lds + c] * mask[m * C + c] (mask: fp32 [M, C] already divided by keep, NULL: a plain copy), plus
+ * the statistics of the stored values into [DFD_STAT_SLOTS][stat_ld] (dsum NULL: none) */
+int dfd_copy_ld(const void* src, int lds, void* dst, int ldd, const float* mask, long long M, int C, int dt, double* dsum,
+                double* dsq, int stat_ld, void* stream);
+/* backward of dfd_bn_relu_ld from g = dL/da [M, C] and a = its stored output (ReLU mask a > 0): the sums s1 = sum g',
+ * s2 = sum g' * (x - mean) * rstd of dfd_bn_bwd_finalize, then dx[m * ldd + c] += cA * g' + cB * x + cC */
+int dfd_relu_bn_bwd_reduce_ld(const void* g, const void* a, const void* x, int ldx, const float* mean, const float* rstd,
+                              long long M, int C, int dt, double* s1, double* s2, void* stream);
+int dfd_relu_bn_bwd_apply_add_ld(const void* g, const void* a, const void* x, int ldx, const float* cA, const float* cB,
+                                 const float* cC, void* dx, int ldd, long long M, int C, int dt, void* stream);
+/* transition (densenet.py:62-70): y [N, H/2, W/2, C] = avgpool2x2_floor(relu(scale * x + shift)), x [N, H, W, C]; the 1x1
+ * conv runs after the pool. Backward: the sums of dfd_bn_bwd_finalize, then dx [N, H, W, C] = cA * g' + cB * x + cC for every
+ * pixel, g' = gp[y/2, x/2] / 4 * [scale * x + shift > 0] (0 in a dropped odd last row / column). */
+int dfd_bn_relu_avgpool2(const void* x, const float* scale, const float* shift, void* y, int N, int H, int W, int C, int dt,
+                         void* stream);
+int dfd_bn_relu_avgpool2_bwd_reduce(const void* gp, const void* x, const float* scale, const float* shift, const float* mean,
+                                    const float* rstd, int N, int H, int W, int C, int dt, double* s1, double* s2, void* stream);
+int dfd_bn_relu_avgpool2_bwd_apply(const void* gp, const void* x, const float* scale, const float* shift, const float* cA,
+                                   const float* cB, const float* cC, void* dx, int N, int H, int W, int C, int dt, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
