@@ -9,8 +9,8 @@ it (tests/test_host_plan.py::test_no_oracle_on_product_path).
 Parity pin: the reference has NO tests, golden vectors or fixtures of its own (SURVEY.md section 4/8c), so
 this restatement is pinned against outputs of the reference itself: `oracle/mint_goldens.py` and `tools/mint_*_goldens.py`
 import the unmodified reference (authoring container only), run it on seeded synthetic weights and inputs, and commit the
-results under tests/golden/; tests/test_oracle_vs_reference_goldens.py and the family `tests/test_*_cpu.py` check this file
-against them on CPU.
+results under tests/golden/; tests/test_oracle_vs_reference_goldens.py checks this file against them on CPU, one run per
+step fixture of tests/reference_steps.py's CPU_STEPS.
 
 What each function follows (file:line under /root/reference):
   efficientnet_forward : dfd/timm/models/efficientnet.py:320-348

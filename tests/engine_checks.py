@@ -7,14 +7,12 @@ Two oracles are run beside the CUDA path:
   * `fp32`: the plain reference arithmetic (the north_star tolerance: 1e-2 relative for bf16).
 Per-layer taps localise the first diverging layer; per-parameter gradient errors localise a wrong backward kernel.
 """
-import json
-import os
-
 import torch
 
 from deepfake_detection_b200.arch import get_spec, param_entries
 from deepfake_detection_b200.engine import Engine
 from deepfake_detection_b200.optim import ArenaOptimizer
+from deepfake_detection_b200.trainer import Trainer
 from oracle import train as OT
 from oracle.weights import synth_batch, synth_state, tame_state
 
@@ -112,20 +110,23 @@ def run_parity(arch, batch, H, W, dtype="bf16", steps=2, gemm_impl="tc", opt_kin
     return report
 
 
-def golden_compare(case, golden_dir, dtype="bf16", gemm_impl="tc"):
-    """Native path vs the committed reference-minted fixture (loss / logits of step 0 and 1)."""
-    rec = json.load(open(os.path.join(golden_dir, case + ".json")))
-    spec = get_spec(rec["arch"])
-    eng = Engine(rec["arch"], rec["batch"], rec["H"], rec["W"], dtype=dtype, gemm_impl=gemm_impl)
-    eng.load_state_dict(synth_state(spec, seed=rec["weight_seed"]))
-    opt = ArenaOptimizer(eng, opt=rec["opt"], lr=rec["lr"], momentum=rec["momentum"], weight_decay=rec["weight_decay"])
+def trainer_steps(arch, batch, H, W, dtype, steps, sd0, loss_scale=1.0, **trainer_kw):
+    """`steps` Trainer steps (graph-captured; SGD at lr 0.01, momentum 0.9, weight decay 1e-4 unless `trainer_kw` says
+    otherwise) from the weights `sd0` on synth_batch(seed=1234 + i): per step the loss, the logits, the gradient arena with
+    the loss scale it carries, and the updated parameters. The default static loss scale 1 leaves the fp16 gradients
+    unscaled, as the oracle's fp16 emulation rounds them; a dynamically scaled first step can overflow and be skipped."""
+    tr = Trainer(arch, batch, H, W, dtype=dtype, loss_scale=loss_scale, **trainer_kw)
+    tr.engine.load_state_dict(sd0)
     out = []
-    for i, st in enumerate(rec["steps"]):
-        x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=1234 + i, soft=rec["soft"])
-        engine_step(eng, opt, x.cuda(), y.cuda(), rec["smoothing"])
-        ref_logits = torch.tensor(st["logits"])
-        out.append(dict(loss_native=float(eng.loss), loss_ref=st["loss"], logits_rel=relerr(eng.logits, ref_logits)))
-    return out
+    for i in range(steps):
+        x, y = synth_batch(batch, 3, H, W, seed=1234 + i)
+        e = tr.engine
+        scale = float(e.loss_scale_state[0])
+        loss, _ = tr.train_step(x.cuda(), y.cuda())
+        torch.cuda.synchronize()
+        out.append(dict(loss=float(loss), logits=e.logits.detach().cpu().clone(), scale=scale,
+                        grads=e.grads32.detach().cpu().clone(), params=e.params32.detach().cpu().clone()))
+    return tr, out
 
 
 def engine_masks(eng):

@@ -11,6 +11,7 @@ import torch.nn.functional as F
 
 import densenet_ref as R
 from deepfake_detection_b200.arch import DENSENET_ARCHS, SUPPORTED_ARCHS, get_spec, param_entries, state_entries
+from reference_steps import check_summ, digest
 
 # densenet.py at num_classes=2: state_dict entries, parameter tensors, parameters
 TABLE = {"densenet121": (727, 364, 6955906), "densenet169": (1015, 508, 12487810),
@@ -169,12 +170,6 @@ def _golden(name):
     return json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", name)))
 
 
-def _digest(entries):
-    import hashlib
-    import json
-    return hashlib.sha256(json.dumps(entries, separators=(",", ":")).encode()).hexdigest()
-
-
 @pytest.mark.parametrize("key", list(DENSENET_ARCHS) + ["densenet121@in_chans12"])
 def test_state_keys_match_reference(key):
     ref = _golden("densenet_state_keys.json")[key]
@@ -184,22 +179,9 @@ def test_state_keys_match_reference(key):
     params = [[n, list(s)] for n, s, _ in param_entries(spec)]
     if "state" in ref:
         assert state == ref["state"] and params == ref["params"]
-    assert _digest(state) == ref["state_sha256"] and _digest(params) == ref["params_sha256"]
+    assert digest(state) == ref["state_sha256"] and digest(params) == ref["params_sha256"]
     assert (len(state), len(params), sum(math.prod(s) for _, s in params)) == (ref["n_state"], ref["n_param_tensors"],
                                                                               ref["n_params"])
-
-
-def _close(t, s, rtol=2e-4, floor=1e-7):
-    """tests/test_oracle_vs_reference_goldens.py's comparison of a tensor with its recorded summary: the norm within rtol, the
-    samples within 5 * rtol of the tensor's RMS plus rtol of their largest magnitude; `floor` is the absolute slack of
-    quantities that are mathematically zero"""
-    f = t.detach().reshape(-1).to(torch.float64)
-    norm = float(f.norm())
-    assert norm == pytest.approx(s["norm"], rel=rtol, abs=floor * max(f.numel(), 1) ** 0.5), (norm, s["norm"])
-    got = f[torch.tensor(s["idx"])]
-    ref = torch.tensor(s["samples"], dtype=torch.float64)
-    scale = max(s["norm"] / max(f.numel(), 1) ** 0.5, 1e-8)
-    assert float((got - ref).abs().max()) <= 5 * rtol * scale + rtol * float(ref.abs().max()) + floor, (got, ref)
 
 
 def _fixture_masks(rec, spec):
@@ -232,20 +214,20 @@ def test_restatement_matches_reference_steps(name):
         new = {}
         loss, logits, grads = R.train_grads(spec, sd, x, y, masks=masks, head_mask=head, new_sd=new, dtype=torch.float32)
         assert loss == pytest.approx(st["loss"], rel=1e-4), (i, loss, st["loss"])
-        _close(logits, st["logits"], 1e-3)
+        check_summ(logits, st["logits"], "logits step %d" % i, 1e-3)
         rt = 2e-4 * (1 if i == 0 else 25)           # after the first update fp32 differences are amplified through BN
         gfloor = 1e-5 * max(v["norm"] / max(grads[k].numel(), 1) ** 0.5 for k, v in st["grads"].items())
         for n, s in st["grads"].items():
-            _close(grads[n], s, rt, floor=gfloor)
+            check_summ(grads[n], s, "grad %s step %d" % (n, i), rt, floor=gfloor)
         params = {n: sd[n].clone() for n in grads}
         OT.optimizer_step(ost, params, grads)
         sd.update(params)
         sd.update(new)
         for n, s in st["params"].items():
-            _close(sd[n], s, rt)
+            check_summ(sd[n], s, "param %s step %d" % (n, i), rt)
         for n, s in st.get("buffers", {}).items():
-            _close(sd[n], s, rt)
+            check_summ(sd[n], s, "buffer %s step %d" % (n, i), rt)
     if "eval" in rec:
         x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=999)
         with torch.no_grad():
-            _close(R.forward(spec, sd, x, training=False), rec["eval"]["logits"], 5e-3)
+            check_summ(R.forward(spec, sd, x, training=False), rec["eval"]["logits"], "eval logits", 5e-3)

@@ -1,5 +1,5 @@
-"""-m gpu: the native train / validate step (through the C-ABI, whole network) against the CPU oracle and against
-the committed reference-minted fixtures.
+"""-m gpu: the native train / validate step (through the C-ABI, whole network) against the CPU oracle (the committed
+reference-minted fixtures are held by tests/test_reference_steps_gpu.py).
 
 Tolerances: `emul` (oracle rounding activations at the native storage points) isolates kernel logic: 2e-2 on logits
 and total gradient; `fp32` is the north_star parity statement for bf16: logits/loss within 1e-2 relative of the
@@ -56,16 +56,6 @@ def test_resnet_train_step_parity(arch, dtype):
     assert fp["logits_rel"] < 1.5 * yd["logits_rel"] + 1e-2, (fp, yd)
     assert fp["grad_rel_total"] < 1.5 * yd["grad_rel_total"] + 3e-2, (fp, yd)
     assert rep["eval_logits_rel"] < 5e-2, rep["eval_logits_rel"]
-
-
-def test_against_reference_goldens(golden_dir):
-    out = _ec().golden_compare("step_efficientnet_b0", golden_dir)
-    for i, o in enumerate(out):
-        # batch 4 @ 64x64 with lr 0.01 is a chaotic regime for 16-bit storage (the oracle's own bf16 emulation moves the
-        # step-1 logits by ~0.4 relative); the fixture pins step 0 tightly and step 1 on the loss only
-        assert abs(o["loss_native"] - o["loss_ref"]) < (1e-2 if i == 0 else 5e-2) * abs(o["loss_ref"]), o
-        if i == 0:
-            assert o["logits_rel"] < 7e-2, o
 
 
 def test_full_size_properties():

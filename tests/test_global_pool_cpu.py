@@ -1,8 +1,9 @@
 """Selectable global pooling (avg / max / avgmax / catavgmax) on the host side, without a GPU.
 
-The oracle's pool (oracle.model.global_pool) at 'avg' against its default call form and against the global-pool fixtures minted from the UNMODIFIED reference (tools/mint_gpool_goldens.py) at the
-tolerances of test_head_multiclass_cpu.py; the arch restatement against the reference's catavgmax state_dict names and
-shapes; create_model / get_spec carrying the pool type; the plans of both families."""
+The oracle's pool (oracle.model.global_pool) at 'avg' against its default call form; the arch restatement against the
+reference's catavgmax state_dict names and shapes; create_model / get_spec carrying the pool type; the plans of both families.
+The global-pool fixtures minted from the UNMODIFIED reference (tools/mint_gpool_goldens.py) are held by
+tests/reference_steps.py's tables."""
 import json
 import os
 
@@ -13,37 +14,6 @@ from deepfake_detection_b200.arch import SUPPORTED_ARCHS, get_spec, param_entrie
 from oracle import model as OM
 from oracle import train as OT
 from oracle.weights import synth_batch, synth_state
-
-from test_head_multiclass_cpu import RTOL, _check_summ
-
-CASES = ["step_efficientnet_b0_gp_max", "step_efficientnet_b0_k5_gp_catavgmax_ls", "step_resnet18_gp_avgmax"]
-
-
-@pytest.mark.parametrize("case", CASES)
-def test_oracle_global_pool_steps_match_reference(case, golden_dir):
-    rec = json.load(open(os.path.join(golden_dir, case + ".json")))
-    K, gp = rec["num_classes"], rec["global_pool"]
-    torch.set_num_threads(8)
-    spec = get_spec(rec["arch"], num_classes=K, global_pool=gp)
-    sd = synth_state(spec, seed=rec["weight_seed"])
-    opt = OT.OptState(kind=rec["opt"], lr=rec["lr"], momentum=rec["momentum"], weight_decay=rec["weight_decay"], eps=1e-8)
-    for i, st in enumerate(rec["steps"]):
-        x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=1234 + i, soft=rec["soft"], num_classes=K)
-        out = OT.train_step(spec, sd, x, y, opt, smoothing=rec["smoothing"])
-        _check_summ(out["logits"], st["logits"], "logits step %d" % i, rtol=1e-3)
-        assert float(out["loss"]) == pytest.approx(st["loss"], rel=1e-4)
-        assert float(out["prec1"]) == pytest.approx(st["prec1"], abs=1e-3)
-        rt = RTOL * (1 if i == 0 else 25)
-        gfloor = 1e-5 * max(v["norm"] / max(out["grads"][k].numel(), 1) ** 0.5 for k, v in st["grads"].items())
-        for k, s in st["grads"].items():
-            _check_summ(out["grads"][k], s, "grad %s step %d" % (k, i), rt, floor=gfloor)
-        for k, s in st["params"].items():
-            _check_summ(sd[k], s, "param %s step %d" % (k, i), rt)
-        for k, s in st["buffers"].items():
-            _check_summ(sd[k].float(), s, "buffer %s step %d" % (k, i), rt)
-    x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=999, num_classes=K)
-    ev = OT.validate_step(spec, sd, x, y)
-    _check_summ(ev["logits"], rec["eval"]["logits"], "eval logits", rtol=5e-3)
 
 
 @pytest.mark.parametrize("arch", ["efficientnet_b0", "resnet18"])

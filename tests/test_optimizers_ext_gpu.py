@@ -4,13 +4,12 @@
   wiring (tests/update_phase.py), in bf16 and in fp16 with loss scaling, over three update phases against an fp64
   restatement with first-order rounding-error bounds; the middle fp16 step overflows and must change nothing;
 - the per-tensor sums of squares against fp64, bit-identical across runs;
-- captured Trainer steps against oracle/train.py and against the reference's step fixtures;
+- captured Trainer steps against oracle/train.py (the reference's step fixtures are held by
+  tests/test_reference_steps_gpu.py);
 - one captured graph across a per-step lr schedule; state_dict round trips with torch's classes and between native
   optimizers; the runner.
 """
-import json
 import math
-import os
 from types import SimpleNamespace
 
 import pytest
@@ -336,36 +335,6 @@ def test_captured_trainer_against_oracle(kind):
     # 16-bit activations move the gradients by a few percent; an update taken with the wrong lr, decay or per-tensor
     # scalar is off by tens of percent
     assert sum(r for _, r in upd) / len(upd) < 5e-2 and worst[0][1] < 0.3, worst
-
-
-@pytest.mark.parametrize("case", ["step_efficientnet_b0_radam", "step_resnet18_nvnovograd"])
-def test_native_against_reference_step_fixtures(case, golden_dir):
-    """the tolerances of test_head_multiclass_gpu.py::test_native_against_k_class_reference_goldens"""
-    from deepfake_detection_b200.engine import Engine
-    from deepfake_detection_b200.optim import ArenaOptimizer
-    rec = json.load(open(os.path.join(golden_dir, case + ".json")))
-    K = rec["num_classes"]
-    spec = get_spec(rec["arch"], num_classes=K)
-    eng = Engine(rec["arch"], rec["batch"], rec["H"], rec["W"], num_classes=K, dtype="fp16")
-    eng.load_state_dict(synth_state(spec, seed=rec["weight_seed"]))
-    opt = ArenaOptimizer(eng, opt=rec["opt"], lr=rec["lr"], momentum=rec["momentum"], weight_decay=rec["weight_decay"])
-    st_ = torch.cuda.current_stream().cuda_stream
-    for i, st in enumerate(rec["steps"]):
-        x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=1234 + i, num_classes=K)
-        eng.set_input(x.cuda())
-        eng.set_target(y.cuda())
-        eng.zero_step_scratch(st_, grads=True)
-        eng.forward(training=True)
-        eng.head(True, smoothing=0.0, soft=False)
-        eng.backward()
-        opt.step()
-        torch.cuda.synchronize()
-        assert abs(float(eng.loss) - st["loss"]) < (1e-2 if i == 0 else 5e-2) * abs(st["loss"]), (i, float(eng.loss), st["loss"])
-        if i == 0:
-            s = st["logits"]
-            got = eng.logits.flatten().cpu()
-            assert _relerr(got[torch.tensor(s["idx"])], torch.tensor(s["samples"])) < 7e-2
-    assert opt.step_count == len(rec["steps"])
 
 
 def test_one_graph_survives_lr_schedule_for_every_kind():

@@ -1,110 +1,88 @@
 """Pins oracle/ (the CPU restatement) to the reference: every fixture under tests/golden/ was produced by
-the UNMODIFIED reference (oracle/mint_goldens.py); here the oracle must reproduce them in fp32 on CPU.
+the UNMODIFIED reference (oracle/mint_goldens.py, tools/mint_*_goldens.py); here the oracle must reproduce them in fp32 on CPU.
 Tolerance: 2e-4 relative on norms / 1e-4 absolute+relative on samples (same fp32 arithmetic, possibly
 different op ordering inside torch between the module and functional forms)."""
+import glob
+import importlib
 import json
 import os
 
 import pytest
 import torch
 
+import reference_steps as RS
 from deepfake_detection_b200.arch import get_spec
 from oracle import model as OM
 from oracle import train as OT
-from oracle.weights import synth_batch, synth_state
-
-RTOL = 2e-4
-
-
-def _check_summ(t, s, what, rtol=RTOL, floor=1e-7):
-    """`floor`: absolute slack for quantities that are mathematically zero (e.g. the gradient of a BN bias
-    that feeds conv+BN), which are pure fp32 round-off in both implementations."""
-    f = t.detach().reshape(-1).to(torch.float64)
-    norm = float(f.norm())
-    assert norm == pytest.approx(s["norm"], rel=rtol, abs=floor * max(f.numel(), 1) ** 0.5), what + " norm"
-    got = f[torch.tensor(s["idx"])]
-    ref = torch.tensor(s["samples"], dtype=torch.float64)
-    scale = max(s["norm"] / max(f.numel(), 1) ** 0.5, 1e-8)
-    assert float((got - ref).abs().max()) <= 5 * rtol * scale + rtol * float(ref.abs().max()) + floor, what + " samples"
+from oracle.weights import synth_batch, synth_state, tame_state
+from reference_steps import DECAY_PER_LR, RTOL, check_summ
 
 
-CASES = ["step_efficientnet_b0", "step_efficientnet_b4", "step_resnet18", "step_resnet50",
-         "step_efficientnet_b0_ls", "step_efficientnet_b0_soft_rmsprop", "step_efficientnet_b0_adamw"]
-
-
-@pytest.mark.parametrize("case", CASES)
-def test_train_steps_match_reference(case, golden_dir):
-    rec = json.load(open(os.path.join(golden_dir, case + ".json")))
+@pytest.mark.parametrize("case", RS.CPU_STEPS)
+def test_oracle_matches_reference_steps(case, golden_dir):
+    """oracle.train.train_step / validate_step, which read every field of the spec they are given, against the reference's
+    own train steps and eval; what runs comes from the fixture's fields"""
+    rec = RS.load(golden_dir, case)
+    assert rec.get("drop_rate", 0.0) == 0.0
+    K = rec.get("num_classes", 2)
     torch.set_num_threads(8)
-    spec = get_spec(rec["arch"])
+    spec = get_spec(rec["arch"], num_classes=K, global_pool=rec.get("global_pool", "avg"))
     sd = synth_state(spec, seed=rec["weight_seed"])
-    wd = rec["weight_decay"]
-    if rec["opt"] == "adamw":
-        wd = wd / rec["lr"]  # optim_factory.py:29-33
+    if "tame" in rec:
+        sd = tame_state(spec, sd, rec["tame"])
+    wd = rec["weight_decay"] / rec["lr"] if rec["opt"] in DECAY_PER_LR else rec["weight_decay"]
     opt = OT.OptState(kind=rec["opt"], lr=rec["lr"], momentum=rec["momentum"], weight_decay=wd, eps=1e-8)
     for i, st in enumerate(rec["steps"]):
-        x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=1234 + i, soft=rec["soft"])
+        x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=1234 + i, soft=rec["soft"], num_classes=K)
         out = OT.train_step(spec, sd, x, y, opt, smoothing=rec["smoothing"])
-        ref_logits = torch.tensor(st["logits"])
-        assert torch.allclose(out["logits"], ref_logits, rtol=1e-3, atol=1e-4 * float(ref_logits.abs().max() + 1)), "logits step %d" % i
+        assert out["logits"].shape == (rec["batch"], K)
+        if isinstance(st["logits"], list):
+            ref = torch.tensor(st["logits"])
+            assert torch.allclose(out["logits"], ref, rtol=1e-3, atol=1e-4 * float(ref.abs().max() + 1)), "logits step %d" % i
+        else:
+            check_summ(out["logits"], st["logits"], "logits step %d" % i, rtol=1e-3)
         assert float(out["loss"]) == pytest.approx(st["loss"], rel=1e-4)
         assert float(out["prec1"]) == pytest.approx(st["prec1"], abs=1e-3)
         # after the first update tiny fp32 differences are amplified through BN: loosen progressively
         rt = RTOL * (1 if i == 0 else 25)
         gfloor = 1e-5 * max(v["norm"] / max(out["grads"][k].numel(), 1) ** 0.5 for k, v in st["grads"].items())
         for k, s in st["grads"].items():
-            _check_summ(out["grads"][k], s, "grad %s step %d" % (k, i), rt, floor=gfloor)
-        # adaptive optimizers normalise the gradient, so a mathematically-zero (round-off) gradient becomes an
-        # O(lr) random update in BOTH implementations: such parameters carry no parity information
+            check_summ(out["grads"][k], s, "grad %s step %d" % (k, i), rt, floor=gfloor)
+        # adaptive optimizers normalise the gradient, so a mathematically-zero (round-off) gradient becomes an O(lr) random
+        # update in BOTH implementations: such parameters carry no parity information
         noise = {k for k, v in st["grads"].items()
                  if v["norm"] / max(out["grads"][k].numel(), 1) ** 0.5 < 10 * gfloor} if rec["opt"] != "sgd" else set()
-        if i == 0:
-            skipped = set(noise)
         for k, s in st["params"].items():
-            if k in skipped or k in noise:
-                continue
-            _check_summ(sd[k], s, "param %s step %d" % (k, i), rt)
+            if k not in noise:
+                check_summ(sd[k], s, "param %s step %d" % (k, i), rt)
         for k, s in st["buffers"].items():
-            _check_summ(sd[k].float(), s, "buffer %s step %d" % (k, i), rt)
-    x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=999)
-    ev = OT.validate_step(spec, sd, x, y)
-    ref = torch.tensor(rec["eval"]["logits"])
-    assert torch.allclose(ev["logits"], ref, rtol=5e-3, atol=5e-3 * float(ref.abs().max()))
-
-
-# one fixture per option the default EfficientNet / ResNet-18/50 cases above do not reach: a selectable global pool, TF "SAME"
-# padding with BatchNorm eps 1e-3, the ResNet-D stem and shortcut, the SE-ResNet blocks and stem pool, Xception
-FAMILY_CASES = ["step_resnet18_gp_avgmax", "step_efficientnet_b0_gp_max", "step_efficientnet_b0_k5_gp_catavgmax_ls",
-                "step_tf_efficientnet_b0_64x96", "step_resnet50d", "step_seresnet18_70x72", "step_xception_64x80"]
-
-
-@pytest.mark.parametrize("case", FAMILY_CASES)
-def test_generic_steps_match_family_fixtures(case, golden_dir):
-    """oracle.train.train_step / validate_step read every field of the spec they are given: each family's fixture through the
-    generic entry points, at the tolerances of that family's CPU test"""
-    rec = json.load(open(os.path.join(golden_dir, case + ".json")))
-    K = rec["num_classes"]
-    torch.set_num_threads(8)
-    spec = get_spec(rec["arch"], num_classes=K, global_pool=rec.get("global_pool", "avg"))
-    sd = synth_state(spec, seed=rec["weight_seed"])
-    opt = OT.OptState(kind=rec["opt"], lr=rec["lr"], momentum=rec["momentum"], weight_decay=rec["weight_decay"], eps=1e-8)
-    for i, st in enumerate(rec["steps"]):
-        x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=1234 + i, soft=rec["soft"], num_classes=K)
-        out = OT.train_step(spec, sd, x, y, opt, smoothing=rec["smoothing"])
-        _check_summ(out["logits"], st["logits"], "logits step %d" % i, rtol=1e-3)
-        assert float(out["loss"]) == pytest.approx(st["loss"], rel=1e-4)
-        assert float(out["prec1"]) == pytest.approx(st["prec1"], abs=1e-3)
-        rt = RTOL * (1 if i == 0 else 25)
-        gfloor = 1e-5 * max(v["norm"] / max(out["grads"][k].numel(), 1) ** 0.5 for k, v in st["grads"].items())
-        for k, s in st["grads"].items():
-            _check_summ(out["grads"][k], s, "grad %s step %d" % (k, i), rt, floor=gfloor)
-        for k, s in st["params"].items():
-            _check_summ(sd[k], s, "param %s step %d" % (k, i), rt)
-        for k, s in st["buffers"].items():
-            _check_summ(sd[k].float(), s, "buffer %s step %d" % (k, i), rt)
+            check_summ(sd[k].float(), s, "buffer %s step %d" % (k, i), rt)
     x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=999, num_classes=K)
     ev = OT.validate_step(spec, sd, x, y)
-    _check_summ(ev["logits"], rec["eval"]["logits"], "eval logits", rtol=5e-3)
+    if isinstance(rec["eval"]["logits"], list):
+        ref = torch.tensor(rec["eval"]["logits"])
+        assert torch.allclose(ev["logits"], ref, rtol=5e-3, atol=5e-3 * float(ref.abs().max())), "eval logits"
+    else:
+        check_summ(ev["logits"], rec["eval"]["logits"], "eval logits", rtol=5e-3)
+    assert float(ev["loss"]) == pytest.approx(rec["eval"]["loss"], rel=2e-3)
+
+
+def test_every_step_fixture_is_checked_once(golden_dir):
+    """each tests/golden/step_*.json is held by the table above or by one named test, never both; the native path's table
+    is a subset of the oracle's"""
+    on_disk = {os.path.basename(p)[:-len(".json")] for p in glob.glob(os.path.join(golden_dir, "step_*.json"))}
+    cpu = RS.CPU_STEPS
+    elsewhere = [c for c, _ in RS.ELSEWHERE]
+    assert len(set(cpu)) == len(cpu) and len(set(elsewhere)) == len(elsewhere)
+    assert not set(cpu) & set(elsewhere)
+    assert set(cpu) | set(elsewhere) == on_disk, (on_disk - set(cpu) - set(elsewhere), set(cpu) | set(elsewhere) - on_disk)
+    gpu = [c for c, _ in RS.GPU_STEPS]
+    assert len(set(gpu)) == len(gpu) and set(gpu) <= set(cpu), set(gpu) - set(cpu)
+    for case, o in RS.GPU_STEPS:
+        assert o["kind"] in ("engine", "tamed") and o["dtypes"] and set(o["dtypes"]) <= {"bf16", "fp16"}, case
+    for case, test in RS.ELSEWHERE:
+        module, _, name = test.partition("::")
+        assert name.startswith("test_") and callable(getattr(importlib.import_module(module), name, None)), (case, test)
 
 
 def test_optimizers_match_reference(golden_dir):
@@ -113,7 +91,7 @@ def test_optimizers_match_reference(golden_dir):
         g0 = torch.Generator().manual_seed(3)
         params = {"w": torch.randn(5, 7, generator=g0), "bias": torch.randn(7, generator=g0),
                   "k": torch.randn(4, 1, 3, 3, generator=g0)}
-        wd = r["weight_decay"] / r["lr"] if name == "adamw" else r["weight_decay"]
+        wd = r["weight_decay"] / r["lr"] if name in DECAY_PER_LR else r["weight_decay"]
         opt = OT.OptState(kind=name, lr=r["lr"], momentum=r["momentum"], weight_decay=wd, eps=r["eps"])
         g = torch.Generator().manual_seed(11)
         for step in range(3):
@@ -154,7 +132,7 @@ def test_runner_config1_resnet18(golden_dir):
     vl = [float(OT.validate_step(spec, sd, x, y)["loss"]) for x, y in batches]
     assert sum(vl) / 2 == pytest.approx(rec["validate"]["loss"], rel=2e-3)
     for k, s in rec["params"].items():
-        _check_summ(sd[k], s, "param " + k, 25 * RTOL)
+        check_summ(sd[k], s, "param " + k, 25 * RTOL)
 
 
 def test_dropped_step_matches_reference(golden_dir):
@@ -178,9 +156,9 @@ def test_dropped_step_matches_reference(golden_dir):
     assert float(out["loss"]) == pytest.approx(rec["loss"], rel=1e-4)
     gfloor = 1e-5 * max(v["norm"] / max(out["grads"][k].numel(), 1) ** 0.5 for k, v in rec["grads"].items())
     for k, s in rec["grads"].items():
-        _check_summ(out["grads"][k], s, "grad " + k, RTOL, floor=gfloor)
+        check_summ(out["grads"][k], s, "grad " + k, RTOL, floor=gfloor)
     for k, s in rec["params"].items():
-        _check_summ(sd[k], s, "param " + k, RTOL)
+        check_summ(sd[k], s, "param " + k, RTOL)
 
 
 def test_aux_formulas_match_reference(golden_dir):

@@ -1,27 +1,16 @@
 """Host logic of the dense ResNet family (resnet26/34/101/152, tv_resnet34/50, wide_resnet50_2/101_2, resnet26d, resnet50d),
-no GPU: the specs against the reference's state keys, the oracle (oracle/model.py) against the reference's train
-steps, the model factory's registry, default_cfg and init, and the plans. Fixtures: tools/mint_resnet_family_goldens.py."""
-import hashlib
+no GPU: the specs against the reference's state keys, the model factory's registry, default_cfg and init, and the plans.
+Fixtures: tools/mint_resnet_family_goldens.py; their train steps are held by tests/reference_steps.py's tables."""
 import json
 import os
 from collections import Counter
 
 import pytest
-import torch
 
 from deepfake_detection_b200 import _lib
 from deepfake_detection_b200.arch import RESNET_ARCHS, SUPPORTED_ARCHS, get_spec, param_entries, state_entries
 from deepfake_detection_b200.engine import Engine
-from oracle import train as OT
-from oracle.weights import synth_batch, synth_state, tame_state
-from test_tf_efficientnet_cpu import RTOL, _check_summ
-
-STEP_CASES = ["step_resnet26d_72x88", "step_resnet50d", "step_resnet34", "step_wide_resnet50_2", "step_resnet101",
-              "step_resnet26d_tame_104x88", "step_resnet34_tame_96", "step_wide_resnet50_2_tame_96", "step_resnet101_tame_96"]
-
-
-def _digest(entries):
-    return hashlib.sha256(json.dumps(entries, separators=(",", ":")).encode()).hexdigest()
+from reference_steps import digest
 
 
 def test_registry():
@@ -44,7 +33,7 @@ def test_specs_match_reference_state_keys(key, golden_dir):
     if "state" in ref:          # written out in full: a mismatch shows the first differing entry
         assert state == ref["state"] and params == ref["params"]
     assert (len(state), len(params)) == (ref["n_state"], ref["n_param_tensors"])
-    assert _digest(state) == ref["state_sha256"] and _digest(params) == ref["params_sha256"]
+    assert digest(state) == ref["state_sha256"] and digest(params) == ref["params_sha256"]
     n = 0
     for _, s, _ in param_entries(spec):
         k = 1
@@ -52,36 +41,6 @@ def test_specs_match_reference_state_keys(key, golden_dir):
             k *= d
         n += k
     assert n == ref["n_params"]
-
-
-@pytest.mark.parametrize("case", STEP_CASES)
-def test_oracle_matches_reference_steps(case, golden_dir):
-    """oracle/model.py against the reference's own train steps and eval, at the tolerances of
-    test_oracle_vs_reference_goldens.py / test_tf_efficientnet_cpu.py"""
-    rec = json.load(open(os.path.join(golden_dir, case + ".json")))
-    torch.set_num_threads(8)
-    spec = get_spec(rec["arch"], num_classes=rec["num_classes"])
-    sd = synth_state(spec, seed=rec["weight_seed"])
-    if "tame" in rec:
-        sd = tame_state(spec, sd, rec["tame"])
-    opt = OT.OptState(kind=rec["opt"], lr=rec["lr"], momentum=rec["momentum"], weight_decay=rec["weight_decay"], eps=1e-8)
-    for i, st in enumerate(rec["steps"]):
-        x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=1234 + i)
-        out = OT.train_step(spec, sd, x, y, opt)
-        _check_summ(out["logits"], st["logits"], "logits step %d" % i, rtol=1e-3)
-        assert float(out["loss"]) == pytest.approx(st["loss"], rel=1e-4)
-        assert float(out["prec1"]) == pytest.approx(st["prec1"], abs=1e-3)
-        rt = RTOL * (1 if i == 0 else 25)
-        gfloor = 1e-5 * max(v["norm"] / max(out["grads"][k].numel(), 1) ** 0.5 for k, v in st["grads"].items())
-        for k, s in st["grads"].items():
-            _check_summ(out["grads"][k], s, "grad %s step %d" % (k, i), rt, floor=gfloor)
-        for k, s in st["params"].items():
-            _check_summ(sd[k], s, "param %s step %d" % (k, i), rt)
-        for k, s in st["buffers"].items():
-            _check_summ(sd[k].float(), s, "buffer %s step %d" % (k, i), rt)
-    x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=999)
-    ev = OT.validate_step(spec, sd, x, y)
-    _check_summ(ev["logits"], rec["eval"]["logits"], "eval logits", rtol=5e-3)
 
 
 @pytest.mark.parametrize("in_chans", [3, 12])

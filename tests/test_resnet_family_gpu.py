@@ -2,14 +2,13 @@
 
   * dfd_avgpool2_fwd / dfd_avgpool2_bwd_add against fp64 F.avg_pool2d(2, 2, ceil_mode=True, count_include_pad=False) and its
     autograd, and bit for bit against a torch emulation of their one-rounding formulas, at even and odd extents, bf16 / fp16;
-  * whole train steps of resnet26d, resnet34, wide_resnet50_2 and resnet101 against the oracle (oracle/model.py)
-    and the reference's step fixtures; resnet101 and resnet50d at batch 32, 224x224, from the reference init against the fp32
-    oracle; the runner's train_epoch over create_model("resnet101"); resnet50d with DropBlock, drop path and dropout;
+  * resnet101 and resnet50d at batch 32, 224x224, from the reference init against the fp32 oracle; the runner's train_epoch
+    over create_model("resnet101"); resnet50d with DropBlock, drop path and dropout;
   * checkpoints round-trip bit for bit, and two resnet50d engines agree bit for bit.
 No test here reads the reference tree: the fixtures under tests/golden/ came from tools/mint_resnet_family_goldens.py.
+Their train steps are held by tests/test_reference_steps_gpu.py.
 """
 import io
-import json
 import os
 from types import SimpleNamespace
 
@@ -106,77 +105,6 @@ def test_avgpool2_bwd_add_in_place(dtype):
     _call("dfd_avgpool2_bwd_add", dy.data_ptr(), acc.data_ptr(), acc.data_ptr(), N_POOL, H, W, C, DT_CODE[dtype])
     torch.cuda.synchronize()
     assert torch.equal(acc, ref)
-
-
-# ---- whole steps --------------------------------------------------------------------------------------------------------
-def _run_steps(arch, batch, H, W, dtype, steps, sd0=None):
-    from deepfake_detection_b200.arch import get_spec
-    from deepfake_detection_b200.trainer import Trainer
-    from oracle.weights import synth_batch, synth_state
-    spec = get_spec(arch)
-    sd0 = synth_state(spec, seed=7) if sd0 is None else sd0
-    # static loss scale 1: the oracle's fp16 emulation rounds the unscaled gradients, and a dynamically scaled first step can
-    # overflow and be skipped
-    tr = Trainer(arch, batch, H, W, dtype=dtype, opt="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4, loss_scale=1.0)
-    tr.engine.load_state_dict(sd0)
-    out = []
-    for i in range(steps):
-        x, y = synth_batch(batch, 3, H, W, seed=1234 + i)
-        e = tr.engine
-        scale = float(e.loss_scale_state[0])        # fp16: the gradient arena holds loss-scaled gradients (1 in bf16)
-        loss, _ = tr.train_step(x.cuda(), y.cuda())
-        torch.cuda.synchronize()
-        out.append(dict(loss=float(loss), logits=e.logits.detach().cpu().clone(), scale=scale,
-                        grads=e.grads32.detach().cpu().clone(), params=e.params32.detach().cpu().clone()))
-    return spec, sd0, tr, out
-
-
-STEP_CASES = [("resnet26d", 8, 104, 88, "step_resnet26d_tame_104x88"), ("resnet34", 8, 96, 96, "step_resnet34_tame_96"),
-              ("wide_resnet50_2", 8, 96, 96, "step_wide_resnet50_2_tame_96"), ("resnet101", 8, 96, 96, "step_resnet101_tame_96")]
-
-
-@pytest.mark.parametrize("dtype", ["bf16", "fp16"])
-@pytest.mark.parametrize("arch,batch,H,W,fixture", STEP_CASES, ids=[c[0] for c in STEP_CASES])
-def test_steps_match_oracle_and_reference(arch, batch, H, W, fixture, dtype, golden_dir):
-    """Train steps from the reference's tamed fixtures (batch 8, the residual branches damped as engine_checks.run_parity(tame=True)
-    does, so 16-bit storage stays a small perturbation): step 0 with test_engine_gpu.py::test_resnet_train_step_parity's
-    statements (logits and loss against the oracle's 16-bit emulation; logits and gradients against the fp32 oracle within 1.5 x
-    the emulation's own distance + a margin), every step's loss against the reference, and the step-0 logits against the
-    reference's samples. resnet101 in bf16 is the one case where the emulation itself moves the logits by more than the
-    emulation bound (7.4e-2): there that bound is 1.5 x the emulation's distance."""
-    from deepfake_detection_b200.arch import param_entries
-    from oracle import train as OT
-    from oracle.weights import synth_batch, synth_state, tame_state
-    from deepfake_detection_b200.arch import get_spec
-    rec = json.load(open(os.path.join(golden_dir, fixture + ".json")))
-    assert (rec["arch"], rec["batch"], rec["H"], rec["W"]) == (arch, batch, H, W)
-    spec = get_spec(arch)
-    sd0 = tame_state(spec, synth_state(spec, seed=rec["weight_seed"]), rec["tame"])
-    spec, sd0, tr, runs = _run_steps(arch, batch, H, W, dtype, len(rec["steps"]), sd0)
-    sd = {k: v.clone() for k, v in sd0.items()}
-    ost = OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4)
-    e = tr.engine
-    for i, (r, st) in enumerate(zip(runs, rec["steps"])):
-        x, y = synth_batch(batch, 3, H, W, seed=1234 + i)
-        o = OT.train_step(spec, sd, x, y, ost, act_dtype=TDT[dtype])
-        if i == 0:
-            o32 = OT.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None)
-            yard_logits = _rel(o["logits"], o32["logits"])
-            bound = max(2e-2 if dtype == "fp16" else 6e-2, 1.5 * yard_logits)
-            assert _rel(r["logits"], o["logits"]) < bound, (_rel(r["logits"], o["logits"]), yard_logits)
-            assert abs(r["loss"] - float(o["loss"])) < 5e-3, (r["loss"], float(o["loss"]))
-            assert _rel(r["logits"], o32["logits"]) < 1.5 * yard_logits + 1e-2, (_rel(r["logits"], o32["logits"]), yard_logits)
-            names = [n for n, _, _ in param_entries(spec)]
-            gn = torch.cat([r["grads"][e.p_off[n][0]:e.p_off[n][0] + e.p_off[n][2]] for n in names]) / r["scale"]
-            go, g32 = (torch.cat([oo["grads"][n].flatten() for n in names]) for oo in (o, o32))
-            yard = _rel(go, g32)
-            assert _rel(gn, g32) < 1.5 * yard + 3e-2, (_rel(gn, g32), yard)
-            f = r["logits"].double().flatten()
-            ref = torch.tensor(st["logits"]["samples"], dtype=torch.float64)
-            got = f[torch.tensor(st["logits"]["idx"])]
-            assert float((got - ref).norm() / ref.norm()) < 1.5 * yard_logits + 2e-2, (got, ref)
-        # the reference's losses: 1e-2 at step 0, 5e-2 after an update (tests/test_engine_gpu.py::test_against_reference_goldens)
-        assert abs(r["loss"] - st["loss"]) < (1e-2 if i == 0 else 5e-2) * abs(st["loss"]), (i, r["loss"], st["loss"])
 
 
 # ---- realistic size -------------------------------------------------------------------------------------------------------
@@ -340,7 +268,11 @@ def test_checkpoint_round_trip_is_bit_exact():
 
 
 def test_two_resnet50d_engines_agree_bit_for_bit():
-    runs = [_run_steps("resnet50d", 8, 96, 96, "bf16", 2)[3] for _ in range(2)]
+    from deepfake_detection_b200.arch import get_spec
+    from engine_checks import trainer_steps
+    from oracle.weights import synth_state
+    sd0 = synth_state(get_spec("resnet50d"), seed=7)
+    runs = [trainer_steps("resnet50d", 8, 96, 96, "bf16", 2, sd0)[1] for _ in range(2)]
     for a, b in zip(*runs):
         assert a["loss"] == b["loss"]
         assert torch.equal(a["logits"], b["logits"]) and torch.equal(a["grads"], b["grads"]) and torch.equal(a["params"], b["params"])

@@ -1,6 +1,6 @@
-"""Host logic of the SE-ResNets, no GPU: the specs against the reference's state keys, the oracle (oracle/model.py) against
-the reference's train steps, the model factory (default_cfg, init, the keyword arguments the reference refuses or drops) and the
-plans. Fixtures: tools/mint_senet_goldens.py."""
+"""Host logic of the SE-ResNets, no GPU: the specs against the reference's state keys, the model factory (default_cfg, init,
+the keyword arguments the reference refuses or drops) and the plans. Fixtures: tools/mint_senet_goldens.py; their train steps
+are held by tests/reference_steps.py's tables."""
 import json
 import math
 import os
@@ -13,13 +13,7 @@ from deepfake_detection_b200 import _lib
 from deepfake_detection_b200.arch import (RESNET_ARCHS, SENET_ARCHS, SUPPORTED_ARCHS, get_spec, param_entries, state_entries,
                                           stem_pool_out)
 from deepfake_detection_b200.engine import Engine
-from oracle import train as OT
-from oracle.weights import synth_batch, synth_state, tame_state
-from test_resnet_family_cpu import _digest
-from test_tf_efficientnet_cpu import RTOL, _check_summ
-
-STEP_CASES = ["step_seresnet18_70x72", "step_seresnet50_64x64", "step_seresnet101", "step_seresnet18_tame_70x72",
-              "step_seresnet50_tame_64x64", "step_seresnet101_tame_64x64"]
+from reference_steps import digest
 N_STATE = {"seresnet18": 154, "seresnet34": 282, "seresnet50": 384, "seresnet101": 758, "seresnet152": 1132}
 
 
@@ -45,7 +39,7 @@ def test_spec_matches_reference_state_keys(key, golden_dir):
     if "state" in ref:
         assert state == ref["state"] and params == ref["params"]
     assert len(state) == ref["n_state"] == N_STATE[arch] and len(params) == ref["n_param_tensors"]
-    assert _digest(state) == ref["state_sha256"] and _digest(params) == ref["params_sha256"]
+    assert digest(state) == ref["state_sha256"] and digest(params) == ref["params_sha256"]
     assert sum(math.prod(s) for _, s, _ in param_entries(spec)) == ref["n_params"]
     if key == "seresnet50":
         assert ref["n_params"] == 26043122
@@ -59,36 +53,6 @@ def test_se_widths_and_strides():
     assert sorted({b.cse for b in s50.blocks}) == [16, 32, 64, 128]
     assert s50.stride_in_1x1 and not s18.stride_in_1x1 and s50.stem_pool == s18.stem_pool == "ceil"
     assert [b.name for b in s50.blocks if b.downsample] == ["layer1.0", "layer2.0", "layer3.0", "layer4.0"]
-
-
-@pytest.mark.parametrize("case", STEP_CASES)
-def test_oracle_matches_reference_steps(case, golden_dir):
-    """oracle/model.py against the reference's own train steps and eval, at the ResNet family's fp32 tolerances"""
-    rec = json.load(open(os.path.join(golden_dir, case + ".json")))
-    assert rec["drop_rate"] == 0.0
-    torch.set_num_threads(8)
-    spec = get_spec(rec["arch"], num_classes=rec["num_classes"])
-    sd = synth_state(spec, seed=rec["weight_seed"])
-    if "tame" in rec:
-        sd = tame_state(spec, sd, rec["tame"])
-    opt = OT.OptState(kind=rec["opt"], lr=rec["lr"], momentum=rec["momentum"], weight_decay=rec["weight_decay"], eps=1e-8)
-    for i, st in enumerate(rec["steps"]):
-        x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=1234 + i)
-        out = OT.train_step(spec, sd, x, y, opt)
-        _check_summ(out["logits"], st["logits"], "logits step %d" % i, rtol=1e-3)
-        assert float(out["loss"]) == pytest.approx(st["loss"], rel=1e-4)
-        assert float(out["prec1"]) == pytest.approx(st["prec1"], abs=1e-3)
-        rt = RTOL * (1 if i == 0 else 25)
-        gfloor = 1e-5 * max(v["norm"] / max(out["grads"][k].numel(), 1) ** 0.5 for k, v in st["grads"].items())
-        for k, s in st["grads"].items():
-            _check_summ(out["grads"][k], s, "grad %s step %d" % (k, i), rt, floor=gfloor)
-        for k, s in st["params"].items():
-            _check_summ(sd[k], s, "param %s step %d" % (k, i), rt)
-        for k, s in st["buffers"].items():
-            _check_summ(sd[k].float(), s, "buffer %s step %d" % (k, i), rt)
-    x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=999)
-    ev = OT.validate_step(spec, sd, x, y)
-    _check_summ(ev["logits"], rec["eval"]["logits"], "eval logits", rtol=5e-3)
 
 
 # ---- factory ------------------------------------------------------------------------------------------------------------

@@ -4,13 +4,12 @@
     extents with forced ties; dfd_pool_se_relu against the SEModule formula in fp64 at every (C, Cse, HW) of seresnet18 / 50,
     batch 1 (chunked) and 64; dfd_relu_se_bwd_reduce + dfd_act_bwd + the BatchNorm backward + dfd_se_fc_wgrad against fp64
     autograd of relu(se(bn(y)) + res); bf16 and fp16;
-  * whole train steps against the oracle (oracle/model.py) and the reference's tamed step fixtures; seresnet50 at batch
-    32, 224x224, from the reference init against the fp32 oracle; fp16 eval at batch 1; max / avgmax pooling; the default
-    dropout; checkpoints and two engines bit for bit; the runner's train_epoch with an EMA update.
+  * seresnet50 at batch 32, 224x224, from the reference init against the fp32 oracle; fp16 eval at batch 1; max / avgmax
+    pooling; the default dropout; checkpoints and two engines bit for bit; the runner's train_epoch with an EMA update.
 No test here reads the reference tree: the fixtures under tests/golden/ came from tools/mint_senet_goldens.py.
+Their train steps are held by tests/test_reference_steps_gpu.py.
 """
 import io
-import json
 import os
 from types import SimpleNamespace
 
@@ -179,65 +178,6 @@ def test_se_tail_backward(N, HW, C, Cse, act, dtype):
     assert not bad, bad
 
 
-# ---- whole steps --------------------------------------------------------------------------------------------------------
-def _run_steps(arch, batch, H, W, dtype, steps, sd0, **kw):
-    from deepfake_detection_b200.trainer import Trainer
-    from oracle.weights import synth_batch
-    tr = Trainer(arch, batch, H, W, dtype=dtype, opt="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4, loss_scale=1.0, **kw)
-    tr.engine.load_state_dict(sd0)
-    out = []
-    for i in range(steps):
-        x, y = synth_batch(batch, 3, H, W, seed=1234 + i)
-        e = tr.engine
-        scale = float(e.loss_scale_state[0])
-        loss, _ = tr.train_step(x.cuda(), y.cuda())
-        torch.cuda.synchronize()
-        out.append(dict(loss=float(loss), logits=e.logits.detach().cpu().clone(), scale=scale,
-                        grads=e.grads32.detach().cpu().clone(), params=e.params32.detach().cpu().clone()))
-    return tr, out
-
-
-STEP_CASES = [("seresnet18", 8, 70, 72, "step_seresnet18_tame_70x72"), ("seresnet50", 8, 64, 64, "step_seresnet50_tame_64x64"),
-              ("seresnet101", 8, 64, 64, "step_seresnet101_tame_64x64")]
-
-
-@pytest.mark.parametrize("dtype", ["bf16", "fp16"])
-@pytest.mark.parametrize("arch,batch,H,W,fixture", STEP_CASES, ids=[c[0] for c in STEP_CASES])
-def test_steps_match_oracle_and_reference(arch, batch, H, W, fixture, dtype, golden_dir):
-    """tests/test_resnet_family_gpu.py::test_steps_match_oracle_and_reference's statements over the tamed SE-ResNet fixtures"""
-    from deepfake_detection_b200.arch import get_spec, param_entries
-    from oracle import train as OT
-    from oracle.weights import synth_batch, synth_state, tame_state
-    rec = json.load(open(os.path.join(golden_dir, fixture + ".json")))
-    assert (rec["arch"], rec["batch"], rec["H"], rec["W"]) == (arch, batch, H, W)
-    spec = get_spec(arch)
-    sd0 = tame_state(spec, synth_state(spec, seed=rec["weight_seed"]), rec["tame"])
-    tr, runs = _run_steps(arch, batch, H, W, dtype, len(rec["steps"]), sd0)
-    sd = {k: v.clone() for k, v in sd0.items()}
-    ost = OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4)
-    e = tr.engine
-    for i, (r, st) in enumerate(zip(runs, rec["steps"])):
-        x, y = synth_batch(batch, 3, H, W, seed=1234 + i)
-        o = OT.train_step(spec, sd, x, y, ost, act_dtype=TDT[dtype])
-        if i == 0:
-            o32 = OT.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None)
-            yard_logits = _rel(o["logits"], o32["logits"])
-            bound = max(2e-2 if dtype == "fp16" else 6e-2, 1.5 * yard_logits)
-            assert _rel(r["logits"], o["logits"]) < bound, (_rel(r["logits"], o["logits"]), yard_logits)
-            assert abs(r["loss"] - float(o["loss"])) < 5e-3, (r["loss"], float(o["loss"]))
-            assert _rel(r["logits"], o32["logits"]) < 1.5 * yard_logits + 1e-2, (_rel(r["logits"], o32["logits"]), yard_logits)
-            names = [n for n, _, _ in param_entries(spec)]
-            gn = torch.cat([r["grads"][e.p_off[n][0]:e.p_off[n][0] + e.p_off[n][2]] for n in names]) / r["scale"]
-            go, g32 = (torch.cat([oo["grads"][n].flatten() for n in names]) for oo in (o, o32))
-            yard = _rel(go, g32)
-            assert _rel(gn, g32) < 1.5 * yard + 3e-2, (_rel(gn, g32), yard)
-            f = r["logits"].double().flatten()
-            ref = torch.tensor(st["logits"]["samples"], dtype=torch.float64)
-            got = f[torch.tensor(st["logits"]["idx"])]
-            assert float((got - ref).norm() / ref.norm()) < 1.5 * yard_logits + 2e-2, (got, ref)
-        assert abs(r["loss"] - st["loss"]) < (1e-2 if i == 0 else 5e-2) * abs(st["loss"]), (i, r["loss"], st["loss"])
-
-
 # ---- realistic size -------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("dtype", ["bf16", "fp16"])
 def test_seresnet50_batch32_224_reference_init(dtype, record_property):
@@ -389,8 +329,9 @@ def test_two_engines_agree_bit_for_bit(arch, batch):
     """batch 2: the SE pools and the tail backward split each image over several CTAs (fixed-slot partials)"""
     from deepfake_detection_b200.arch import get_spec
     from oracle.weights import synth_state
+    from engine_checks import trainer_steps
     sd0 = synth_state(get_spec(arch), seed=7)
-    runs = [_run_steps(arch, batch, 96, 96, "bf16", 2, sd0)[1] for _ in range(2)]
+    runs = [trainer_steps(arch, batch, 96, 96, "bf16", 2, sd0)[1] for _ in range(2)]
     for a, b in zip(*runs):
         assert a["loss"] == b["loss"]
         assert torch.equal(a["logits"], b["logits"]) and torch.equal(a["grads"], b["grads"]) and torch.equal(a["params"], b["params"])

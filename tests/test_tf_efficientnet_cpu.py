@@ -1,7 +1,8 @@
 """Host logic of the TensorFlow-ported EfficientNets (tf_efficientnet_b0..b7, _ap, _ns), no GPU: the specs against the
 reference's state keys, the engine's TF "SAME" pads against the reference's own `pad_same`, the oracle against the reference's
-train steps, the model factory's BatchNorm and default_cfg rules, the plans (where they differ from the symmetric models and
-where they must not), and the coverage contract of the GPU file's kernel cases. Fixtures: tools/mint_tf_goldens.py."""
+eval logits, the model factory's BatchNorm and default_cfg rules, the plans (where they differ from the symmetric models and
+where they must not), and the coverage contract of the GPU file's kernel cases. Fixtures: tools/mint_tf_goldens.py; their
+train steps are held by tests/reference_steps.py's tables."""
 import json
 import os
 
@@ -14,18 +15,7 @@ from deepfake_detection_b200.arch import SUPPORTED_ARCHS, TF_ARCHS, conv_pads, g
 from deepfake_detection_b200.engine import Engine, base_name
 from oracle import train as OT
 from oracle.weights import synth_batch, synth_state
-
-RTOL = 2e-4
-
-
-def _check_summ(t, s, what, rtol=RTOL, floor=1e-7):
-    # tests/test_head_multiclass_cpu.py's summary check
-    f = t.detach().reshape(-1).to(torch.float64)
-    assert float(f.norm()) == pytest.approx(s["norm"], rel=rtol, abs=floor * max(f.numel(), 1) ** 0.5), what + " norm"
-    got = f[torch.tensor(s["idx"])]
-    ref = torch.tensor(s["samples"], dtype=torch.float64)
-    scale = max(s["norm"] / max(f.numel(), 1) ** 0.5, 1e-8)
-    assert float((got - ref).abs().max()) <= 5 * rtol * scale + rtol * float(ref.abs().max()) + floor, what + " samples"
+from reference_steps import digest
 
 
 def test_tf_archs_are_the_24_entrypoints_and_supported_archs_unchanged():
@@ -37,7 +27,6 @@ def test_tf_archs_are_the_24_entrypoints_and_supported_archs_unchanged():
 
 @pytest.mark.parametrize("key", list(TF_ARCHS) + ["tf_efficientnet_b7@in_chans12"])
 def test_specs_match_reference_state_keys(key, golden_dir):
-    import hashlib
     ref = json.load(open(os.path.join(golden_dir, "tf_state_keys.json")))[key]
     arch, _, ic = key.partition("@in_chans")
     spec = get_spec(arch, num_classes=2, in_chans=int(ic or 3))
@@ -45,7 +34,6 @@ def test_specs_match_reference_state_keys(key, golden_dir):
     params = [[n, list(s)] for n, s, _ in param_entries(spec)]
     if "state" in ref:          # tf_efficientnet_b0 in full: a mismatch shows the first differing entry
         assert state == ref["state"] and params == ref["params"]
-    digest = lambda e: hashlib.sha256(json.dumps(e, separators=(",", ":")).encode()).hexdigest()    # noqa: E731
     assert (len(state), len(params)) == (ref["n_state"], ref["n_param_tensors"])
     assert digest(state) == ref["state_sha256"] and digest(params) == ref["params_sha256"]
     n = 0
@@ -90,34 +78,6 @@ def test_issue_pad_table_at_default_resolutions():
                                                              "blocks.3.0.conv_dw", "blocks.5.0.conv_dw"]
     assert "blocks.2.0.conv_dw" not in [n for n, _, _ in asym("tf_efficientnet_b4")] and len(asym("tf_efficientnet_b4")) == 4
     assert "blocks.3.0.conv_dw" not in [n for n, _, _ in asym("tf_efficientnet_b7")] and len(asym("tf_efficientnet_b7")) == 4
-
-
-@pytest.mark.parametrize("case", ["step_tf_efficientnet_b0_64x96", "step_tf_efficientnet_b0_66x96"])
-def test_oracle_matches_reference_steps(case, golden_dir):
-    """oracle/model.py against the reference's own tf_efficientnet_b0 train steps, at the tolerances of
-    test_oracle_vs_reference_goldens.py / test_head_multiclass_cpu.py"""
-    rec = json.load(open(os.path.join(golden_dir, case + ".json")))
-    torch.set_num_threads(8)
-    spec = get_spec(rec["arch"], num_classes=rec["num_classes"])
-    sd = synth_state(spec, seed=rec["weight_seed"])
-    opt = OT.OptState(kind=rec["opt"], lr=rec["lr"], momentum=rec["momentum"], weight_decay=rec["weight_decay"], eps=1e-8)
-    for i, st in enumerate(rec["steps"]):
-        x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=1234 + i)
-        out = OT.train_step(spec, sd, x, y, opt)
-        _check_summ(out["logits"], st["logits"], "logits step %d" % i, rtol=1e-3)
-        assert float(out["loss"]) == pytest.approx(st["loss"], rel=1e-4)
-        assert float(out["prec1"]) == pytest.approx(st["prec1"], abs=1e-3)
-        rt = RTOL * (1 if i == 0 else 25)
-        gfloor = 1e-5 * max(v["norm"] / max(out["grads"][k].numel(), 1) ** 0.5 for k, v in st["grads"].items())
-        for k, s in st["grads"].items():
-            _check_summ(out["grads"][k], s, "grad %s step %d" % (k, i), rt, floor=gfloor)
-        for k, s in st["params"].items():
-            _check_summ(sd[k], s, "param %s step %d" % (k, i), rt)
-        for k, s in st["buffers"].items():
-            _check_summ(sd[k].float(), s, "buffer %s step %d" % (k, i), rt)
-    x, y = synth_batch(rec["batch"], 3, rec["H"], rec["W"], seed=999)
-    ev = OT.validate_step(spec, sd, x, y)
-    _check_summ(ev["logits"], rec["eval"]["logits"], "eval logits", rtol=5e-3)
 
 
 def test_oracle_eval_logits_match_reference(golden_dir):

@@ -63,33 +63,19 @@ def test_symmetric_pads_equal_the_symmetric_entry_points(H, W, C, k, dtype):
 
 
 # ---- whole steps --------------------------------------------------------------------------------------------------------
-def _trainer(arch, batch, H, W, dtype, sd):
-    from deepfake_detection_b200.trainer import Trainer
-    tr = Trainer(arch, batch, H, W, dtype=dtype, opt="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4, bn_eps=1e-3)
-    tr.engine.load_state_dict(sd)
-    return tr
-
-
 def _relerr(a, b):
     a, b = a.double().flatten().cpu(), b.double().flatten().cpu()
     return float((a - b).norm() / (b.norm() + 1e-30))
 
 
 def _run_steps(arch, batch, H, W, dtype, steps):
+    """graph-captured Trainer steps from the synthetic weights at BatchNorm eps 1e-3; fp16 with dynamic loss scaling"""
     from deepfake_detection_b200.arch import get_spec
-    from oracle.weights import synth_batch, synth_state
+    from engine_checks import trainer_steps
+    from oracle.weights import synth_state
     spec = get_spec(arch)
     sd0 = synth_state(spec, seed=7)
-    tr = _trainer(arch, batch, H, W, dtype, sd0)
-    out = []
-    for i in range(steps):
-        x, y = synth_batch(batch, 3, H, W, seed=1234 + i)
-        e = tr.engine
-        scale = float(e.loss_scale_state[0])        # fp16: the gradient arena holds loss-scaled gradients (1 in bf16)
-        loss, _ = tr.train_step(x.cuda(), y.cuda())
-        torch.cuda.synchronize()
-        out.append(dict(loss=float(loss), logits=e.logits.detach().cpu().clone(), scale=scale,
-                        grads=e.grads32.detach().cpu().clone(), params=e.params32.detach().cpu().clone()))
+    tr, out = trainer_steps(arch, batch, H, W, dtype, steps, sd0, loss_scale=None, bn_eps=1e-3)
     assert tr.use_graph and tr.n_captures >= 1
     return spec, sd0, tr, out
 
@@ -116,7 +102,7 @@ def test_tf_b0_captured_steps_match_oracle_and_reference(H, W, dtype, golden_dir
         emul_loss.append(float(o["loss"]))
         # tests/test_engine_gpu.py's step tolerances for B0 (fp16 per step; bf16 as its emulation bound). Batch 4 is a chaotic
         # regime for bf16 storage after the first update (the oracle's own bf16 emulation moves the step-1 logits by tens of
-        # percent): there bf16 step 1 is held to the loss only, as tests/test_engine_gpu.py does with its batch-4 fixture
+        # percent): there bf16 step 1 is held to the loss only, as tests/test_reference_steps_gpu.py holds batch-4 fixtures
         lrel = _relerr(r["logits"], o["logits"])
         if dtype == "fp16" or i == 0:
             assert lrel < (2e-2 if dtype == "fp16" else 6e-2) * (1 + i), (i, lrel)
@@ -131,8 +117,9 @@ def test_tf_b0_captured_steps_match_oracle_and_reference(H, W, dtype, golden_dir
             go, g32 = (torch.cat([oo["grads"][n].flatten() for n in names]) for oo in (o, o32))
             yard = _relerr(go, g32)
             assert _relerr(gn, g32) < 1.5 * yard + 3e-2, (_relerr(gn, g32), yard)
-    # the reference's own fp32 steps (fixture): step 0 tightly, step 1 on the loss (tests/test_engine_gpu.py::test_golden_b0),
-    # each widened by the distance of the oracle's 16-bit emulation from the fixture (the rounding any 16-bit path pays)
+    # the reference's own fp32 steps (fixture): step 0 tightly, step 1 on the loss (the "engine" runs of
+    # tests/test_reference_steps_gpu.py), each widened by the distance of the oracle's 16-bit emulation from the fixture (the
+    # rounding any 16-bit path pays)
     rec = json.load(open(os.path.join(golden_dir, "step_tf_efficientnet_b0_%dx%d.json" % (H, W))))
     for i, (r, st) in enumerate(zip(runs, rec["steps"])):
         yard = abs(emul_loss[i] - st["loss"])

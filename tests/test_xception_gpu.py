@@ -3,14 +3,13 @@
   * the depthwise forward with a ReLU input (after a BN or alone) and the fused depthwise backward in its two ReLU modes
     against fp64 torch at Xception's shapes; the strided block tail (dfd_bn_maxpool_add) and its backward
     (dfd_maxpool_bn_bwd_reduce) against F.max_pool2d and its indices, with negative inputs and forced ties;
-  * whole train steps against the oracle (oracle/model.py) and the reference's fixture; batch 32 at 299x299 from the
-    reference init against the fp32 oracle; eval at batch 1 in fp16 (the test_img path);
+  * batch 32 at 299x299 from the reference init against the fp32 oracle; eval at batch 1 in fp16 (the test_img path);
   * drop_rate changes no bit; checkpoints round-trip bit for bit and two engines agree bit for bit; the runner's train_epoch
     with SGD and RMSpropTF and an EMA update.
 No test here reads the reference tree: the fixtures under tests/golden/ came from tools/mint_xception_goldens.py.
+Their train steps are held by tests/test_reference_steps_gpu.py.
 """
 import io
-import json
 import os
 from types import SimpleNamespace
 
@@ -186,61 +185,6 @@ def test_act_bwd_gpool_relu(dtype):
         assert _rel(s1.view(S, C).sum(0), gu.double().sum((0, 1))) < 1e-5
 
 
-# ---- whole steps --------------------------------------------------------------------------------------------------------
-def _trainer_steps(batch, H, W, dtype, steps, sd0, drop_rate=0.0, opt="sgd"):
-    from deepfake_detection_b200.trainer import Trainer
-    from oracle.weights import synth_batch
-    tr = Trainer("xception", batch, H, W, dtype=dtype, opt=opt, lr=0.01, momentum=0.9, weight_decay=1e-4, loss_scale=1.0,
-                 drop_rate=drop_rate)
-    tr.engine.load_state_dict(sd0)
-    out = []
-    for i in range(steps):
-        x, y = synth_batch(batch, 3, H, W, seed=1234 + i)
-        e = tr.engine
-        loss, _ = tr.train_step(x.cuda(), y.cuda())
-        torch.cuda.synchronize()
-        out.append(dict(loss=float(loss), logits=e.logits.detach().cpu().clone(), grads=e.grads32.detach().cpu().clone(),
-                        params=e.params32.detach().cpu().clone()))
-    return tr, out
-
-
-@pytest.mark.parametrize("dtype", ["bf16", "fp16"])
-def test_steps_match_oracle_and_reference(dtype, golden_dir):
-    """the tamed fixture (batch 8, 64x80) with tests/test_resnet_family_gpu.py's statements: step 0 logits and loss against the
-    oracle's 16-bit emulation, logits and gradients against the fp32 oracle within 1.5 x the emulation's own distance + a
-    margin, every step's loss against the reference, the step-0 logits against the reference's samples"""
-    from deepfake_detection_b200.arch import get_spec, param_entries
-    from oracle import train as OT
-    from oracle.weights import synth_batch, synth_state, tame_state
-    rec = json.load(open(os.path.join(golden_dir, "step_xception_tame_64x80.json")))
-    batch, H, W = rec["batch"], rec["H"], rec["W"]
-    spec = get_spec("xception")
-    sd0 = tame_state(spec, synth_state(spec, seed=rec["weight_seed"]), rec["tame"])
-    tr, runs = _trainer_steps(batch, H, W, dtype, len(rec["steps"]), sd0)
-    e = tr.engine
-    sd = {k: v.clone() for k, v in sd0.items()}
-    ost = OT.OptState(kind="sgd", lr=0.01, momentum=0.9, weight_decay=1e-4)
-    for i, (r, st) in enumerate(zip(runs, rec["steps"])):
-        x, y = synth_batch(batch, 3, H, W, seed=1234 + i)
-        o = OT.train_step(spec, sd, x, y, ost, act_dtype=TDT[dtype])
-        if i == 0:
-            o32 = OT.train_step(spec, {k: v.clone() for k, v in sd0.items()}, x, y, None)
-            yard_logits = _rel(o["logits"], o32["logits"])
-            assert _rel(r["logits"], o["logits"]) < max(2e-2 if dtype == "fp16" else 6e-2, 1.5 * yard_logits)
-            assert abs(r["loss"] - float(o["loss"])) < 5e-3, (r["loss"], float(o["loss"]))
-            assert _rel(r["logits"], o32["logits"]) < 1.5 * yard_logits + 1e-2, (_rel(r["logits"], o32["logits"]), yard_logits)
-            names = [n for n, _, _ in param_entries(spec)]
-            gn = torch.cat([r["grads"][e.p_off[n][0]:e.p_off[n][0] + e.p_off[n][2]] for n in names])
-            go, g32 = (torch.cat([oo["grads"][n].flatten() for n in names]) for oo in (o, o32))
-            yard = _rel(go, g32)
-            assert _rel(gn, g32) < 1.5 * yard + 3e-2, (_rel(gn, g32), yard)
-            f = r["logits"].double().flatten()
-            ref = torch.tensor(st["logits"]["samples"], dtype=torch.float64)
-            got = f[torch.tensor(st["logits"]["idx"])]
-            assert float((got - ref).norm() / ref.norm()) < 1.5 * yard_logits + 2e-2, (got, ref)
-        assert abs(r["loss"] - st["loss"]) < (1e-2 if i == 0 else 5e-2) * abs(st["loss"]), (i, r["loss"], st["loss"])
-
-
 @pytest.mark.parametrize("dtype", ["bf16", "fp16"])
 def test_batch32_299_reference_init(dtype):
     """loss and updated weights within 1e-2 of the fp32 oracle from the reference's initialisers (batch 32, 299x299)"""
@@ -306,19 +250,21 @@ def test_eval_batch1_fp16_299():
 
 def test_drop_rate_changes_nothing():
     from deepfake_detection_b200.arch import get_spec
+    from engine_checks import trainer_steps
     from oracle.weights import synth_state
     sd0 = synth_state(get_spec("xception"), seed=7)
-    a = _trainer_steps(4, 64, 80, "bf16", 2, sd0)[1]
-    b = _trainer_steps(4, 64, 80, "bf16", 2, sd0, drop_rate=0.5)[1]
+    a = trainer_steps("xception", 4, 64, 80, "bf16", 2, sd0)[1]
+    b = trainer_steps("xception", 4, 64, 80, "bf16", 2, sd0, drop_rate=0.5)[1]
     for ra, rb in zip(a, b):
         assert ra["loss"] == rb["loss"] and torch.equal(ra["logits"], rb["logits"]) and torch.equal(ra["params"], rb["params"])
 
 
 def test_two_engines_agree_bit_for_bit():
     from deepfake_detection_b200.arch import get_spec
+    from engine_checks import trainer_steps
     from oracle.weights import synth_state
     sd0 = synth_state(get_spec("xception"), seed=7)
-    runs = [_trainer_steps(8, 96, 96, "bf16", 2, sd0)[1] for _ in range(2)]
+    runs = [trainer_steps("xception", 8, 96, 96, "bf16", 2, sd0)[1] for _ in range(2)]
     for a, b in zip(*runs):
         assert a["loss"] == b["loss"]
         assert torch.equal(a["logits"], b["logits"]) and torch.equal(a["grads"], b["grads"]) and torch.equal(a["params"], b["params"])

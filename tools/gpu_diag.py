@@ -97,7 +97,6 @@ def main():
         run("engine_b0_fp16_%s" % a.gemm, EC.run_parity, "efficientnet_b0", 16, 96, 96, dtype="fp16", gemm_impl=a.gemm, verbose=True)
         run("engine_b0_bf16_%s" % a.gemm, EC.run_parity, "efficientnet_b0", 16, 96, 96, dtype="bf16", gemm_impl=a.gemm)
         run("engine_b4_fp16_%s" % a.gemm, EC.run_parity, "efficientnet_b4", 4, 76, 76, dtype="fp16", gemm_impl=a.gemm)
-        run("golden_b0_%s" % a.gemm, EC.golden_compare, "step_efficientnet_b0", os.path.join(ROOT, "tests", "golden"), gemm_impl=a.gemm)
     ok = sum(1 for v in results.values() if v["ok"])
     print("DIAG DONE: %d/%d checks ran without exception" % (ok, len(results)))
 
